@@ -36,30 +36,13 @@
 
 #include "conv.h"
 #include "conv_pers.cuh"
+#include "exact_dot.cuh"
+#include "label_count.h"
 
 namespace dirb {
 namespace {
 
 constexpr int SEL_THREADS = 512;
-
-// Exact score of one (query, row) pair by one warp: fp64 accumulation of the fp32 products, fixed summation order
-// (lane-strided float4 loads, xor-shuffle tree).  Every exact score of the library comes from this function, so two
-// evaluations of the same pair - or of two identical rows - are bit-identical wherever they are computed.
-__device__ __forceinline__ double exact_dot_warp(const float* __restrict__ qrow, const float* __restrict__ dbrow, int D,
-                                                 int lane) {
-  const float4* a = reinterpret_cast<const float4*>(qrow);
-  const float4* b = reinterpret_cast<const float4*>(dbrow);
-  double acc = 0.0;
-  for (int i = lane; i < D / 4; i += 32) {
-    const float4 x = __ldg(a + i), y = __ldg(b + i);
-    acc += static_cast<double>(x.x) * y.x;
-    acc += static_cast<double>(x.y) * y.y;
-    acc += static_cast<double>(x.z) * y.z;
-    acc += static_cast<double>(x.w) * y.w;
-  }
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  return acc;
-}
 
 __device__ __forceinline__ uint32_t f2key(float f) {  // monotone increasing map float -> uint32
   const uint32_t u = __float_as_uint(f);
@@ -783,6 +766,8 @@ struct dirb200_index {
   int64_t sample_rows = 0;
   int cand_cap = 0;          // 0 = auto
   int count_cap = 0;         // candidate capacity per query of dirb200_index_rank_count (0 = 32768)
+  double count_eps = 0;      // dirb200_index_count_ge: absolute score-error bound (0 = derived from the norms per call)
+  int band_cap = 0;          // dirb200_index_count_ge: band-list capacity (0 = 1 << 20 entries)
   int retries = 1;           // gated retry passes enqueued after the first filter pass (device-side predicate)
   int deferred = 0;          // 1 = search calls never synchronise; the caller collects the status (dirb200_index_check)
   // workspaces (grown on demand)
@@ -898,6 +883,8 @@ int dirb200_index_set_option(dirb200_index* h, const char* key, double value) {
   else if (k == "cand_cap") h->cand_cap = static_cast<int>(value);
   else if (k == "profile") h->profile = value != 0;
   else if (k == "count_cap") h->count_cap = static_cast<int>(value);
+  else if (k == "count_eps") h->count_eps = std::max(0.0, value);
+  else if (k == "band_cap") h->band_cap = std::max(0, static_cast<int>(value));
   else if (k == "retries") h->retries = std::max(0, std::min(4, static_cast<int>(value)));
   else if (k == "deferred_check") h->deferred = value != 0;
   else DIRB_REQUIRE(false, DIRB200_EKEY, "unknown index option '%s'", key);
@@ -1332,6 +1319,44 @@ int dirb200_index_rank_count(dirb200_index* h, const float* q32, int Q, const in
   }
   h->stats[1] = cand_total;
   h->stats[3] = static_cast<int64_t>(list.size());
+  h->stats[4] = launches_total() - launches0;
+  return 0;
+}
+
+// ---- threshold counts for label-based AP (kernels: label_count.cu)
+int dirb200_index_count_ge(dirb200_index* h, const float* q32, int Q, const int* thr_off_dev, const float* thr_dev, int T,
+                           const int64_t* skip_row_dev, int64_t* count_dev, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DIRB_REQUIRE(h && Q >= 0 && T >= 0, DIRB200_EINVAL, "bad arguments");
+  DIRB_REQUIRE(h->has_db, DIRB200_ESTATE, "index has no database attached");
+  DIRB_REQUIRE(Q <= 65535 * 64, DIRB200_ENOTSUP, "count_ge takes at most %d queries per call (got %d)", 65535 * 64, Q);
+  h->stats[0] = h->stats[1] = h->stats[2] = h->stats[3] = h->stats[4] = 0;
+  if (Q == 0 || T == 0) return 0;
+  DIRB_REQUIRE(q32 && thr_off_dev && thr_dev && count_dev, DIRB200_EINVAL, "null argument");
+  DIRB_CUDA(cudaSetDevice(h->device));
+  DIRB_TRY(dirb200_index_check(h));
+  h->pend.active = false;                        // shares the search workspace
+  const int64_t launches0 = launches_total();
+  const int cap = h->band_cap > 0 ? h->band_cap : (1 << 20);
+  const size_t need = count_ge_ws_bytes(Q, T, cap);
+  if (need > h->ws_bytes) {
+    if (h->ws) DIRB_CUDA(cudaFree(h->ws));
+    h->ws = nullptr;
+    h->ws_bytes = 0;
+    DIRB_CUDA(cudaMalloc(&h->ws, need));
+    h->ws_bytes = need;
+    h->tmaps.es.clear();
+  }
+  CountGeArgs a;
+  a.q32 = q32; a.Q = Q;
+  a.db32 = h->db32; a.N = h->N; a.offset = h->offset; a.D = h->dim;
+  a.thr_off = thr_off_dev; a.thr = thr_dev; a.T = T;
+  a.skip_row = skip_row_dev; a.count = count_dev;
+  a.eps = h->count_eps; a.band_cap = cap;
+  CountGeStats st;
+  DIRB_TRY(count_ge_run(a, h->ws, &st, stream));
+  h->stats[1] = st.band;
+  h->stats[3] = st.fallback;
   h->stats[4] = launches_total() - launches0;
   return 0;
 }

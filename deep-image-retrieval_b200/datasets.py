@@ -151,6 +151,54 @@ class ImageListLabels(Dataset):
         correct = np.array([lab == qlabel for lab in self.labels], dtype=bool)[np.argsort(-np.asarray(scores))]
         return {k_: float(correct[:k_].any()) for k_ in k if k_ < len(correct)}
 
+    # ---- the same AP / top-k from threshold counts (dirb200_index_count_ge) and a ranked prefix, no score row
+    def _class_ids(self):
+        """(class id of every database row, class id of every query); -1 for a query label absent from the database."""
+        if getattr(self, "_ids", None) is None:
+            qdb = self.get_query_db()
+            db_ids = np.array([self.cls_idx[l] for l in self.labels], dtype=np.int64)
+            present = set(self.labels)
+            q_ids = np.array([self.cls_idx[l] if l in present else -1 for l in qdb.labels], dtype=np.int64)
+            self._ids = (db_ids, q_ids)
+        return self._ids
+
+    def label_targets(self, queries=None):
+        """Positives of the given queries (default: all), built at once and grouped by class: database rows with the
+        query's label, the query's own row excluded when the queries are the database (get_query_groundtruth marks it
+        0).  -> (t_off int64 (Q+1,), t_rows int64 (T,) ascending within each query, skip_row int64 (Q,), -1 = none)."""
+        db_ids, q_ids = self._class_ids()
+        queries = np.arange(len(q_ids), dtype=np.int64) if queries is None else np.asarray(queries, dtype=np.int64)
+        qc = q_ids[queries]
+        by_class = np.argsort(db_ids, kind="stable")                       # rows grouped by class, ascending inside
+        nclass = int(max(db_ids.max(initial=-1), q_ids.max(initial=-1))) + 1
+        size = np.bincount(db_ids, minlength=nclass)
+        start = np.concatenate([[0], np.cumsum(size)[:-1]])
+        n = np.where(qc >= 0, size[np.maximum(qc, 0)], 0)
+        first = np.where(qc >= 0, start[np.maximum(qc, 0)], 0)
+        off = np.concatenate([[0], np.cumsum(n)])
+        pos = np.arange(off[-1], dtype=np.int64) - np.repeat(off[:-1] - first, n)
+        rows = by_class[pos]
+        skip = queries.copy() if self.get_query_db() is self else -np.ones(len(queries), dtype=np.int64)
+        keep = rows != np.repeat(skip, n)
+        n = n - (skip >= 0)                                  # a self-query's own row is always in its class
+        return np.concatenate([[0], np.cumsum(n)]).astype(np.int64), rows[keep].astype(np.int64), skip
+
+    def eval_query_AP_from_ge_counts(self, query_idx, thr, counts):
+        """AP of `eval_query_AP` from the fp32 scores of the query's positives in descending order (thr) and, for each,
+        the number of rows other than the query's own with a score >= it (counts, dirb200_index_count_ge):
+        AP = (1/|P|) sum_t TP_t / c_t, TP_t = positives scoring >= thr[t] (tied positives share TP and c)."""
+        thr = np.asarray(thr, dtype=np.float32)
+        if thr.shape[0] == 0:
+            return -1                                            # no relevant image: excluded from the mean
+        tp = np.searchsorted(-thr, -thr, side="right")
+        return float(np.sum(tp / np.asarray(counts, dtype=np.float64)) / thr.shape[0])
+
+    def eval_query_top_from_ranking(self, query_idx, ranked_idx, k=(1, 5, 10, 20, 50, 100)):
+        """`eval_query_top` from the database indices of the best-ranked rows (at least min(max(k), N - 1) of them)."""
+        db_ids, q_ids = self._class_ids()
+        correct = db_ids[np.asarray(ranked_idx, dtype=np.int64)] == q_ids[query_idx]
+        return {k_: float(correct[:k_].any()) for k_ in k if k_ < self.nimg}
+
 
 class ImageListLabelsQ(ImageListLabels):
     """Labelled database + a separate labelled query list (generic.py:80-105)."""

@@ -32,6 +32,12 @@ def shard_quota(k: int, shard_sizes) -> int:
     return min(c, int(k))
 
 
+def sort_thresholds(s: torch.Tensor, t_q: torch.Tensor) -> torch.Tensor:
+    """Values s grouped by query (t_q non-decreasing) -> the same groups, each sorted in descending order."""
+    order = torch.sort(s, descending=True, stable=True).indices
+    return s[order][torch.sort(t_q[order], stable=True).indices]
+
+
 def all_gather_packed(packed: torch.Tensor, group=None) -> torch.Tensor:
     """packed (2,Q,k) int64 per rank -> (G,2,Q,k); a single collective."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
@@ -167,6 +173,24 @@ class ShardedIndex:
         if multi:
             dist.all_reduce(above, op=dist.ReduceOp.SUM, group=self.group)
         return sc, above
+
+    def count_ge(self, q32: torch.Tensor, t_off, t_rows, skip_row=None):
+        """Label AP counts over the WHOLE sharded database.  t_off int32 (Q+1,) / t_rows int64 (T,) CUDA tensors: the
+        positives of each query (global indices).  Each shard scores the positives it owns (one SUM all-reduce of T
+        doubles); the fp32 roundings, sorted descending within each query, are the thresholds; each shard counts its
+        own rows reaching them (one SUM all-reduce of T int64).  Returns (thresholds fp32 (T,), counts int64 (T,)) in
+        the sorted order, CUDA tensors."""
+        t_q = torch.repeat_interleave(torch.arange(q32.shape[0], dtype=torch.int32, device=q32.device),
+                                      (t_off[1:] - t_off[:-1]).long())
+        multi = dist.is_initialized() and dist.get_world_size(self.group) > 1
+        sc = self.local.target_scores(q32, t_q, t_rows)
+        if multi:
+            dist.all_reduce(sc, op=dist.ReduceOp.SUM, group=self.group)      # exactly one shard contributes a non-zero
+        thr = sort_thresholds(sc.float(), t_q)
+        count = self.local.count_ge(q32, t_off, thr, skip_row)
+        if multi:
+            dist.all_reduce(count, op=dist.ReduceOp.SUM, group=self.group)
+        return thr, count
 
     def expand_queries(self, q32: torch.Tensor, k: int, alpha: float, check: bool = True):
         """alpha-QE (test_dir.py:24-44) over the sharded database: global top-k, each rank sums the neighbours it

@@ -78,6 +78,7 @@ SIGNATURES = {
     "dirb200_index_last_profile": (i32, [p, C.POINTER(f64)]),
     "dirb200_index_target_scores": (i32, [p, p, i32, p, p, i32, p, p]),
     "dirb200_index_rank_count": (i32, [p, p, i32, p, p, p, p, p, i32, p, p]),
+    "dirb200_index_count_ge": (i32, [p, p, i32, p, p, i32, p, p, p]),
     "dirb200_index_destroy": (i32, [p]),
     "dirb200_topk_merge": (i32, [p, p, i32, i32, i32, i64, p, p, p]),
     "dirb200_exchange_create": (i32, [i32, i32, i32, i32, i32, C.POINTER(p)]),

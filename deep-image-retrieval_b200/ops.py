@@ -430,6 +430,24 @@ class Index:
         sc = self.target_scores(q32, t_q, rows)
         return sc, self.rank_count(q32, off, rows, flags, sc)
 
+    def count_ge(self, q32, thr_off, thr, skip_row=None):
+        """count[t] = number of rows of this shard (global index != skip_row[q]) whose fp32-rounded exact score with
+        query q reaches thr[t], for the thresholds thr[thr_off[q]:thr_off[q+1]] of each query (descending) - what
+        label AP needs (datasets.ImageListLabels.eval_query_AP_from_ge_counts).  thr_off int32 (Q+1,), thr fp32 (T,),
+        skip_row int64 (Q,) or None: CUDA tensors.  Afterwards stats()["candidates"] = pairs re-scored exactly
+        (within eps of a boundary) and stats()["retries"] = queries counted exactly over all rows (band overflow)."""
+        _chk(q32, torch.float32, "q32")
+        _chk(thr_off, torch.int32, "thr_off")
+        _chk(thr, torch.float32, "thr")
+        if skip_row is not None:
+            _chk(skip_row, torch.int64, "skip_row")
+            assert skip_row.shape[0] == q32.shape[0]
+        assert thr_off.shape[0] == q32.shape[0] + 1
+        count = torch.zeros(thr.shape[0], dtype=torch.int64, device=q32.device)
+        lib.call("dirb200_index_count_ge", self._h, _ptr(q32), q32.shape[0], _ptr(thr_off), _ptr(thr), thr.shape[0],
+                 _ptr(skip_row), _ptr(count), _stream())
+        return count
+
     def check(self):
         """Collect the status of the last search (option deferred_check): raises DirbError on an unresolved overflow."""
         lib.call("dirb200_index_check", self._h)

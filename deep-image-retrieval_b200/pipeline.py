@@ -219,12 +219,46 @@ def _aps_from_counts(db, qdescs, bdescs):
             for q in range(qd.shape[0])]
 
 
+def _aps_from_label_counts(db, qdescs, bdescs, max_thresholds=1 << 26, q_block=4096):
+    """Per-query label AP and top-k without the Q x N score matrix (label datasets, dataset.py:83-101).  AP: the fp32
+    exact scores of each query's positives are the thresholds, dirb200_index_count_ge counts the rows reaching each
+    one, datasets.eval_query_AP_from_ge_counts turns that into sklearn's AP.  Top-k: the exact top-100 of
+    dirb200_index_search.  Queries go through in blocks of at most ~max_thresholds thresholds (a class of c images
+    gives c^2 of them).  -> (aps, tops)."""
+    from .dist import ShardedIndex
+    dim = qdescs.shape[1]
+    pad = (-dim) % 64
+    f = lambda a: torch.nn.functional.pad(_dev_f32(a), (0, pad)).contiguous() if pad else _dev_f32(a)
+    qd, bd = f(qdescs), f(bdescs)
+    nq, n, dev = qd.shape[0], bd.shape[0], qd.device
+    index = ShardedIndex(bd, 0)
+    t_off, t_rows, skip = db.label_targets()
+    aps, q0 = [], 0
+    while q0 < nq:
+        q1 = int(np.searchsorted(t_off, t_off[q0] + max_thresholds, side="right")) - 1
+        q1 = min(max(q1, q0 + 1), nq)
+        lo, hi = int(t_off[q0]), int(t_off[q1])
+        off = t_off[q0:q1 + 1] - lo
+        thr, cnt = index.count_ge(qd[q0:q1], torch.from_numpy(off.astype(np.int32)).to(dev),
+                                  torch.from_numpy(t_rows[lo:hi]).to(dev), torch.from_numpy(skip[q0:q1]).to(dev))
+        thr, cnt = thr.cpu().numpy(), cnt.cpu().numpy()
+        aps += [db.eval_query_AP_from_ge_counts(q0 + i, thr[off[i]:off[i + 1]], cnt[off[i]:off[i + 1]]) for i in range(q1 - q0)]
+        q0 = q1
+    tops, k = [], min(100, n)
+    for c0 in range(0, nq, q_block):
+        _, idx = index.search(qd[c0:c0 + q_block].contiguous(), k)
+        idx = idx.cpu().numpy()
+        tops += [db.eval_query_top_from_ranking(c0 + i, idx[i]) for i in range(idx.shape[0])]
+    return aps, tops
+
+
 def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=None, aqe=None, adba=None, threads=8,
                batch_size=16, save_feats=None, load_feats=None, dbg=(), rank_topk=0, dense_scores=False):
     """Evaluate a network on a retrieval dataset (test_dir.py:97-180).  aqe / adba: dict(k=..., alpha=...).
-    Ranking: datasets with relevance lists (Oxford/Paris style) are graded from GPU rank counts - no Q x N score
-    matrix, no host argsort; dense_scores=True (extension) forces the literal matmul + per-query sort of the
-    reference, which label datasets always use; rank_topk > 0 (extension) grades from the exact top-k lists."""
+    Ranking: datasets with relevance lists (Oxford/Paris style) are graded from GPU rank counts and label datasets
+    from GPU threshold counts + the exact top-100 - no Q x N score matrix, no host argsort; dense_scores=True
+    (extension) forces the literal matmul + per-query sort of the reference; rank_topk > 0 (extension) grades
+    relevance-list datasets from the exact top-k lists."""
     print("\n>> Evaluation...")
     query_db = db.get_query_db()
     bdescs, qdescs = [], []
@@ -261,6 +295,7 @@ def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=Non
     if aqe is not None:
         qdescs = expand_descriptors(qdescs, db=bdescs, to_numpy=False, **aqe)
     res = {}
+    tops = None
     qn, bn = _dev_f32(qdescs), _dev_f32(bdescs)
     unit = bool(float((qn.norm(dim=1) - 1).abs().max()) < 1e-3 and float((bn.norm(dim=1) - 1).abs().max()) < 1e-3)
     if rank_topk and hasattr(db, "eval_query_AP_from_ranking"):
@@ -272,6 +307,10 @@ def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=Non
         # default for relevance-list datasets: exact rank counts of the labelled rows from one tensor-core pass
         # (the error bound of the fp16 pass assumes unit-norm rows, which pooling / whitening / QE all produce)
         aps = _aps_from_counts(db, qn, bn)
+        scores = None
+    elif not dense_scores and unit and hasattr(db, "eval_query_AP_from_ge_counts"):
+        # label datasets: threshold counts on fp64 tensor cores (same unit-norm condition: the top-k search needs it)
+        aps, tops = _aps_from_label_counts(db, qn, bn)
         scores = None
     else:
         scores = matmul(qn, bn)
@@ -294,9 +333,10 @@ def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=Non
     except NotImplementedError:
         print(" AP not implemented!")
     try:
-        if scores is None:
-            raise NotImplementedError()
-        tops = [db.eval_query_top(q, s) for q, s in enumerate(tqdm.tqdm(scores, desc="top1"))]
+        if tops is None:
+            if scores is None:
+                raise NotImplementedError()
+            tops = [db.eval_query_top(q, s) for q, s in enumerate(tqdm.tqdm(scores, desc="top1"))]
         if detailed:
             res["tops"] = tops
         for k in tops[0]:

@@ -195,7 +195,8 @@ int dirb200_index_set_db(dirb200_index* idx, const float* db32_dev, const void* 
  * candidate-list capacity (0 = auto; a small value forces the overflow -> tightened re-run path); "retries": gated
  * retry passes enqueued after the filter pass (default 1; they return at once unless a list overflowed);
  * "deferred_check" = 1: search calls never synchronise the host, the caller collects the status with
- * dirb200_index_check (it is also collected at the start of the next search); "profile". */
+ * dirb200_index_check (it is also collected at the start of the next search); "profile"; "count_eps" / "band_cap":
+ * see dirb200_index_count_ge. */
 int dirb200_index_set_option(dirb200_index* idx, const char* key, double value);
 /* q32_dev [Q][dim] fp32.  Outputs (device): scores_dev [Q][k] fp64 exact scores, idx_dev [Q][k] int64.
  * If N < k the tail is filled with score -inf / index -1.  Everything is enqueued on `stream`; the call then waits
@@ -246,6 +247,20 @@ int dirb200_index_target_scores(dirb200_index* idx, const float* q32_dev, int Q,
 int dirb200_index_rank_count(dirb200_index* idx, const float* q32_dev, int Q, const int* t_off_host, const int* t_off_dev,
                              const int64_t* t_rows_dev, const unsigned char* t_flags_dev, const double* t_score_dev,
                              int T, int64_t* above_dev, void* stream);
+
+/* Threshold counts for label-based AP without the Q x N score matrix (replaces sklearn's average_precision_score over
+ * a full score row, dataset.py:83-92 / evaluation.py:41-43, and the full argsort of the top-k, dataset.py:94-101).
+ * Thresholds of each query, grouped by query: thr_off_dev[Q+1] (CSR from 0 to T), thr_dev[T] fp32 in DESCENDING order
+ * within each query (typically s_t = fp32 rounding of the exact scores of its positives, dirb200_index_target_scores).
+ *   count_dev[t] = number of rows r OF THIS SHARD, global index r + offset != skip_row_dev[q] (-1 or a null pointer:
+ *                  no row skipped), with fp32(exact score <q, row r>) >= thr[t].  Several shards: SUM all-reduce.
+ * One fp64 tensor-core pass; pairs within eps of a rounding boundary are re-scored exactly (last_stats[1] = their
+ * number), and a query whose pairs overflow the band list (option "band_cap", default 2^20 entries) is counted exactly
+ * over all rows (last_stats[3] = number of such queries).  eps = 4 gamma_D |q| max|row| from the norms of the call,
+ * or option "count_eps" (> 0) as an absolute override.  Synchronises the stream; DIRB200_EINVAL for malformed offsets
+ * or thresholds that are not finite and descending. */
+int dirb200_index_count_ge(dirb200_index* idx, const float* q32_dev, int Q, const int* thr_off_dev, const float* thr_dev,
+                           int T, const int64_t* skip_row_dev, int64_t* count_dev, void* stream);
 
 /* Merge G per-shard top-k lists (scores fp64 + global indices int64, as produced by an all-gather of
  * dirb200_index_search outputs: each list ordered best first, empty slots = index -1 at the tail, no row in two
