@@ -53,6 +53,17 @@ static int g_conv_halo = 1;
 void set_conv_halo(int on) { g_conv_halo = on; }
 int get_conv_halo() { return g_conv_halo; }
 
+// Ragged batch: the epilogue zeroes every output pixel outside its image's extent (conv_pers.cuh).
+static void set_ext(ConvPersParams& p, const ConvExt* ext, int out_h, int out_w) {
+  if (ext == nullptr) return;
+  p.ext = ext->hw;
+  p.kc_major = ext->kc_major;
+  p.ext_ld = ext->ld;
+  p.ext_n = ext->n;
+  p.out_h = out_h;
+  p.out_w = out_w;
+}
+
 // Ring depth: as many 128 x 64 + BN x 64 operand slots as fit next to the convolution's staging buffers.
 template <int BN>
 struct PersStages {
@@ -62,7 +73,8 @@ struct PersStages {
 
 template <int BN>
 static int conv_pers_bn(const ConvShape& s, const __half* in, const __half* w, const float* scale, const float* shift,
-                        const __half* res, int relu, __half* out, cudaStream_t stream, int grid_limit) {
+                        const __half* res, int relu, __half* out, cudaStream_t stream, int grid_limit,
+                        const ConvExt* ext) {
   const int Ho = s.Ho(), Wo = s.Wo();
   const int Ktot = s.KH * s.KW * s.Cin;
   ConvPersParams p{};
@@ -76,6 +88,7 @@ static int conv_pers_bn(const ConvShape& s, const __half* in, const __half* w, c
   p.relu = relu;
   p.scale = scale;
   p.shift = shift;
+  set_ext(p, ext, Ho, Wo);
   CUtensorMap tmA, tmB, tmR, tmO;
   int64_t m_tiles;
   const bool flat = (s.KH == 1 && s.KW == 1 && s.stride == 1 && s.pad == 0);
@@ -89,7 +102,11 @@ static int conv_pers_bn(const ConvShape& s, const __half* in, const __half* w, c
     if (res) DIRB_TRY(encode_tmap_2d(&tmR, res, s.Cout, M, (uint64_t)s.Cout * 2, 64, 128));
   } else {
     p.a_spatial = 1;
-    pick_patch(s.B, Ho, Wo, &p.tw, &p.th, &p.nb);
+    if (p.kc_major != nullptr) {     // the K order is chosen per image: one image per tile
+      p.tw = 8; p.th = 16; p.nb = 1;
+    } else {
+      pick_patch(s.B, Ho, Wo, &p.tw, &p.th, &p.nb);
+    }
     p.tiles_w = (int)ceil_div(Wo, p.tw);
     p.tiles_h = (int)ceil_div(Ho, p.th);
     m_tiles = (int64_t)p.tiles_w * p.tiles_h * ceil_div(s.B, p.nb);
@@ -102,13 +119,15 @@ static int conv_pers_bn(const ConvShape& s, const __half* in, const __half* w, c
   const int64_t total = m_tiles * p.n_tiles;
   DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
   p.total_tiles = static_cast<int>(total);
+  if (p.ext != nullptr)
+    return conv_pers_launch<BN, PersStages<BN>::CONV, PERS_EPI_CONV, false, true>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
   return conv_pers_launch<BN, PersStages<BN>::CONV, PERS_EPI_CONV>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
 }
 
 // 3x3 / stride 1 / pad 1 with the input patch loaded once per 64-channel block (HALO mode of conv_pers.cuh).
 template <int BN>
 static int conv_halo_bn(const ConvShape& s, const __half* in, const __half* w, const float* scale, const float* shift,
-                        const __half* res, int relu, __half* out, cudaStream_t stream) {
+                        const __half* res, int relu, __half* out, cudaStream_t stream, const ConvExt* ext) {
   ConvPersParams p{};
   p.a_spatial = 1;
   p.taps = 9; p.kw_taps = 3;
@@ -122,6 +141,7 @@ static int conv_halo_bn(const ConvShape& s, const __half* in, const __half* w, c
   p.relu = relu;
   p.scale = scale;
   p.shift = shift;
+  set_ext(p, ext, s.H, s.W);
   const int64_t total = (int64_t)p.tiles_w * p.tiles_h * s.B * p.n_tiles;
   DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
   p.total_tiles = static_cast<int>(total);
@@ -131,6 +151,8 @@ static int conv_halo_bn(const ConvShape& s, const __half* in, const __half* w, c
   if (res) DIRB_TRY(encode_tmap_nhwc(&tmR, res, s.B, s.H, s.W, s.Cout, 8, 16, 1, 1));
   else tmR = tmO;
   DIRB_TRY(encode_tmap_2d(&tmB, w, 9 * s.Cin, s.Cout, (uint64_t)9 * s.Cin * 2, 64, BN));
+  if (p.ext != nullptr)
+    return conv_pers_launch<BN, BN == 128 ? 6 : 8, PERS_EPI_CONV, true, true>(tmA, tmB, tmR, tmO, p, num_sms(), stream);
   return conv_pers_launch<BN, BN == 128 ? 6 : 8, PERS_EPI_CONV, true>(tmA, tmB, tmR, tmO, p, num_sms(), stream);
 }
 
@@ -138,35 +160,39 @@ static int conv_halo_bn(const ConvShape& s, const __half* in, const __half* w, c
 // leaves most SMs idle (e.g. layer3 conv1 of ONE 1024x1024 image is 64 tiles of 128 channels), so the tile narrows
 // to 64 channels - the reference's default evaluation mode is batch 1 (test_dir.py:52-53,114).
 static int conv_pers_any(const ConvShape& s, const __half* in, const __half* w, const float* scale, const float* shift,
-                         const __half* res, int relu, __half* out, cudaStream_t stream, int grid_limit) {
+                         const __half* res, int relu, __half* out, cudaStream_t stream, int grid_limit,
+                         const ConvExt* ext) {
   DIRB_REQUIRE(s.Cin % 64 == 0 && s.Cout % 64 == 0, DIRB200_ENOTSUP,
                "wgmma conv needs Cin %% 64 == 0 and Cout %% 64 == 0 (got %d, %d)", s.Cin, s.Cout);
   DIRB_REQUIRE(s.stride == 1 || s.stride == 2, DIRB200_ENOTSUP, "stride %d unsupported", s.stride);
   const int64_t m_tiles = ceil_div(static_cast<int64_t>(s.B) * s.Ho() * s.Wo(), 128);
   const bool wide = s.Cout % 128 == 0 && m_tiles * (s.Cout / 128) >= num_sms();
-  if (g_conv_halo && grid_limit == num_sms() && s.KH == 3 && s.KW == 3 && s.stride == 1 && s.pad == 1 && s.H >= 16 && s.W >= 8)
-    return wide ? conv_halo_bn<128>(s, in, w, scale, shift, res, relu, out, stream)
-                : conv_halo_bn<64>(s, in, w, scale, shift, res, relu, out, stream);
+  DIRB_REQUIRE(ext == nullptr || ext->kc_major == nullptr || (s.KH == 3 && s.KW == 3 && s.stride == 1 && s.pad == 1),
+               DIRB200_EINVAL, "a per-image K order applies to 3x3 stride-1 convolutions only");
+  const bool per_image_order = ext != nullptr && ext->kc_major != nullptr;
+  if (g_conv_halo && !per_image_order && grid_limit == num_sms() && s.KH == 3 && s.KW == 3 && s.stride == 1 && s.pad == 1 && s.H >= 16 && s.W >= 8)
+    return wide ? conv_halo_bn<128>(s, in, w, scale, shift, res, relu, out, stream, ext)
+                : conv_halo_bn<64>(s, in, w, scale, shift, res, relu, out, stream, ext);
   if (wide)
-    return conv_pers_bn<128>(s, in, w, scale, shift, res, relu, out, stream, grid_limit);
-  return conv_pers_bn<64>(s, in, w, scale, shift, res, relu, out, stream, grid_limit);
+    return conv_pers_bn<128>(s, in, w, scale, shift, res, relu, out, stream, grid_limit, ext);
+  return conv_pers_bn<64>(s, in, w, scale, shift, res, relu, out, stream, grid_limit, ext);
 }
 
 int conv_tc(const ConvShape& s, const __half* in, const __half* w, const float* scale, const float* shift,
-            const __half* res, int relu, __half* out, cudaStream_t stream) {
-  return conv_pers_any(s, in, w, scale, shift, res, relu, out, stream, num_sms());
+            const __half* res, int relu, __half* out, cudaStream_t stream, const ConvExt* ext) {
+  return conv_pers_any(s, in, w, scale, shift, res, relu, out, stream, num_sms(), ext);
 }
 
 int conv_tc_np(const ConvShape& s, const __half* in, const __half* w, const float* scale, const float* shift,
-               const __half* res, int relu, __half* out, cudaStream_t stream) {
-  return conv_pers_any(s, in, w, scale, shift, res, relu, out, stream, 1 << 30);   // one tile per CTA
+               const __half* res, int relu, __half* out, cudaStream_t stream, const ConvExt* ext) {
+  return conv_pers_any(s, in, w, scale, shift, res, relu, out, stream, 1 << 30, ext);   // one tile per CTA
 }
 
 // conv3 (1x1) of block 0 fused with the projection shortcut: out = relu([t2 | x_strided] . [W3*s3 | Wd*sd]^T + shift).
 // t2: (B,Ho,Wo,Cmid); x: (B,Hx,Wx,Cx) read with spatial stride `xstride`; wcat: [Cout][Cmid + Cx] fp16.
 int conv_fused_ds(int B, int Ho, int Wo, int Cmid, const __half* t2, int Hx, int Wx, int Cx, int xstride,
                   const __half* x, const __half* wcat, int Cout, const float* scale, const float* shift, __half* out,
-                  cudaStream_t stream) {
+                  cudaStream_t stream, const ConvExt* ext) {
   DIRB_REQUIRE(Cmid % 64 == 0 && Cx % 64 == 0 && Cout % 256 == 0, DIRB200_ENOTSUP, "fused shortcut needs 64-multiples");
   constexpr int BN = 128;
   ConvPersParams p{};
@@ -184,6 +210,7 @@ int conv_fused_ds(int B, int Ho, int Wo, int Cmid, const __half* t2, int Hx, int
   p.relu = 1;
   p.scale = scale;
   p.shift = shift;
+  set_ext(p, ext, Ho, Wo);
   const int64_t total = (int64_t)p.tiles_w * p.tiles_h * ceil_div(B, p.nb) * p.n_tiles;
   DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
   p.total_tiles = static_cast<int>(total);
@@ -192,6 +219,8 @@ int conv_fused_ds(int B, int Ho, int Wo, int Cmid, const __half* t2, int Hx, int
   DIRB_TRY(encode_tmap_nhwc(&tmX, x, B, Hx, Wx, Cx, p.tw, p.th, p.nb, xstride));
   DIRB_TRY(encode_tmap_nhwc(&tmO, out, B, Ho, Wo, Cout, p.tw, p.th, p.nb, 1));
   DIRB_TRY(encode_tmap_2d(&tmB, wcat, Cmid + Cx, Cout, (uint64_t)(Cmid + Cx) * 2, 64, BN));
+  if (p.ext != nullptr)
+    return conv_pers_launch<BN, PersStages<BN>::CONV, PERS_EPI_CONV, false, true>(tmA, tmB, tmX, tmO, p, num_sms(), stream);
   return conv_pers_launch<BN, PersStages<BN>::CONV, PERS_EPI_CONV>(tmA, tmB, tmX, tmO, p, num_sms(), stream);
 }
 
@@ -205,7 +234,7 @@ bool conv_c23_profitable(int B, int H, int W, int Cm) {
 
 int conv_c23(int B, int H, int W, int Cm, const __half* t1, const __half* w2, const float* scale2, const float* shift2,
              const __half* w3, const float* scale3, const float* shift3, const __half* res, __half* out,
-             cudaStream_t stream) {
+             cudaStream_t stream, const ConvExt* ext) {
   DIRB_REQUIRE(conv_c23_supported(H, W, Cm), DIRB200_ENOTSUP, "fused conv2+conv3 needs Cm in {64, 128, 256}, H >= 16, W >= 8 (got %d, %d, %d)", Cm, H, W);
   DIRB_REQUIRE(t1 && w2 && w3 && res && out, DIRB200_EINVAL, "null argument");
   ConvPersParams p{};
@@ -216,6 +245,7 @@ int conv_c23(int B, int H, int W, int Cm, const __half* t1, const __half* w2, co
   p.n_tiles = 1;
   p.scale = scale3;
   p.shift = shift3;
+  set_ext(p, ext, H, W);
   const int64_t total = (int64_t)p.tiles_w * p.tiles_h * B;
   DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
   p.total_tiles = static_cast<int>(total);
@@ -225,6 +255,11 @@ int conv_c23(int B, int H, int W, int Cm, const __half* t1, const __half* w2, co
   DIRB_TRY(encode_tmap_2d(&tmB3, w3, Cm, 4 * Cm, (uint64_t)Cm * 2, 64, 128));
   DIRB_TRY(encode_tmap_nhwc(&tmR, res, B, H, W, 4 * Cm, 8, 16, 1, 1));
   DIRB_TRY(encode_tmap_nhwc(&tmO, out, B, H, W, 4 * Cm, 8, 16, 1, 1));
+  if (p.ext != nullptr) {
+    if (Cm == 256) return conv_c23_launch<256, true>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
+    if (Cm == 64) return conv_c23_launch<64, true>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
+    return conv_c23_launch<128, true>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
+  }
   if (Cm == 256) return conv_c23_launch<256>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
   if (Cm == 64) return conv_c23_launch<64>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
   return conv_c23_launch<128>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
@@ -241,13 +276,15 @@ int conv_c23(int B, int H, int W, int Cm, const __half* t1, const __half* w2, co
 // (X < Wo, 64 channels = 128 bytes per pixel), so the stem is a 4x1 convolution over R with Cin = 64 and runs on the
 // wgmma kernel (conv_pers.cuh) with the weight layout W2 unchanged (K index = a*64 + b*16 + j).
 // NCHW fp32 -> R: one thread per 2x2 block and horizontal neighbour b.
+// Ragged batch: ext = the pictures' {h, w} (stride ext_ld); pixels outside them are never read and enter as 0.
 __global__ void s2d_kernel(const float* __restrict__ in, __half* __restrict__ out, int H, int W, int Hs, int Wo,
-                           int64_t total) {
+                           int64_t total, const int* __restrict__ ext, int ext_ld) {
   const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i >= total) return;
   const int X = static_cast<int>((i >> 2) % Wo) + static_cast<int>(i & 3);
   const int Y = static_cast<int>(((i >> 2) / Wo) % Hs);
   const int64_t n = (i >> 2) / (static_cast<int64_t>(Wo) * Hs);
+  const int hn = ext ? __ldg(ext + n * ext_ld) : H, wn = ext ? __ldg(ext + n * ext_ld + 1) : W;
   const float* img = in + n * 3 * static_cast<int64_t>(H) * W;
   const int64_t plane = static_cast<int64_t>(H) * W;
   uint32_t o[8];
@@ -257,7 +294,7 @@ __global__ void s2d_kernel(const float* __restrict__ in, __half* __restrict__ ou
     for (int dx = 0; dx < 2; ++dx) {
       const int y = 2 * Y + dy - 3, x = 2 * X + dx - 3;
       float c0 = 0.f, c1 = 0.f, c2 = 0.f;
-      if (y >= 0 && y < H && x >= 0 && x < W) {
+      if (y >= 0 && y < hn && x >= 0 && x < wn) {
         const int64_t off = static_cast<int64_t>(y) * W + x;
         c0 = __ldg(img + off);
         c1 = __ldg(img + plane + off);
@@ -274,13 +311,16 @@ __global__ void s2d_kernel(const float* __restrict__ in, __half* __restrict__ ou
 // Same from uint8 HWC pixels (what an image decoder yields): ToTensor (x / 255) and Normalize ((v - mean) / std) of
 // dirtorch/utils/transforms.py:27 are applied on the fly in fp32, in torch's order and with true divisions, so the
 // fp16 values are bit-identical to those of the fp32-input path.
+// Outside a ragged batch's pictures the input is 0 in normalised space (a uint8 0 would normalise to -mean/std).
 __global__ void s2d_u8_kernel(const uint8_t* __restrict__ in, __half* __restrict__ out, int H, int W, int Hs, int Wo,
-                              int64_t total, float m0, float m1, float m2, float s0, float s1, float s2) {
+                              int64_t total, float m0, float m1, float m2, float s0, float s1, float s2,
+                              const int* __restrict__ ext, int ext_ld) {
   const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i >= total) return;
   const int X = static_cast<int>((i >> 2) % Wo) + static_cast<int>(i & 3);
   const int Y = static_cast<int>(((i >> 2) / Wo) % Hs);
   const int64_t n = (i >> 2) / (static_cast<int64_t>(Wo) * Hs);
+  const int hn = ext ? __ldg(ext + n * ext_ld) : H, wn = ext ? __ldg(ext + n * ext_ld + 1) : W;
   const uint8_t* img = in + n * 3 * static_cast<int64_t>(H) * W;
   uint32_t o[8];
 #pragma unroll
@@ -289,7 +329,7 @@ __global__ void s2d_u8_kernel(const uint8_t* __restrict__ in, __half* __restrict
     for (int dx = 0; dx < 2; ++dx) {
       const int y = 2 * Y + dy - 3, x = 2 * X + dx - 3;
       float c0 = 0.f, c1 = 0.f, c2 = 0.f;
-      if (y >= 0 && y < H && x >= 0 && x < W) {
+      if (y >= 0 && y < hn && x >= 0 && x < wn) {
         const uint8_t* px = img + (static_cast<int64_t>(y) * W + x) * 3;
         c0 = __fdiv_rn(__fdiv_rn(static_cast<float>(px[0]), 255.0f) - m0, s0);
         c1 = __fdiv_rn(__fdiv_rn(static_cast<float>(px[1]), 255.0f) - m1, s1);
@@ -332,20 +372,24 @@ void pack_stem_w2(const float* w, __half* out) {
 }
 
 int stem_tc(const float* imgs, int B, int H, int W, const __half* w2, const float* scale, const float* shift,
-            __half* s2d_ws, __half* out, cudaStream_t stream, const uint8_t* imgs_u8, const float* mean_std) {
+            __half* s2d_ws, __half* out, cudaStream_t stream, const uint8_t* imgs_u8, const float* mean_std,
+            const ConvExt* in_ext, const ConvExt* out_ext) {
+  const int* ext = in_ext ? in_ext->hw : nullptr;
+  const int ext_ld = in_ext ? in_ext->ld : 0;
   int Ho, Wo, Hs, Ws;
   stem_dims(H, W, &Ho, &Wo, &Hs, &Ws);
   (void)Ho;
   const int64_t total = static_cast<int64_t>(B) * Hs * Wo * 4;
   if (imgs_u8 != nullptr)
     s2d_u8_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(
-        imgs_u8, s2d_ws, H, W, Hs, Wo, total, mean_std[0], mean_std[1], mean_std[2], mean_std[3], mean_std[4], mean_std[5]);
+        imgs_u8, s2d_ws, H, W, Hs, Wo, total, mean_std[0], mean_std[1], mean_std[2], mean_std[3], mean_std[4], mean_std[5],
+        ext, ext_ld);
   else
-    s2d_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(imgs, s2d_ws, H, W, Hs, Wo, total);
+    s2d_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(imgs, s2d_ws, H, W, Hs, Wo, total, ext, ext_ld);
   count_launch();
   DIRB_CUDA(cudaGetLastError());
   const ConvShape s{B, Hs, Wo, 64, 64, 4, 1, 1, 0};      // 4x1 over the row-expanded tensor: Ho = Hs - 3, Wo
-  return conv_tc(s, s2d_ws, w2, scale, shift, nullptr, 1, out, stream);
+  return conv_tc(s, s2d_ws, w2, scale, shift, nullptr, 1, out, stream, out_ext);
 }
 
 // ------------------------------------------------------------------------------------------------ mma.sync path

@@ -34,7 +34,7 @@ struct C23Smem {
   static constexpr int TOTAL = BAR_OFF + 8 * NUM_BARS + 1024;
 };
 
-template <int CM>
+template <int CM, bool RAGGED>
 __global__ void __launch_bounds__(PERS_THREADS, 1)
 conv_c23_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB2,
                 const __grid_constant__ CUtensorMap tmB3, const __grid_constant__ CUtensorMap tmR,
@@ -210,6 +210,13 @@ conv_c23_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       if (wg_leader) mbar_arrive(&empty_bar[(g - 1) % STAGES]);
 
       mbar_wait(res_bar, rc & 1);                   // residual chunk has landed in the staging buffers
+      // ragged batch: conv2's T2 rows outside the image are not masked - they feed conv3 at the same pixel only, whose
+      // output is zeroed here
+      bool keep[2] = {true, true};
+      if constexpr (RAGGED) {
+        keep[0] = row_in_extent(p, c.m_tile, c.wo0, c.ho0, c.n0, r0);
+        keep[1] = row_in_extent(p, c.m_tile, c.wo0, c.ho0, c.n0, r0 + 8);
+      }
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int col = j * 8 + 2 * t4;
@@ -224,8 +231,8 @@ conv_c23_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           uint32_t rv;
           asm volatile("ld.shared.u32 %0, [%1];" : "=r"(rv) : "r"(sp));
           const float2 f = unpack_h2(rv);
-          v0 = fmaxf(v0 + f.x, 0.f);
-          v1 = fmaxf(v1 + f.y, 0.f);
+          v0 = keep[h] ? fmaxf(v0 + f.x, 0.f) : 0.f;
+          v1 = keep[h] ? fmaxf(v1 + f.y, 0.f) : 0.f;
           asm volatile("st.shared.u32 [%0], %1;" ::"r"(sp), "r"(pack_h2(v0, v1)) : "memory");
         }
       }
@@ -240,13 +247,13 @@ conv_c23_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   if (leader) bulk_wait<0>();
 }
 
-template <int CM>
+template <int CM, bool RAGGED = false>
 int conv_c23_launch(const CUtensorMap& tmA, const CUtensorMap& tmB2, const CUtensorMap& tmB3, const CUtensorMap& tmR,
                     const CUtensorMap& tmO, const ConvPersParams& p, const float* scale2, const float* shift2, int num_sms,
                     cudaStream_t stream) {
   using L = C23Smem<CM>;
   static_assert(L::TOTAL <= 232448, "shared memory budget exceeded");
-  auto kern = conv_c23_kernel<CM>;
+  auto kern = conv_c23_kernel<CM, RAGGED>;
   static std::atomic<uint64_t> attr_done{0};
   if (first_launch_on_device(attr_done))
     DIRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));

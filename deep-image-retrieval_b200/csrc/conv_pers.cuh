@@ -57,7 +57,33 @@ struct ConvPersParams {
   // Device-side launch predicate (retry passes of the search): when non-null the whole grid returns at once unless
   // *gate != 0.  The value was written by the previous kernel of the stream, so it is read after pdl_wait().
   const int* gate;
+  // Ragged batches (convolution epilogue): image n of the output tensor holds a picture of ext[n*ext_ld] x
+  // ext[n*ext_ld + 1] pixels in its top-left corner; every output pixel outside it is written as 0.  ext_n = images in
+  // the tensor, out_h / out_w = its spatial dims (the flat 2-D mode decodes a row index with them).  kc_major (spatial
+  // tiles with nb == 1 only): kc_major[n*ext_ld] != 0 walks image n's K loop channel block outer, tap inner - the
+  // order of the HALO mode - so its bits equal those of a HALO launch.  Null = a plain dense batch.
+  const int* ext;
+  const int* kc_major;
+  int ext_ld, ext_n, out_h, out_w;
 };
+
+// Whether accumulator row r of tile c lies inside its image's extent (ragged batches; true without an extent table).
+__device__ __forceinline__ bool row_in_extent(const ConvPersParams& p, int m_tile, int wo0, int ho0, int n0, int r) {
+  if (p.ext == nullptr) return true;
+  int n, y, x;
+  if (p.a_spatial) {
+    x = wo0 + r % p.tw;
+    y = ho0 + (r / p.tw) % p.th;
+    n = n0 + r / (p.tw * p.th);
+  } else {
+    const int64_t m = static_cast<int64_t>(m_tile) * 128 + r;
+    x = static_cast<int>(m % p.out_w);
+    y = static_cast<int>((m / p.out_w) % p.out_h);
+    n = static_cast<int>(m / (static_cast<int64_t>(p.out_w) * p.out_h));
+  }
+  if (n >= p.ext_n) return false;                  // beyond the tensor: the TMA store clips the row anyway
+  return y < __ldg(p.ext + static_cast<int64_t>(n) * p.ext_ld) && x < __ldg(p.ext + static_cast<int64_t>(n) * p.ext_ld + 1);
+}
 
 // HALO (3x3 / stride 1 / pad 1, 8 x 16 output tiles): the ring holds weight tiles only; per 64-channel block ONE TMA box
 // brings the 10 x 18 input patch into a separate ring of NP patch slots, and the nine taps read it as shifted views.
@@ -117,7 +143,8 @@ __device__ __forceinline__ void store_dense_pair(const ConvPersParams& p, int64_
   }
 }
 
-template <int BN, int STAGES, int EPI, bool HALO>
+// RAGGED: the launch carries an extent table (ConvPersParams::ext); dense launches compile without its code.
+template <int BN, int STAGES, int EPI, bool HALO, bool RAGGED>
 __global__ void __launch_bounds__(PERS_THREADS, 1)
 conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO,
@@ -171,6 +198,8 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       uint32_t gp = 0;  // patch slot counter (HALO)
       for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
         const TileCoord c = decode_tile(p, t);
+        const bool kcm = RAGGED && !HALO && p.kc_major != nullptr &&
+                         __ldg(p.kc_major + static_cast<int64_t>(c.n0) * p.ext_ld) != 0;
         if constexpr (HALO) {
           for (int kc = 0; kc < p.cin_blocks; ++kc, ++gp) {
             const int ps = gp % L::NP;
@@ -190,8 +219,14 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           mbar_wait(&empty_bar[s], ((g / STAGES) & 1) ^ 1);
           mbar_expect_tx(&full_bar[s], L::STAGE_BYTES);
           uint8_t* sa = smem + s * L::STAGE_BYTES;
-          const int tap = it / p.cin_blocks;
-          const int kc = it - tap * p.cin_blocks;
+          int tap = it / p.cin_blocks;
+          int kc = it - tap * p.cin_blocks;
+          int kb = it;                                // weight block of this k-iteration
+          if (kcm) {                                  // HALO order: channel block outer, tap inner
+            kc = it / p.taps;
+            tap = it - kc * p.taps;
+            kb = tap * p.cin_blocks + kc;
+          }
           if (EPI == PERS_EPI_F32) {
             const int part = it / p.k_per_part;
             const int kk = it - part * p.k_per_part;
@@ -212,7 +247,7 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           } else {
             tma_load_2d(sa, &tmA, &full_bar[s], it * 64, c.m_tile * 128);
           }
-          tma_load_2d(sa + L::A_BYTES, &tmB, &full_bar[s], it * 64, c.n_tile * BN);
+          tma_load_2d(sa + L::A_BYTES, &tmB, &full_bar[s], kb * 64, c.n_tile * BN);
         }
       }
     }
@@ -317,6 +352,11 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         named_bar_sync(1, PERS_CONSUMER_THREADS);
       }
       const uint32_t stg_addr = smem_u32(stg);
+      bool keep[2] = {true, true};
+      if constexpr (RAGGED) {
+        keep[0] = row_in_extent(p, c.m_tile, c.wo0, c.ho0, c.n0, r0);
+        keep[1] = row_in_extent(p, c.m_tile, c.wo0, c.ho0, c.n0, r0 + 8);
+      }
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int col = j * 8 + 2 * t4;
@@ -338,6 +378,10 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (p.relu) {
             v0 = fmaxf(v0, 0.f);
             v1 = fmaxf(v1, 0.f);
+          }
+          if (RAGGED && !keep[h]) {                           // ragged batch: outside the image = zero padding of the next layer
+            v0 = 0.f;
+            v1 = 0.f;
           }
           asm volatile("st.shared.u32 [%0], %1;" ::"r"(sp), "r"(pack_h2(v0, v1)) : "memory");
         }
@@ -432,12 +476,12 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (EPI == PERS_EPI_CONV && leader) bulk_wait<0>();     // all output bytes written before the CTA retires
 }
 
-template <int BN, int STAGES, int EPI, bool HALO = false>
+template <int BN, int STAGES, int EPI, bool HALO = false, bool RAGGED = false>
 int conv_pers_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO,
                      const ConvPersParams& p, int num_sms, cudaStream_t stream) {
   using L = ConvPersSmem<BN, STAGES, EPI, HALO>;
   static_assert(L::TOTAL <= 232448, "shared memory budget exceeded");
-  auto kern = conv_pers_kernel<BN, STAGES, EPI, HALO>;
+  auto kern = conv_pers_kernel<BN, STAGES, EPI, HALO, RAGGED>;
   static std::atomic<uint64_t> attr_done{0};
   if (first_launch_on_device(attr_done))
     DIRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));

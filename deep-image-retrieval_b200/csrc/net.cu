@@ -119,6 +119,9 @@ struct dirb200_net {
   int desc_dim() const { return without_fc ? feat_in() : out_dim; }
   int sub[5] = {0, 0, 0, 0, 0};   // images per sub-chunk of stage 0..4 (0 = auto)
   int stage_sched = 0;            // 0 = every stage over the whole chunk (fastest measured), 1 = per-stage sub-chunks
+  // ragged entry points: device copy of the extent table (see RG_LD)
+  int* ext_dev = nullptr;
+  size_t ext_bytes = 0;
   // pipelined host entry point
   cudaStream_t copy_stream = nullptr;
   std::vector<cudaEvent_t> pipe_events;
@@ -239,7 +242,7 @@ static ConvLayer make_layer(const std::string& conv, const std::string& bn, int 
 }
 
 static int run_conv(dirb200_net* n, const ConvLayer& L, const __half* in, int B, int H, int W, const __half* res,
-                    int relu, __half* out, cudaStream_t stream, int force_mma = 0) {
+                    int relu, __half* out, cudaStream_t stream, int force_mma = 0, const ConvExt* ext = nullptr) {
   ConvShape s{B, H, W, L.CinPad, L.Cout, L.K, L.K, L.stride, L.pad};
   const double flops = 2.0 * B * s.Ho() * s.Wo() * static_cast<double>(L.Cout) * L.K * L.K * L.Cin;
   // algorithmic bytes: input + output (+ residual) activations once, weights once
@@ -254,10 +257,11 @@ static int run_conv(dirb200_net* n, const ConvLayer& L, const __half* in, int B,
     tag = buf;
   }
   ProfScope ps(n, stream, mma ? 1 : 0, flops, bytes, tag);
+  DIRB_REQUIRE(!(mma && ext), DIRB200_ENOTSUP, "ragged batches need the wgmma convolutions (conv_impl 0 or 2)");
   if (mma)
     return conv_mma(s, in, L.w, L.Kpad, L.scale, L.shift, res, relu, out, stream);
-  if (n->conv_impl == 2) return conv_tc_np(s, in, L.w, L.scale, L.shift, res, relu, out, stream);
-  return conv_tc(s, in, L.w, L.scale, L.shift, res, relu, out, stream);
+  if (n->conv_impl == 2) return conv_tc_np(s, in, L.w, L.scale, L.shift, res, relu, out, stream, ext);
+  return conv_tc(s, in, L.w, L.scale, L.shift, res, relu, out, stream, ext);
 }
 
 extern "C" {
@@ -515,6 +519,60 @@ struct Workspace {
 };
 }  // namespace
 
+// Ragged batches: B pictures of sizes (h_i, w_i) in the top-left corners of B slots of one shape (H, W).  Every kernel
+// writes 0 outside a picture (what zero padding feeds its border) and the head pools over the picture's own pixels,
+// so each descriptor equals, bit for bit, the one of a B = 1 forward of the picture at its own size.  The extent table
+// holds per picture and resolution level one row {h, w, plain, block}: level 0 = input, 1 = stem convolution output,
+// 2 + s = output of stage s (0 maxpool, 1..4 layer1..4), sizes from the formulas of setup_workspace.  plain / block =
+// the K order (1 = HALO order, 0 = tap by tap) that a B = 1 forward gives a 3x3 stride-1 convolution at that level,
+// standalone / as conv2 of an identity Bottleneck (which fuse_c23 may take).  Where a pass's pictures disagree with
+// the slot's kernel choice, that convolution runs image by image in each picture's own order (ConvExt::kc_major).
+constexpr int RG_LEVELS = 7, RG_LD = 4 * RG_LEVELS;
+
+namespace {
+struct Ragged {
+  const int* dev = nullptr;    // table rows of the pass's pictures (device)
+  const int* host = nullptr;   // the same rows on the host
+  bool on() const { return dev != nullptr; }
+  ConvExt at(int lvl, int b0, int nb, int slot_w) const {
+    return ConvExt{dev + static_cast<size_t>(b0) * RG_LD + 4 * lvl, RG_LD, nb, nullptr, slot_w};
+  }
+  bool all(int lvl, int col, int b0, int nb, int v) const {
+    for (int i = b0; i < b0 + nb; ++i)
+      if (host[static_cast<size_t>(i) * RG_LD + 4 * lvl + col] != v) return false;
+    return true;
+  }
+};
+}  // namespace
+
+// The HALO mode's choice of conv_pers_any for a 3x3 stride-1 convolution at h x w (conv_impl 2 never takes it).
+static bool halo_order_plain(const dirb200_net* n, int h, int w) {
+  return get_conv_halo() && n->conv_impl == 0 && h >= 16 && w >= 8;
+}
+
+// Whether an identity Bottleneck of B images at h x w with Cm mid channels runs as the fused conv_c23 kernel.
+static bool c23_taken(const dirb200_net* n, int B, int h, int w, int Cm) {
+  return !n->basic && n->fuse_c23 && n->conv_impl == 0 &&
+         (n->fuse_c23 == 2 ? conv_c23_supported(h, w, Cm) : conv_c23_profitable(B, h, w, Cm));
+}
+
+static void ragged_table(const dirb200_net* n, const int* hw, int B, std::vector<int>* t) {
+  t->assign(static_cast<size_t>(B) * RG_LD, 0);
+  for (int i = 0; i < B; ++i) {
+    int* r = t->data() + static_cast<size_t>(i) * RG_LD;
+    int h = hw[2 * i], w = hw[2 * i + 1];
+    for (int l = 0; l < RG_LEVELS; ++l) {
+      if (l == 1) { h = (h + 6 - 7) / 2 + 1; w = (w + 6 - 7) / 2 + 1; }           // stem conv
+      else if (l == 2 || l >= 4) { h = (h + 2 - 3) / 2 + 1; w = (w + 2 - 3) / 2 + 1; }   // maxpool, layer2..4
+      const int Cm = 64 << std::max(0, l - 3);   // mid channels of the identity blocks at level l (layer1 at 2 and 3)
+      r[4 * l] = h;
+      r[4 * l + 1] = w;
+      r[4 * l + 2] = halo_order_plain(n, h, w) ? 1 : 0;
+      r[4 * l + 3] = (c23_taken(n, 1, h, w, Cm) || r[4 * l + 2]) ? 1 : 0;
+    }
+  }
+}
+
 static int setup_workspace(dirb200_net* n, int chunk, int H, int W, Workspace* w) {
   w->H1 = (H + 6 - 7) / 2 + 1; w->W1 = (W + 6 - 7) / 2 + 1;                 // stem conv
   w->h[0] = (w->H1 + 2 - 3) / 2 + 1; w->w[0] = (w->W1 + 2 - 3) / 2 + 1;     // maxpool
@@ -575,8 +633,23 @@ static int setup_workspace(dirb200_net* n, int chunk, int H, int W, Workspace* w
 
 // One pass of the network over `cb` images (NCHW fp32 on the device) -> cb descriptors.
 static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs_dev, int cb, int H, int W, float* desc_dev,
-                     __half* desc16_dev, cudaStream_t stream, const uint8_t* imgs_u8 = nullptr) {
+                     __half* desc16_dev, cudaStream_t stream, const uint8_t* imgs_u8 = nullptr,
+                     const Ragged& rg = Ragged()) {
   const int D = n->desc_dim();
+  ConvExt e0, e1;   // extents handed to one launch (ragged batches; the launchers read them on the host)
+  auto ext = [&](ConvExt& e, int lvl, int b0, int nb, int slot_w) -> const ConvExt* {
+    if (!rg.on()) return nullptr;
+    e = rg.at(lvl, b0, nb, slot_w);
+    return &e;
+  };
+  // 3x3 stride-1 convolution whose K order on the slot is slot_order: pictures that a B = 1 forward gives another
+  // order (column col of the table) make the launch pick the order image by image
+  auto ext3 = [&](ConvExt& e, int lvl, int b0, int nb, int slot_w, int col, bool slot_order) -> const ConvExt* {
+    if (!rg.on()) return nullptr;
+    e = rg.at(lvl, b0, nb, slot_w);
+    if (!rg.all(lvl, col, b0, nb, slot_order ? 1 : 0)) e.kc_major = e.hw + col;
+    return &e;
+  };
   // ---------------------------------------------------------------- stage 0: stem + maxpool
   for (int b0 = 0; b0 < cb; b0 += w.sub[0]) {
     const int sb = std::min(w.sub[0], cb - b0);
@@ -594,11 +667,12 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs_dev, 
       n->last_flops += flops;
       ProfScope ps(n, stream, 1, flops, static_cast<double>(sb) * (12.0 * H * W + 2.0 * stem_workspace_bytes(1, H, W) + 128.0 * w.H1 * w.W1), "stem s2d + 7x7/s2 3->64");
       DIRB_TRY(stem_tc(img, sb, H, W, n->stem_w2, n->stem.scale, n->stem.shift, w.stem_ws, w.stem_out, stream, img8,
-                       n->mean_std));
+                       n->mean_std, ext(e0, 0, b0, sb, W), ext(e1, 1, b0, sb, w.W1)));
     }
     ProfScope ps(n, stream, 2, 0, 2.0 * sb * 64 * (static_cast<double>(w.H1) * w.W1 + static_cast<double>(w.h[0]) * w.w[0]), "maxpool 3x3/s2");
     DIRB_TRY(maxpool_3x3s2(w.stem_out, sb, w.H1, w.W1, 64,
-                           w.stage_out[0] + static_cast<size_t>(b0) * w.h[0] * w.w[0] * 64, stream));
+                           w.stage_out[0] + static_cast<size_t>(b0) * w.h[0] * w.w[0] * 64, stream,
+                           ext(e0, 2, b0, sb, w.w[0])));
   }
   DIRB_TRY(record_tap(n, "stem", w.stage_out[0], cb, w.h[0], w.w[0], 64, stream));
   // ---------------------------------------------------------------- stages 1..4: layer1..layer4 (+ head)
@@ -611,9 +685,12 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs_dev, 
       const int sb = std::min(w.sub[s], cb - b0);
       const __half* x = stage_in + static_cast<size_t>(b0) * hi * wi * n->stage_ch[s - 1];
       int h = hi, wd = wi;
+      int lvl = 1 + s;                          // extent-table level of x
       for (int bi = first; bi < last; ++bi) {
         const Block& blk = n->blocks[bi];
         const int j = bi - first;
+        const int lvl_in = lvl;
+        if ((n->basic ? blk.c1.stride : blk.c2.stride) == 2) lvl = 2 + s;   // level of the block's output
         __half* t1 = w.scratch[0];
         __half* t2 = w.scratch[1];
         __half* rs = w.scratch[2];
@@ -623,13 +700,15 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs_dev, 
           // BasicBlock, resnet.py:27-44: 3x3(stride) + BN + ReLU -> 3x3 + BN -> + (projected) x -> ReLU
           const int st = blk.c1.stride;
           const int h2 = (h + 2 - 3) / st + 1, w2 = (wd + 2 - 3) / st + 1;
-          DIRB_TRY(run_conv(n, blk.c1, x, sb, h, wd, nullptr, 1, t1, stream));
+          DIRB_TRY(run_conv(n, blk.c1, x, sb, h, wd, nullptr, 1, t1, stream, 0,
+                            st == 1 ? ext3(e0, lvl, b0, sb, w2, 2, halo_order_plain(n, h2, w2)) : ext(e0, lvl, b0, sb, w2)));
           const __half* res = x;
           if (blk.has_down) {
-            DIRB_TRY(run_conv(n, blk.down, x, sb, h, wd, nullptr, 0, rs, stream));
+            DIRB_TRY(run_conv(n, blk.down, x, sb, h, wd, nullptr, 0, rs, stream, 0, ext(e0, lvl, b0, sb, w2)));
             res = rs;
           }
-          DIRB_TRY(run_conv(n, blk.c2, t1, sb, h2, w2, res, 1, y, stream));
+          DIRB_TRY(run_conv(n, blk.c2, t1, sb, h2, w2, res, 1, y, stream, 0,
+                            ext3(e0, lvl, b0, sb, w2, 2, halo_order_plain(n, h2, w2))));
           x = y;
           h = h2;
           wd = w2;
@@ -637,9 +716,12 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs_dev, 
         }
         const int st = blk.c2.stride;
         const int h2 = (h + 2 - 3) / st + 1, w2 = (wd + 2 - 3) / st + 1;
-        DIRB_TRY(run_conv(n, blk.c1, x, sb, h, wd, nullptr, 1, t1, stream));
-        if (!blk.has_down && n->fuse_c23 && n->conv_impl == 0 && st == 1 &&
-            (n->fuse_c23 == 2 ? conv_c23_supported(h, wd, blk.c2.Cin) : conv_c23_profitable(sb, h, wd, blk.c2.Cin))) {
+        DIRB_TRY(run_conv(n, blk.c1, x, sb, h, wd, nullptr, 1, t1, stream, 0, ext(e0, lvl_in, b0, sb, wd)));
+        const bool c23 = !blk.has_down && st == 1 && c23_taken(n, sb, h, wd, blk.c2.Cin);
+        // ragged: a stride-1 conv2 in the K order of the slot's kernel choice (the fused kernel has the HALO order)
+        const ConvExt* e2 = st == 1 ? ext3(e1, lvl, b0, sb, wd, blk.has_down ? 2 : 3, c23 || halo_order_plain(n, h, wd))
+                                    : ext(e1, lvl, b0, sb, w2);
+        if (c23 && (e2 == nullptr || e2->kc_major == nullptr)) {
           // identity block: conv2 -> conv3 (+ x) in one kernel, the conv2 output stays in shared memory
           const int Cm = blk.c2.Cin;
           const double flops = 2.0 * sb * h * wd * (9.0 * Cm * Cm + 4.0 * Cm * Cm);
@@ -649,11 +731,11 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs_dev, 
           snprintf(tg, sizeof(tg), "3x3 %d->%d + 1x1 ->%d +res fused @%dx%d", Cm, Cm, 4 * Cm, h, wd);
           ProfScope ps(n, stream, 0, flops, bytes, tg);
           DIRB_TRY(conv_c23(sb, h, wd, Cm, t1, blk.c2.w, blk.c2.scale, blk.c2.shift, blk.c3.w, blk.c3.scale, blk.c3.shift, x, y,
-                            stream));
+                            stream, e2));
           x = y;
           continue;
         }
-        DIRB_TRY(run_conv(n, blk.c2, t1, sb, h, wd, nullptr, 1, t2, stream));
+        DIRB_TRY(run_conv(n, blk.c2, t1, sb, h, wd, nullptr, 1, t2, stream, 0, e2));
         const __half* res = x;
         if (blk.has_down && n->fuse_ds && n->conv_impl == 0 && blk.c3.Cout % 256 == 0) {
           const double flops = 2.0 * sb * h2 * w2 * static_cast<double>(blk.c3.Cout) * (blk.c3.Cin + blk.down.Cin);
@@ -665,17 +747,17 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs_dev, 
           snprintf(tbuf_, sizeof(tbuf_), "1x1 [%d|%d%s]->%d fused-shortcut @%dx%d", blk.c3.Cin, blk.down.Cin, st == 2 ? "/s2" : "", blk.c3.Cout, h2, w2);
           ProfScope ps(n, stream, 0, flops, bytes, tbuf_);
           DIRB_TRY(conv_fused_ds(sb, h2, w2, blk.c3.Cin, t2, h, wd, blk.down.Cin, st, x, blk.wcat, blk.c3.Cout, blk.ones,
-                                 blk.cat_shift, y, stream));
+                                 blk.cat_shift, y, stream, ext(e0, lvl, b0, sb, w2)));
           x = y;
           h = h2;
           wd = w2;
           continue;
         }
         if (blk.has_down) {
-          DIRB_TRY(run_conv(n, blk.down, x, sb, h, wd, nullptr, 0, rs, stream));
+          DIRB_TRY(run_conv(n, blk.down, x, sb, h, wd, nullptr, 0, rs, stream, 0, ext(e0, lvl, b0, sb, w2)));
           res = rs;
         }
-        DIRB_TRY(run_conv(n, blk.c3, t2, sb, h2, w2, res, 1, y, stream));
+        DIRB_TRY(run_conv(n, blk.c3, t2, sb, h2, w2, res, 1, y, stream, 0, ext(e0, lvl, b0, sb, w2)));
         x = y;
         h = h2;
         wd = w2;
@@ -718,11 +800,12 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs_dev, 
         }
         ProfScope ps(n, stream, 3, n->without_fc ? 0.0 : 2.0 * sb * static_cast<double>(C4) * n->out_dim, 2.0 * sb * ho * wo * static_cast<double>(C4), "head pool+fc+l2");
         if (n->center_bias > 0.0f)   // x is a scratch buffer whose only remaining reader is the pooling below
-          DIRB_TRY(center_bias(const_cast<__half*>(x), sb, ho, wo, C4, n->center_bias, stream));
+          DIRB_TRY(center_bias(const_cast<__half*>(x), sb, ho, wo, C4, n->center_bias, stream, ext(e0, 6, b0, sb, wo)));
         DIRB_TRY(head_pool_fc_l2(x, sb, ho * wo, C4, n->pooling, n->gem_p, n->gem_eps, n->norm_features,
                                  n->without_fc ? nullptr : n->fc_w, n->without_fc ? nullptr : n->fc_b, D, w.head_ws,
                                  desc_dev + static_cast<size_t>(b0) * D,
-                                 desc16_dev ? desc16_dev + static_cast<size_t>(b0) * D : nullptr, stream, n->head_bar));
+                                 desc16_dev ? desc16_dev + static_cast<size_t>(b0) * D : nullptr, stream, n->head_bar,
+                                 ext(e0, 6, b0, sb, wo)));
         if (!n->without_fc) n->last_flops += 2.0 * sb * static_cast<double>(C4) * n->out_dim;
       }
     }
@@ -794,6 +877,64 @@ int dirb200_net_forward_u8(dirb200_net* n, const uint8_t* imgs_dev, int B, int H
   }
   n->last_launches = launches_total() - launches0;
   return 0;
+}
+
+// Ragged batch: B pictures of sizes hw_host[i] in the top-left corners of slots of H x W (see RG_LD).
+static int forward_ragged_impl(dirb200_net* n, const float* slots, const uint8_t* slots_u8, int B, int H, int W,
+                               const int* hw_host, float* desc_dev, void* desc16_dev, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DIRB_REQUIRE(n && (slots || slots_u8) && hw_host && desc_dev, DIRB200_EINVAL, "null argument");
+  DIRB_TRY(check_forward_args(n, B, H, W));
+  DIRB_REQUIRE(!n->fpn, DIRB200_ENOTSUP,
+               "ragged batches do not support FPN heads (their upsampling ratio depends on each picture's size)");
+  DIRB_REQUIRE(n->conv_impl != 1, DIRB200_ENOTSUP, "ragged batches need the wgmma convolutions (conv_impl 0 or 2)");
+  for (int i = 0; i < B; ++i)
+    DIRB_REQUIRE(hw_host[2 * i] >= 32 && hw_host[2 * i] <= H && hw_host[2 * i + 1] >= 32 && hw_host[2 * i + 1] <= W,
+                 DIRB200_EINVAL, "picture %d: size %dx%d is outside [32, %d] x [32, %d]", i, hw_host[2 * i],
+                 hw_host[2 * i + 1], H, W);
+  DIRB_CUDA(cudaSetDevice(n->device));
+  std::vector<int> table;
+  ragged_table(n, hw_host, B, &table);
+  const size_t tbytes = table.size() * sizeof(int);
+  if (tbytes > n->ext_bytes) {
+    if (n->ext_dev) DIRB_CUDA(cudaFree(n->ext_dev));
+    n->ext_dev = nullptr;
+    DIRB_CUDA(cudaMalloc(reinterpret_cast<void**>(&n->ext_dev), tbytes));
+    n->ext_bytes = tbytes;
+  }
+  // pageable source: the copy is staged before the call returns, and it is ordered before the kernels that read it
+  DIRB_CUDA(cudaMemcpyAsync(n->ext_dev, table.data(), tbytes, cudaMemcpyHostToDevice, stream));
+  const int64_t launches0 = launches_total();
+  n->last_flops = 0;
+  if (n->profile != 2) n->prof.reset();
+  const int chunk = n->chunk > 0 ? std::min(n->chunk, B) : auto_chunk(B, H, W);
+  const int D = n->desc_dim();
+  Workspace w;
+  DIRB_TRY(setup_workspace(n, chunk, H, W, &w));
+  for (int b0 = 0; b0 < B; b0 += chunk) {
+    const int cb = std::min(chunk, B - b0);
+    const size_t img = static_cast<size_t>(b0) * 3 * H * W;
+    Ragged rg;
+    rg.dev = n->ext_dev + static_cast<size_t>(b0) * RG_LD;
+    rg.host = table.data() + static_cast<size_t>(b0) * RG_LD;
+    DIRB_TRY(run_chunk(n, w, slots ? slots + img : nullptr, cb, H, W, desc_dev + static_cast<size_t>(b0) * D,
+                       desc16_dev ? static_cast<__half*>(desc16_dev) + static_cast<size_t>(b0) * D : nullptr, stream,
+                       slots_u8 ? slots_u8 + img : nullptr, rg));
+  }
+  n->last_launches = launches_total() - launches0;
+  return 0;
+}
+
+int dirb200_net_forward_ragged_u8(dirb200_net* n, const uint8_t* slots_dev, int B, int H, int W, const int* hw_host,
+                                  float* desc_dev, void* desc16_dev, void* stream) {
+  DIRB_REQUIRE(slots_dev, DIRB200_EINVAL, "null argument");
+  return forward_ragged_impl(n, nullptr, slots_dev, B, H, W, hw_host, desc_dev, desc16_dev, stream);
+}
+
+int dirb200_net_forward_ragged(dirb200_net* n, const float* slots_dev, int B, int H, int W, const int* hw_host,
+                               float* desc_dev, void* desc16_dev, void* stream) {
+  DIRB_REQUIRE(slots_dev, DIRB200_EINVAL, "null argument");
+  return forward_ragged_impl(n, slots_dev, nullptr, B, H, W, hw_host, desc_dev, desc16_dev, stream);
 }
 
 static int forward_host_impl(dirb200_net* n, const void* imgs_host_, int is_u8, int B, int H, int W, float* desc_host) {
@@ -949,6 +1090,7 @@ int dirb200_net_destroy(dirb200_net* n) {
   if (n->ws) cudaFree(n->ws);
   if (n->h2d) cudaFree(n->h2d);
   if (n->d_desc) cudaFree(n->d_desc);
+  if (n->ext_dev) cudaFree(n->ext_dev);
   if (n->own_stream) cudaStreamDestroy(n->own_stream);
   if (n->copy_stream) cudaStreamDestroy(n->copy_stream);
   for (auto e : n->pipe_events) cudaEventDestroy(e);

@@ -34,8 +34,11 @@ int nchw_to_nhwc8(const float* in, int B, int H, int W, __half* out, cudaStream_
 
 // ---------------------------------------------------------------------------------------------------------------
 // MaxPool2d(kernel 3, stride 2, padding 1), NHWC fp16, 8 channels per thread.   (resnet.py:119,161)
+// Ragged batch (ext != nullptr): outputs outside image b's extent are 0.  Inside, a window may reach beyond the
+// extent into the zeros there: its inputs are >= 0 (after ReLU) and it holds a pixel of the image, so the maximum is
+// the one of -inf padding.
 __global__ void maxpool_kernel(const __half* __restrict__ in, __half* __restrict__ out, int B, int H, int W, int C,
-                               int Ho, int Wo) {
+                               int Ho, int Wo, const int* __restrict__ ext, int ext_ld) {
   const int cv = C / 8;
   const int64_t total = static_cast<int64_t>(B) * Ho * Wo * cv;
   const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
@@ -64,14 +67,19 @@ __global__ void maxpool_kernel(const __half* __restrict__ in, __half* __restrict
       for (int e = 0; e < 4; ++e) m[e] = __hmax2(m[e], h[e]);
     }
   }
+  if (ext != nullptr && (ho >= __ldg(ext + static_cast<int64_t>(b) * ext_ld) || wo >= __ldg(ext + static_cast<int64_t>(b) * ext_ld + 1))) {
+    reinterpret_cast<uint4*>(out)[i] = make_uint4(0u, 0u, 0u, 0u);
+    return;
+  }
   reinterpret_cast<uint4*>(out)[i] = *reinterpret_cast<uint4*>(m);
 }
 
-int maxpool_3x3s2(const __half* in, int B, int H, int W, int C, __half* out, cudaStream_t stream) {
+int maxpool_3x3s2(const __half* in, int B, int H, int W, int C, __half* out, cudaStream_t stream, const ConvExt* ext) {
   DIRB_REQUIRE(C % 8 == 0, DIRB200_ENOTSUP, "maxpool needs C %% 8 == 0");
   const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
   const int64_t total = static_cast<int64_t>(B) * Ho * Wo * (C / 8);
-  maxpool_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(in, out, B, H, W, C, Ho, Wo);
+  maxpool_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(in, out, B, H, W, C, Ho, Wo, ext ? ext->hw : nullptr,
+                                                                               ext ? ext->ld : 0);
   count_launch();
   DIRB_CUDA(cudaGetLastError());
   return 0;
@@ -92,6 +100,17 @@ namespace {
 constexpr int HEAD_PX_LANES = 8;
 constexpr int HEAD_THREADS = 256;
 
+// Number of partial sums of one image's pooling: depends on its pixel count only, so that a descriptor does not depend
+// on the batch it was computed in (the partial sums of one image are always combined in the same order).
+__host__ __device__ __forceinline__ int head_splits_hw(int HW) { return max(1, min(16, HW / 64)); }
+
+// Ragged batch: image b pools its own ext[b*ld] x ext[b*ld+1] pixels; pixel p of it sits at row p / w, column p % w
+// of a map whose rows are slot_w pixels long.
+struct HeadExt {
+  const int* ext;
+  int ld, slot_w;
+};
+
 __device__ __forceinline__ float gem_pow(float x, float p, int p_is3) { return p_is3 ? x * x * x : powf(x, p); }
 
 struct HeadSmem {
@@ -102,18 +121,26 @@ struct HeadSmem {
 // phase 1, virtual grid (C/256, S, B): thread = (pixel lane 0..7, channel group 0..31 of 8 channels)
 __device__ __forceinline__ void head_pool_partial_body(HeadSmem& sm, int bx, int s, int b, const __half* __restrict__ feat,
                                                        float* partial, int HW, int C, int S, int pooling, float p,
-                                                       float eps) {
+                                                       float eps, const HeadExt& he) {
   const int cg = threadIdx.x & 31, pl = threadIdx.x >> 5;
   const int c0 = bx * 256 + cg * 8;
-  const int per = (HW + S - 1) / S;
-  const int beg = s * per, end = min(HW, beg + per);
+  int hw = HW, Sb = S, wb = 1;
+  if (he.ext != nullptr) {                                  // S = the slot's splits, Sb <= S of them are this image's
+    wb = __ldg(he.ext + static_cast<int64_t>(b) * he.ld + 1);
+    hw = __ldg(he.ext + static_cast<int64_t>(b) * he.ld) * wb;
+    Sb = head_splits_hw(hw);
+    if (s >= Sb) return;                                    // uniform over the (virtual) block
+  }
+  const int per = (hw + Sb - 1) / Sb;
+  const int beg = s * per, end = min(hw, beg + per);
   const int p_is3 = (p == 3.0f);
   float acc[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) acc[e] = (pooling == 1) ? -INFINITY : 0.f;
   if (c0 < C) {
     for (int px = beg + pl; px < end; px += HEAD_PX_LANES) {
-      const uint4 v = __ldg(reinterpret_cast<const uint4*>(feat + (static_cast<int64_t>(b) * HW + px) * C + c0));
+      const int64_t at = he.ext != nullptr ? static_cast<int64_t>(px / wb) * he.slot_w + px % wb : px;
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(feat + (static_cast<int64_t>(b) * HW + at) * C + c0));
       const uint32_t u[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
@@ -159,12 +186,17 @@ __device__ __forceinline__ float block_sum(float v, float* sh) {
 // columns [col_off, col_off + C) of row b of g (row length g_ld): two feature maps can be pooled side by side (FPN).
 __device__ __forceinline__ void head_pool_final_body(HeadSmem& sm, int b, const float* partial, float* g, int HW, int C,
                                                      int S, int pooling, float p, int norm_features, int g_ld,
-                                                     int col_off) {
+                                                     int col_off, const HeadExt& he) {
   float* grow = g + static_cast<int64_t>(b) * g_ld + col_off;
   float ss = 0.f;
+  int Sb = S;
+  if (he.ext != nullptr) {
+    HW = __ldg(he.ext + static_cast<int64_t>(b) * he.ld) * __ldg(he.ext + static_cast<int64_t>(b) * he.ld + 1);
+    Sb = head_splits_hw(HW);
+  }
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float r = __ldcg(partial + (static_cast<int64_t>(b) * S) * C + c);
-    for (int s = 1; s < S; ++s) {
+    for (int s = 1; s < Sb; ++s) {
       const float q = __ldcg(partial + (static_cast<int64_t>(b) * S + s) * C + c);
       r = (pooling == 1) ? fmaxf(r, q) : r + q;
     }
@@ -233,15 +265,15 @@ __device__ __forceinline__ void l2_row_body(HeadSmem& sm, int64_t r, const float
 
 __global__ void __launch_bounds__(HEAD_THREADS) head_pool_partial_kernel(const __half* __restrict__ feat, float* partial,
                                                                          int HW, int C, int S, int pooling, float p,
-                                                                         float eps) {
+                                                                         float eps, const HeadExt he) {
   __shared__ HeadSmem sm;
-  head_pool_partial_body(sm, blockIdx.x, blockIdx.y, blockIdx.z, feat, partial, HW, C, S, pooling, p, eps);
+  head_pool_partial_body(sm, blockIdx.x, blockIdx.y, blockIdx.z, feat, partial, HW, C, S, pooling, p, eps, he);
 }
 __global__ void __launch_bounds__(HEAD_THREADS) head_pool_final_kernel(const float* partial, float* g, int HW, int C, int S,
                                                                        int pooling, float p, int norm_features, int g_ld,
-                                                                       int col_off) {
+                                                                       int col_off, const HeadExt he) {
   __shared__ HeadSmem sm;
-  head_pool_final_body(sm, blockIdx.x, partial, g, HW, C, S, pooling, p, norm_features, g_ld, col_off);
+  head_pool_final_body(sm, blockIdx.x, partial, g, HW, C, S, pooling, p, norm_features, g_ld, col_off, he);
 }
 __global__ void __launch_bounds__(HEAD_THREADS) head_fc_kernel(const float* g, const float* __restrict__ w,
                                                                const float* __restrict__ bias, float* y, int B, int C,
@@ -286,6 +318,7 @@ struct HeadFusedParams {
   unsigned int* bar;
   int B, HW, C, S, pooling, norm_features, out_dim;
   float p, eps;
+  HeadExt he;
 };
 
 __global__ void __launch_bounds__(HEAD_THREADS, 4) head_fused_kernel(const HeadFusedParams q) {
@@ -295,11 +328,12 @@ __global__ void __launch_bounds__(HEAD_THREADS, 4) head_fused_kernel(const HeadF
     const int gx = (q.C + 255) / 256;
     const int total = gx * q.S * q.B;
     for (int v = blockIdx.x; v < total; v += nb)
-      head_pool_partial_body(sm, v % gx, (v / gx) % q.S, v / (gx * q.S), q.feat, q.partial, q.HW, q.C, q.S, q.pooling, q.p, q.eps);
+      head_pool_partial_body(sm, v % gx, (v / gx) % q.S, v / (gx * q.S), q.feat, q.partial, q.HW, q.C, q.S, q.pooling, q.p, q.eps,
+                             q.he);
   }
   grid_barrier(q.bar, nb);
   for (int b = blockIdx.x; b < q.B; b += nb)   // ---- 2: finish the pooling
-    head_pool_final_body(sm, b, q.partial, q.g, q.HW, q.C, q.S, q.pooling, q.p, q.norm_features, q.C, 0);
+    head_pool_final_body(sm, b, q.partial, q.g, q.HW, q.C, q.S, q.pooling, q.p, q.norm_features, q.C, 0, q.he);
   const float* pre = q.g;
   int D = q.C;
   if (q.fc_w != nullptr) {
@@ -317,10 +351,12 @@ __global__ void __launch_bounds__(HEAD_THREADS, 4) head_fused_kernel(const HeadF
 }  // namespace
 
 static int head_splits(int B, int HW, int C) {
-  // Depends on the spatial size only, so that a descriptor does not depend on the batch it was computed in
-  // (the partial sums of one image are always combined in the same order).
   (void)B; (void)C;
-  return max(1, min(16, HW / 64));
+  return head_splits_hw(HW);
+}
+
+static HeadExt head_ext(const ConvExt* ext) {
+  return ext != nullptr ? HeadExt{ext->hw, ext->ld, ext->slot_w} : HeadExt{nullptr, 0, 0};
 }
 
 static size_t align32(size_t floats) { return (floats + 31) / 32 * 32; }   // 128-byte lines: no line shared by two buffers
@@ -334,13 +370,14 @@ size_t head_workspace_floats(int B, int HW, int C, int out_dim) {
 
 // Global pooling of one NHWC map into g[b][col_off .. col_off + C) (rows of g_ld floats); `partial` = B * S * C floats.
 int head_pool(const __half* feat, int B, int HW, int C, int pooling, float p, float eps, int norm_features, float* partial,
-              float* g, int g_ld, int col_off, cudaStream_t stream) {
+              float* g, int g_ld, int col_off, cudaStream_t stream, const ConvExt* ext) {
   DIRB_REQUIRE(C % 8 == 0 && C % 4 == 0, DIRB200_ENOTSUP, "head needs C %% 8 == 0");
   DIRB_REQUIRE(pooling >= 0 && pooling <= 2, DIRB200_EINVAL, "pooling mode %d", pooling);
   const int S = head_splits(B, HW, C);
   dim3 g1((unsigned)ceil_div(C, 256), (unsigned)S, (unsigned)B);
-  head_pool_partial_kernel<<<g1, HEAD_THREADS, 0, stream>>>(feat, partial, HW, C, S, pooling, p, eps);
-  head_pool_final_kernel<<<B, HEAD_THREADS, 0, stream>>>(partial, g, HW, C, S, pooling, p, norm_features, g_ld, col_off);
+  head_pool_partial_kernel<<<g1, HEAD_THREADS, 0, stream>>>(feat, partial, HW, C, S, pooling, p, eps, head_ext(ext));
+  head_pool_final_kernel<<<B, HEAD_THREADS, 0, stream>>>(partial, g, HW, C, S, pooling, p, norm_features, g_ld, col_off,
+                                                         head_ext(ext));
   count_launch(2);
   DIRB_CUDA(cudaGetLastError());
   return 0;
@@ -373,13 +410,13 @@ int get_head_fused() { return g_head_fused; }
 // reusable state after every launch); nullptr = use the tail of `ws` and clear it on the stream first.
 int head_pool_fc_l2(const __half* feat, int B, int HW, int C, int pooling, float p, float eps, int norm_features,
                     const float* fc_w, const float* fc_b, int out_dim, float* ws, float* desc, __half* desc16,
-                    cudaStream_t stream, unsigned int* bar) {
+                    cudaStream_t stream, unsigned int* bar, const ConvExt* ext) {
   const int S = head_splits(B, HW, C);
   float* partial = ws;
   float* g = partial + head_partial_floats(B, HW, C);
   float* y = g + align32(static_cast<size_t>(B) * C);
   if (!g_head_fused) {
-    DIRB_TRY(head_pool(feat, B, HW, C, pooling, p, eps, norm_features, partial, g, C, 0, stream));
+    DIRB_TRY(head_pool(feat, B, HW, C, pooling, p, eps, norm_features, partial, g, C, 0, stream, ext));
     return head_fc_l2(g, B, C, fc_w, fc_b, out_dim, y, desc, desc16, stream);
   }
   DIRB_REQUIRE(C % 8 == 0, DIRB200_ENOTSUP, "head needs C %% 8 == 0");
@@ -396,7 +433,8 @@ int head_pool_fc_l2(const __half* feat, int B, int HW, int C, int pooling, float
   }
   const int64_t work = std::max<int64_t>(ceil_div(C, 256) * S * B, fc_w ? ceil_div(out_dim, 8) * ceil_div(B, 8) : B);
   const int grid = static_cast<int>(std::min<int64_t>(static_cast<int64_t>(per_sm) * num_sms(), std::max<int64_t>(work, 1)));
-  HeadFusedParams q{feat, fc_w, fc_b, partial, g, y, desc, desc16, bar, B, HW, C, S, pooling, norm_features, out_dim, p, eps};
+  HeadFusedParams q{feat, fc_w, fc_b, partial, g, y, desc, desc16, bar, B, HW, C, S, pooling, norm_features, out_dim, p, eps,
+                    head_ext(ext)};
   head_fused_kernel<<<grid, HEAD_THREADS, 0, stream>>>(q);
   count_launch();
   DIRB_CUDA(cudaGetLastError());
@@ -457,12 +495,20 @@ __device__ __forceinline__ float center_bias_axis(int i, int n, int& i0, int& i1
   return 1.0f - l1;
 }
 
-__global__ void center_bias_kernel(__half* __restrict__ x, int H, int W, int C8, float b, int64_t total) {
+// Ragged batch (ext != nullptr): the map is resized to image n's own extent; pixels outside it stay 0.
+__global__ void center_bias_kernel(__half* __restrict__ x, int H, int W, int C8, float b, int64_t total,
+                                   const int* __restrict__ ext, int ext_ld) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int64_t pix = i / C8;
   const int wq = static_cast<int>(pix % W);
   const int hq = static_cast<int>((pix / W) % H);
+  if (ext != nullptr) {
+    const int64_t n = pix / (static_cast<int64_t>(W) * H);
+    H = __ldg(ext + n * ext_ld);
+    W = __ldg(ext + n * ext_ld + 1);
+    if (hq >= H || wq >= W) return;
+  }
   int h0, h1, w0, w1;
   float lh1, lw1;
   const float lh0 = center_bias_axis(hq, H, h0, h1, lh1);
@@ -482,11 +528,12 @@ __global__ void center_bias_kernel(__half* __restrict__ x, int H, int W, int C8,
   *ptr = v;
 }
 
-int center_bias(__half* x, int B, int H, int W, int C, float b, cudaStream_t stream) {
+int center_bias(__half* x, int B, int H, int W, int C, float b, cudaStream_t stream, const ConvExt* ext) {
   DIRB_REQUIRE(C % 8 == 0, DIRB200_ENOTSUP, "center_bias needs C %% 8 == 0 (got %d)", C);
   const int64_t total = static_cast<int64_t>(B) * H * W * (C / 8);
   if (total == 0 || b == 0.0f) return 0;
-  center_bias_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(x, H, W, C / 8, b, total);
+  center_bias_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(x, H, W, C / 8, b, total, ext ? ext->hw : nullptr,
+                                                                                          ext ? ext->ld : 0);
   count_launch();
   DIRB_CUDA(cudaGetLastError());
   return 0;

@@ -46,6 +46,8 @@ SIGNATURES = {
     "dirb200_net_forward_host": (i32, [p, p, i32, i32, i32, p]),
     "dirb200_net_forward_u8": (i32, [p, p, i32, i32, i32, p, p, p]),
     "dirb200_net_forward_host_u8": (i32, [p, p, i32, i32, i32, p]),
+    "dirb200_net_forward_ragged_u8": (i32, [p, p, i32, i32, i32, p, p, p, p]),
+    "dirb200_net_forward_ragged": (i32, [p, p, i32, i32, i32, p, p, p, p]),
     "dirb200_resize_bilinear_u8": (i32, [p, i32, i32, i32, i32, i32, p, p]),
     "dirb200_resize_coeffs": (i32, [i32, i32, p, p, C.POINTER(i32)]),
     "dirb200_net_debug_stage": (i32, [p, C.c_char_p, p, C.c_size_t, C.POINTER(i32), p]),

@@ -279,6 +279,52 @@ class ResNetRMAC:
                  C.c_void_p(0), C.c_void_p(torch.cuda.current_stream().cuda_stream))
         return desc[0] if b == 1 else desc
 
+    def forward_ragged_u8(self, imgs):
+        """List of uint8 HWC CUDA tensors (h_i, w_i, 3) of different sizes -> (B, D) descriptors in ONE network pass.
+        The images are packed into the top-left corners of (max h_i, max w_i) slots; row i equals, bit for bit, the
+        descriptor of forward_u8 on image i alone (dirb200_net_forward_ragged_u8)."""
+        if not imgs or any(not (x.is_cuda and x.dtype == torch.uint8 and x.dim() == 3 and x.shape[2] == 3) for x in imgs):
+            raise TypeError("expected a non-empty list of (h,w,3) uint8 CUDA tensors")
+        hw = [(int(x.shape[0]), int(x.shape[1])) for x in imgs]
+        slots = imgs[0].new_zeros((len(imgs), max(h for h, _ in hw), max(w for _, w in hw), 3))
+        for i, x in enumerate(imgs):
+            slots[i, :hw[i][0], :hw[i][1]] = x
+        return self.forward_ragged_slots(slots, hw)
+
+    def forward_ragged(self, imgs):
+        """List of normalised (3, h_i, w_i) fp32 tensors -> (B, D) descriptors in one pass (dirb200_net_forward_ragged);
+        row i equals forward() on image i alone, bit for bit."""
+        if not imgs or any(not (isinstance(x, torch.Tensor) and x.dim() == 3 and x.shape[0] == 3) for x in imgs):
+            raise TypeError("expected a non-empty list of (3,h,w) tensors")
+        hw = [(int(x.shape[1]), int(x.shape[2])) for x in imgs]
+        dev = imgs[0].device if imgs[0].is_cuda else torch.device("cuda")
+        slots = torch.zeros((len(imgs), 3, max(h for h, _ in hw), max(w for _, w in hw)), dtype=torch.float32, device=dev)
+        for i, x in enumerate(imgs):
+            slots[i, :, :hw[i][0], :hw[i][1]] = x
+        return self.forward_ragged_slots(slots, hw)
+
+    def forward_ragged_slots(self, slots, hw, want_f16=False):
+        """Already packed slots - uint8 (B,H,W,3) or normalised fp32 (B,3,H,W) CUDA tensor - with the images' sizes
+        hw = [(h_i, w_i)]; content outside the sizes is ignored.  -> (B, D) fp32 (and fp16 with want_f16)."""
+        u8 = slots.dtype == torch.uint8
+        if not slots.is_cuda or slots.dim() != 4 or (slots.shape[3] if u8 else slots.shape[1]) != 3:
+            raise TypeError("expected (B,H,W,3) uint8 or (B,3,H,W) fp32 CUDA slots")
+        x = slots.contiguous() if u8 else slots.contiguous().float()
+        b = int(x.shape[0])
+        hgt, wid = (int(x.shape[1]), int(x.shape[2])) if u8 else (int(x.shape[2]), int(x.shape[3]))
+        if len(hw) != b:
+            raise ValueError("need one (h, w) per slot")
+        table = np.ascontiguousarray(np.asarray(hw, dtype=np.int32).reshape(b, 2))
+        h = self._ensure_with_preprocess(x.device.index or 0) if u8 else self._ensure(x.device.index or 0)
+        with torch.cuda.device(x.device):
+            desc = torch.empty((b, self.descriptor_dim), dtype=torch.float32, device=x.device)
+            d16 = torch.empty((b, self.descriptor_dim), dtype=torch.float16, device=x.device) if want_f16 else None
+            lib.call("dirb200_net_forward_ragged_u8" if u8 else "dirb200_net_forward_ragged", h, C.c_void_p(x.data_ptr()),
+                     b, hgt, wid, table.ctypes.data_as(C.c_void_p), C.c_void_p(desc.data_ptr()),
+                     C.c_void_p(d16.data_ptr()) if want_f16 else C.c_void_p(0),
+                     C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        return (desc, d16) if want_f16 else desc
+
     def forward_u8_multiscale(self, imgs_u8: torch.Tensor, scales=(0.7, 1.0, 1.4), pooling="gem", gemp=3):
         """Multi-scale descriptors entirely on the GPU (BASELINE configs[4]): for every scale s the uint8 batch is
         resized like the reference's `Scale(s)` transform (PIL bilinear, output size int(0.5 + s*w), bit-exact on the

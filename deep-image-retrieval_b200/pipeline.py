@@ -103,6 +103,56 @@ def _gpu_chain_scale(transforms):
     return s if 0 < s <= 4 else None
 
 
+# Mixed-size extraction in batches: decoded images are collected in windows of RAGGED_WINDOW x batch_size, and each
+# window is cut into network passes (ragged_groups) run by the ragged forward, which pads every image of a pass to
+# the pass's largest height and width and masks the padding out.  A pass's padded area B * H * W stays within
+# RAGGED_AREA_BOUND x the sum of its images' true areas.
+RAGGED_WINDOW = 4
+RAGGED_AREA_BOUND = (5, 4)          # 1.25 as an exact ratio: 4 * B * H * W <= 5 * sum(h * w)
+
+
+def ragged_groups(sizes, batch_size):
+    """Cut images of sizes [(h, w), ...] into network passes: sorted by shape, then greedily grouped into runs of at
+    most batch_size images whose padded area (len * max h * max w) is at most 1.25 x the sum of their areas.
+    -> list of lists of indices into `sizes`; every index appears exactly once."""
+    num, den = RAGGED_AREA_BOUND
+    order = sorted(range(len(sizes)), key=lambda i: (int(sizes[i][0]), int(sizes[i][1]), i))
+    groups, cur, hmax, wmax, area = [], [], 0, 0, 0
+    for i in order:
+        h, w = int(sizes[i][0]), int(sizes[i][1])
+        nh, nw, na = max(hmax, h), max(wmax, w), area + h * w
+        if cur and (len(cur) >= batch_size or den * (len(cur) + 1) * nh * nw > num * na):
+            groups.append(cur)
+            cur, nh, nw, na = [], h, w, h * w
+        cur.append(i)
+        hmax, wmax, area = nh, nw, na
+    if cur:
+        groups.append(cur)
+    return groups
+
+
+def _ragged_window(net, imgs, batch_size):
+    """Descriptors (len(imgs), D), in order, of one window of preprocessed images on the GPU: uint8 HWC (h,w,3) or
+    normalised fp32 CHW (3,h,w), through ragged_groups passes of the ragged forward."""
+    u8 = imgs[0].dtype == torch.uint8
+    sizes = [(int(x.shape[0]), int(x.shape[1])) if u8 else (int(x.shape[1]), int(x.shape[2])) for x in imgs]
+    out = [None] * len(imgs)
+    for g in ragged_groups(sizes, batch_size):
+        hh, ww = max(sizes[i][0] for i in g), max(sizes[i][1] for i in g)
+        # slot content outside an image is ignored by the forward: no need to clear it
+        slots = imgs[g[0]].new_empty((len(g), hh, ww, 3) if u8 else (len(g), 3, hh, ww))
+        for k, i in enumerate(g):
+            h, w = sizes[i]
+            if u8:
+                slots[k, :h, :w] = imgs[i]
+            else:
+                slots[k, :, :h, :w] = imgs[i]
+        d = net.forward_ragged_slots(slots, [sizes[i] for i in g])
+        for k, i in enumerate(g):
+            out[i] = d[k:k + 1]
+    return torch.cat(out, dim=0)
+
+
 class _RawImages(torch.utils.data.Dataset):
     """Decoded images as uint8 HWC tensors (the decode stays on CPU workers; everything after it runs on the GPU)."""
 
@@ -122,7 +172,14 @@ def extract_image_features(dataset, transforms, net, ret_imgs=False, same_size=F
     gpu_preprocess (extension): when the chain is '' or 'Scale(<float>)' and images go through one by one, resize
     (byte-identical to PIL bilinear), ToTensor and Normalize run on the GPU from the decoded uint8 pixels
     (dirb200_resize_bilinear_u8 + dirb200_net_forward_u8) - bit-identical descriptors, no PIL resize / float
-    conversion on the host and 4x fewer bytes over PCIe."""
+    conversion on the host and 4x fewer bytes over PCIe.
+    Images of different sizes (no Pad / Crop in the chain) go through the network batch_size at a time as ragged
+    batches (ragged_groups, ResNetRMAC.forward_ragged_slots): the same descriptors, bit for bit, as one image per call,
+    which is what batch_size = 1 and FPN networks (whose head depends on each image's size) still do."""
+    ragged = (not same_size and not ret_imgs and batch_size > 1 and hasattr(net, "forward_ragged_slots")
+              and not getattr(net, "fpn", False))
+    group = batch_size if ragged else 1
+    window = RAGGED_WINDOW * group
     if not same_size:
         batch_size = 1
     scale = _gpu_chain_scale(transforms) if (gpu_preprocess and not same_size and not ret_imgs and hasattr(net, "forward_u8")) else None
@@ -131,7 +188,7 @@ def extract_image_features(dataset, transforms, net, ret_imgs=False, same_size=F
     if scale is not None:
         loader = torch.utils.data.DataLoader(_RawImages(dataset), batch_size=None, shuffle=False,
                                              num_workers=max(0, threads if threads > 1 else 0), pin_memory=True)
-        img_feats = []
+        img_feats, pending = [], []
         for img in tqdm.tqdm(loader, desc, total=len(dataset)):
             x = img.cuda(non_blocking=True)
             if flip and flip.pop(0):
@@ -141,25 +198,41 @@ def extract_image_features(dataset, transforms, net, ret_imgs=False, same_size=F
             x = x.unsqueeze(0).contiguous()
             if (oh, ow) != (h, w) and min(oh, ow) != min(h, w):          # Scale.__call__: can_upscale / can_downscale
                 x = ops.resize_bilinear_u8(x, (oh, ow))
+            if ragged:
+                pending.append(x[0])
+                if len(pending) == window:
+                    img_feats.append(_ragged_window(net, pending, group))
+                    pending = []
+                continue
             d = net.forward_u8(x)
             img_feats.append(d.unsqueeze(0) if d.dim() == 1 else d)
+        if pending:
+            img_feats.append(_ragged_window(net, pending, group))
         return torch.cat(img_feats, dim=0)
     loader = get_loader(dataset, trf_chain=transforms, preprocess=net.preprocess, iscuda=iscuda, output=["img"],
                         batch_size=batch_size, threads=threads, shuffle=False)
     tocpu = (lambda x: x.cpu()) if ret_imgs == "cpu" else (lambda x: x)
-    img_feats, trf_images = [], []
+    img_feats, trf_images, pending = [], [], []
     for inputs in tqdm.tqdm(loader, desc, total=1 + (len(dataset) - 1) // batch_size):
         imgs = inputs[0]
         for i in range(len(imgs)):
             if flip and flip.pop(0):
                 imgs[i] = imgs[i].flip(2)
         imgs = common.variables(inputs[:1], net.iscuda)[0]
+        if ragged:
+            pending.extend(imgs[i].float().cuda() for i in range(len(imgs)))
+            if len(pending) >= window:
+                img_feats.append(_ragged_window(net, pending, group))
+                pending = []
+            continue
         d = net(imgs)
         if ret_imgs:
             trf_images.append(tocpu(imgs))
         if d.dim() == 1:
             d = d.unsqueeze(0)
         img_feats.append(d)
+    if pending:
+        img_feats.append(_ragged_window(net, pending, group))
     img_feats = torch.cat(img_feats, dim=0)
     if ret_imgs:
         if same_size:

@@ -98,6 +98,17 @@ int dirb200_net_forward_host(dirb200_net* net, const float* imgs_host, int B, in
 int dirb200_net_forward_u8(dirb200_net* net, const uint8_t* imgs_dev, int B, int H, int W, float* desc_dev,
                            void* desc16_dev, void* stream);
 int dirb200_net_forward_host_u8(dirb200_net* net, const uint8_t* imgs_host, int B, int H, int W, float* desc_host);
+/* Ragged batch: B images of different sizes in one network pass (test_dir.py:47-94 feeds them one per call,
+ * test_dir.py:52-53).  Image i (hw_host[i] = {h_i, w_i}, host memory) sits in the top-left corner of slot i of one
+ * (H, W) slot tensor: uint8 HWC (B,H,W,3) for the _u8 entry point, normalised NCHW fp32 (B,3,H,W) for the other.
+ * Slot content outside the images is ignored, whatever it holds.  Every activation outside an image's extent is 0
+ * and the head pools over the image's own pixels, so desc_dev row i (and desc16_dev, optional) equals, bit for bit,
+ * the descriptor of a B = 1 forward of image i alone.  Needs 32 <= h_i <= H and 32 <= w_i <= W (else
+ * DIRB200_EINVAL); FPN heads and conv_impl 1 return DIRB200_ENOTSUP. */
+int dirb200_net_forward_ragged_u8(dirb200_net* net, const uint8_t* slots_dev, int B, int H, int W, const int* hw_host,
+                                  float* desc_dev, void* desc16_dev, void* stream);
+int dirb200_net_forward_ragged(dirb200_net* net, const float* slots_dev, int B, int H, int W, const int* hw_host,
+                               float* desc_dev, void* desc16_dev, void* stream);
 /* Bilinear resize of uint8 HWC RGB images (B,H,W,3) -> (B,Ho,Wo,3), byte-identical to PIL's
  * Image.resize((Wo,Ho), Image.BILINEAR) - the `Scale` transform of dirtorch/utils/transforms.py:133-185 - so that
  * multi-scale extraction (Scale(0.7), Scale(1.4)) can stay on the GPU in front of dirb200_net_forward_u8.
