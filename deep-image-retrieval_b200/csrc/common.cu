@@ -24,6 +24,16 @@ const char* last_error() { return g_err; }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int64_t launches_total() { return g_launches.load(std::memory_order_relaxed); }
 
+int grow_device(void** p, size_t* cap, size_t need) {
+  if (need <= *cap) return 0;
+  if (*p) DIRB_CUDA(cudaFree(*p));
+  *p = nullptr;
+  *cap = 0;
+  DIRB_CUDA(cudaMalloc(p, need));
+  *cap = need;
+  return 0;
+}
+
 // cuTensorMapEncodeTiled is a driver-API symbol; resolve it through the runtime so the library has no
 // link-time dependency on libcuda.so (it must load on a box without a driver for the build/ABI checks).
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

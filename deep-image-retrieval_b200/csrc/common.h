@@ -39,6 +39,11 @@ const char* last_error();
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// Grow the device buffer *p of *cap bytes to `need` bytes (contents are not kept; no-op when it is large enough).
+// Pointer and capacity are cleared before the allocation and the capacity is set only once it succeeded, so after a
+// failed call the buffer is empty rather than a null pointer with a stale capacity.
+int grow_device(void** p, size_t* cap, size_t need);
+
 // fp16 row-major [outer][inner] matrix, box = box_inner x box_outer elements, 128-byte swizzle.
 int encode_tmap_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
                    uint32_t box_inner, uint32_t box_outer);

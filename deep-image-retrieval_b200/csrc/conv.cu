@@ -71,6 +71,32 @@ struct PersStages {
   static constexpr int SIM = 6;
 };
 
+static int set_total_tiles(ConvPersParams& p, int64_t total) {
+  DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
+  p.total_tiles = static_cast<int>(total);
+  return 0;
+}
+
+// Convolution epilogue on the persistent kernel; the RAGGED instantiation when the launch carries image extents.
+template <int BN, int STAGES, bool HALO>
+static int launch_conv_pers(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO,
+                            ConvPersParams& p, int64_t total, int grid_limit, cudaStream_t stream) {
+  DIRB_TRY(set_total_tiles(p, total));
+  if (p.ext != nullptr)
+    return conv_pers_launch<BN, STAGES, PERS_EPI_CONV, HALO, true>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
+  return conv_pers_launch<BN, STAGES, PERS_EPI_CONV, HALO>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
+}
+
+template <int CM>
+static int launch_c23(const CUtensorMap& tmA, const CUtensorMap& tmB2, const CUtensorMap& tmB3, const CUtensorMap& tmR,
+                      const CUtensorMap& tmO, ConvPersParams& p, int64_t total, const float* scale2, const float* shift2,
+                      cudaStream_t stream) {
+  DIRB_TRY(set_total_tiles(p, total));
+  if (p.ext != nullptr)
+    return conv_c23_launch<CM, true>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
+  return conv_c23_launch<CM>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
+}
+
 template <int BN>
 static int conv_pers_bn(const ConvShape& s, const __half* in, const __half* w, const float* scale, const float* shift,
                         const __half* res, int relu, __half* out, cudaStream_t stream, int grid_limit,
@@ -116,12 +142,7 @@ static int conv_pers_bn(const ConvShape& s, const __half* in, const __half* w, c
   }
   if (!res) tmR = tmO;   // (never dereferenced without a residual)
   DIRB_TRY(encode_tmap_2d(&tmB, w, Ktot, s.Cout, (uint64_t)Ktot * 2, 64, BN));
-  const int64_t total = m_tiles * p.n_tiles;
-  DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
-  p.total_tiles = static_cast<int>(total);
-  if (p.ext != nullptr)
-    return conv_pers_launch<BN, PersStages<BN>::CONV, PERS_EPI_CONV, false, true>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
-  return conv_pers_launch<BN, PersStages<BN>::CONV, PERS_EPI_CONV>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
+  return launch_conv_pers<BN, PersStages<BN>::CONV, false>(tmA, tmB, tmR, tmO, p, m_tiles * p.n_tiles, grid_limit, stream);
 }
 
 // 3x3 / stride 1 / pad 1 with the input patch loaded once per 64-channel block (HALO mode of conv_pers.cuh).
@@ -142,18 +163,14 @@ static int conv_halo_bn(const ConvShape& s, const __half* in, const __half* w, c
   p.scale = scale;
   p.shift = shift;
   set_ext(p, ext, s.H, s.W);
-  const int64_t total = (int64_t)p.tiles_w * p.tiles_h * s.B * p.n_tiles;
-  DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
-  p.total_tiles = static_cast<int>(total);
   CUtensorMap tmA, tmB, tmR, tmO;
   DIRB_TRY(encode_tmap_nhwc_halo(&tmA, in, s.B, s.H, s.W, s.Cin));
   DIRB_TRY(encode_tmap_nhwc(&tmO, out, s.B, s.H, s.W, s.Cout, 8, 16, 1, 1));
   if (res) DIRB_TRY(encode_tmap_nhwc(&tmR, res, s.B, s.H, s.W, s.Cout, 8, 16, 1, 1));
   else tmR = tmO;
   DIRB_TRY(encode_tmap_2d(&tmB, w, 9 * s.Cin, s.Cout, (uint64_t)9 * s.Cin * 2, 64, BN));
-  if (p.ext != nullptr)
-    return conv_pers_launch<BN, BN == 128 ? 6 : 8, PERS_EPI_CONV, true, true>(tmA, tmB, tmR, tmO, p, num_sms(), stream);
-  return conv_pers_launch<BN, BN == 128 ? 6 : 8, PERS_EPI_CONV, true>(tmA, tmB, tmR, tmO, p, num_sms(), stream);
+  return launch_conv_pers<BN, BN == 128 ? 6 : 8, true>(tmA, tmB, tmR, tmO, p, (int64_t)p.tiles_w * p.tiles_h * s.B * p.n_tiles,
+                                                       num_sms(), stream);
 }
 
 // Tile width (output channels per tile): 128 unless that would leave SMs without a tile - at batch 1-8 a wide tile
@@ -211,17 +228,14 @@ int conv_fused_ds(int B, int Ho, int Wo, int Cmid, const __half* t2, int Hx, int
   p.scale = scale;
   p.shift = shift;
   set_ext(p, ext, Ho, Wo);
-  const int64_t total = (int64_t)p.tiles_w * p.tiles_h * ceil_div(B, p.nb) * p.n_tiles;
-  DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
-  p.total_tiles = static_cast<int>(total);
   CUtensorMap tmA, tmB, tmX, tmO;
   DIRB_TRY(encode_tmap_nhwc(&tmA, t2, B, Ho, Wo, Cmid, p.tw, p.th, p.nb, 1));
   DIRB_TRY(encode_tmap_nhwc(&tmX, x, B, Hx, Wx, Cx, p.tw, p.th, p.nb, xstride));
   DIRB_TRY(encode_tmap_nhwc(&tmO, out, B, Ho, Wo, Cout, p.tw, p.th, p.nb, 1));
   DIRB_TRY(encode_tmap_2d(&tmB, wcat, Cmid + Cx, Cout, (uint64_t)(Cmid + Cx) * 2, 64, BN));
-  if (p.ext != nullptr)
-    return conv_pers_launch<BN, PersStages<BN>::CONV, PERS_EPI_CONV, false, true>(tmA, tmB, tmX, tmO, p, num_sms(), stream);
-  return conv_pers_launch<BN, PersStages<BN>::CONV, PERS_EPI_CONV>(tmA, tmB, tmX, tmO, p, num_sms(), stream);
+  return launch_conv_pers<BN, PersStages<BN>::CONV, false>(tmA, tmB, tmX, tmO, p,
+                                                           (int64_t)p.tiles_w * p.tiles_h * ceil_div(B, p.nb) * p.n_tiles,
+                                                           num_sms(), stream);
 }
 
 // Bottleneck conv2 (3x3/s1/p1) + BN + ReLU + conv3 (1x1, x4) + BN + residual + ReLU in one kernel (conv_c23.cuh).
@@ -247,22 +261,15 @@ int conv_c23(int B, int H, int W, int Cm, const __half* t1, const __half* w2, co
   p.shift = shift3;
   set_ext(p, ext, H, W);
   const int64_t total = (int64_t)p.tiles_w * p.tiles_h * B;
-  DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
-  p.total_tiles = static_cast<int>(total);
   CUtensorMap tmA, tmB2, tmB3, tmR, tmO;
   DIRB_TRY(encode_tmap_nhwc_halo(&tmA, t1, B, H, W, Cm));
   DIRB_TRY(encode_tmap_2d(&tmB2, w2, 9 * Cm, Cm, (uint64_t)9 * Cm * 2, 64, Cm < 128 ? Cm : 128));
   DIRB_TRY(encode_tmap_2d(&tmB3, w3, Cm, 4 * Cm, (uint64_t)Cm * 2, 64, 128));
   DIRB_TRY(encode_tmap_nhwc(&tmR, res, B, H, W, 4 * Cm, 8, 16, 1, 1));
   DIRB_TRY(encode_tmap_nhwc(&tmO, out, B, H, W, 4 * Cm, 8, 16, 1, 1));
-  if (p.ext != nullptr) {
-    if (Cm == 256) return conv_c23_launch<256, true>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
-    if (Cm == 64) return conv_c23_launch<64, true>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
-    return conv_c23_launch<128, true>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
-  }
-  if (Cm == 256) return conv_c23_launch<256>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
-  if (Cm == 64) return conv_c23_launch<64>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
-  return conv_c23_launch<128>(tmA, tmB2, tmB3, tmR, tmO, p, scale2, shift2, num_sms(), stream);
+  if (Cm == 256) return launch_c23<256>(tmA, tmB2, tmB3, tmR, tmO, p, total, scale2, shift2, stream);
+  if (Cm == 64) return launch_c23<64>(tmA, tmB2, tmB3, tmR, tmO, p, total, scale2, shift2, stream);
+  return launch_c23<128>(tmA, tmB2, tmB3, tmR, tmO, p, total, scale2, shift2, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ stem

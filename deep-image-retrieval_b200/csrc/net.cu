@@ -117,8 +117,6 @@ struct dirb200_net {
   ConvLayer fpn_lat, fpn_smooth;  // conv1x5 (1x1, C4 -> C3), conv3c4 (3x3, C3 -> C3): no BN, ReLU after each
   int feat_in() const { return fpn ? stage_ch[3] + stage_ch[4] : stage_ch[4]; }     // fc.in_features
   int desc_dim() const { return without_fc ? feat_in() : out_dim; }
-  int sub[5] = {0, 0, 0, 0, 0};   // images per sub-chunk of stage 0..4 (0 = auto)
-  int stage_sched = 0;            // 0 = every stage over the whole chunk (fastest measured), 1 = per-stage sub-chunks
   // ragged entry points: device copy of the extent table (see RG_LD)
   int* ext_dev = nullptr;
   size_t ext_bytes = 0;
@@ -153,12 +151,7 @@ static int record_tap(dirb200_net* n, const std::string& name, const __half* src
   if (!n->debug_taps) return 0;
   const size_t bytes = static_cast<size_t>(nb) * h * w * c * 2;
   auto& t = n->taps[name];
-  if (t.cap < bytes) {
-    if (t.ptr) DIRB_CUDA(cudaFree(t.ptr));
-    t.ptr = nullptr;
-    DIRB_CUDA(cudaMalloc(reinterpret_cast<void**>(&t.ptr), bytes));
-    t.cap = bytes;
-  }
+  DIRB_TRY(grow_device(reinterpret_cast<void**>(&t.ptr), &t.cap, bytes));
   t.n = nb; t.h = h; t.w = w; t.c = c;
   DIRB_CUDA(cudaMemcpyAsync(t.ptr, src, bytes, cudaMemcpyDeviceToDevice, stream));
   return 0;
@@ -173,15 +166,27 @@ static int get_tensor(dirb200_net* n, const std::string& name, const HostTensor*
   return 0;
 }
 
-// OIHW fp32 -> [Cout][KH][KW][CinPad] fp16 rows padded to Kpad; BN -> (scale, shift).
-static int pack_conv(dirb200_net* n, ConvLayer& L) {
-  const HostTensor *w, *g, *b, *m, *v;
+// OIHW fp32 -> [Cout][KH][KW][CinPad] fp16 rows padded to Kpad; BN -> (scale, shift), also returned through
+// sc_host / sh_host when given.  An empty BN prefix (the FPN convolutions) means scale 1, shift 0.
+static int pack_conv(dirb200_net* n, ConvLayer& L, std::vector<float>* sc_host = nullptr,
+                     std::vector<float>* sh_host = nullptr) {
+  const HostTensor* w;
   const size_t kk = static_cast<size_t>(L.K) * L.K;
   DIRB_TRY(get_tensor(n, L.conv + ".weight", &w, static_cast<size_t>(L.Cout) * L.Cin * kk));
-  DIRB_TRY(get_tensor(n, L.bn + ".weight", &g, L.Cout));
-  DIRB_TRY(get_tensor(n, L.bn + ".bias", &b, L.Cout));
-  DIRB_TRY(get_tensor(n, L.bn + ".running_mean", &m, L.Cout));
-  DIRB_TRY(get_tensor(n, L.bn + ".running_var", &v, L.Cout));
+  std::vector<float> sc(L.Cout, 1.0f), sh(L.Cout, 0.0f);
+  if (!L.bn.empty()) {
+    const HostTensor *g, *b, *m, *v;
+    DIRB_TRY(get_tensor(n, L.bn + ".weight", &g, L.Cout));
+    DIRB_TRY(get_tensor(n, L.bn + ".bias", &b, L.Cout));
+    DIRB_TRY(get_tensor(n, L.bn + ".running_mean", &m, L.Cout));
+    DIRB_TRY(get_tensor(n, L.bn + ".running_var", &v, L.Cout));
+    for (int o = 0; o < L.Cout; ++o) {
+      // BatchNorm2d eval: y = (x - mean) / sqrt(var + 1e-5) * gamma + beta   (eps: torch default, resnet.py:57)
+      const float s = g->data[o] / sqrtf(v->data[o] + 1e-5f);
+      sc[o] = s;
+      sh[o] = b->data[o] - m->data[o] * s;
+    }
+  }
   L.CinPad = (L.Cin % 8 == 0) ? L.Cin : ((L.Cin + 7) / 8 * 8);
   const int Ktot = L.K * L.K * L.CinPad;
   L.Kpad = (Ktot + 31) / 32 * 32;
@@ -192,44 +197,14 @@ static int pack_conv(dirb200_net* n, ConvLayer& L) {
         for (int kw = 0; kw < L.K; ++kw)
           hw[static_cast<size_t>(o) * L.Kpad + (static_cast<size_t>(kh) * L.K + kw) * L.CinPad + c] =
               __float2half_rn(w->data[((static_cast<size_t>(o) * L.Cin + c) * L.K + kh) * L.K + kw]);
-  std::vector<float> sc(L.Cout), sh(L.Cout);
-  for (int o = 0; o < L.Cout; ++o) {
-    // BatchNorm2d eval: y = (x - mean) / sqrt(var + 1e-5) * gamma + beta   (eps: torch default, resnet.py:57)
-    const float s = g->data[o] / sqrtf(v->data[o] + 1e-5f);
-    sc[o] = s;
-    sh[o] = b->data[o] - m->data[o] * s;
-  }
   DIRB_TRY(dev_alloc(n, reinterpret_cast<void**>(&L.w), hw.size() * sizeof(__half)));
   DIRB_TRY(dev_alloc(n, reinterpret_cast<void**>(&L.scale), L.Cout * sizeof(float)));
   DIRB_TRY(dev_alloc(n, reinterpret_cast<void**>(&L.shift), L.Cout * sizeof(float)));
   DIRB_CUDA(cudaMemcpy(L.w, hw.data(), hw.size() * sizeof(__half), cudaMemcpyHostToDevice));
   DIRB_CUDA(cudaMemcpy(L.scale, sc.data(), L.Cout * sizeof(float), cudaMemcpyHostToDevice));
   DIRB_CUDA(cudaMemcpy(L.shift, sh.data(), L.Cout * sizeof(float), cudaMemcpyHostToDevice));
-  return 0;
-}
-
-// Convolution without BatchNorm (FPN lateral / smoothing convs): scale = 1, shift = 0.
-static int pack_conv_plain(dirb200_net* n, ConvLayer& L) {
-  const HostTensor* w;
-  const size_t kk = static_cast<size_t>(L.K) * L.K;
-  DIRB_TRY(get_tensor(n, L.conv + ".weight", &w, static_cast<size_t>(L.Cout) * L.Cin * kk));
-  L.CinPad = L.Cin;
-  const int Ktot = L.K * L.K * L.CinPad;
-  L.Kpad = (Ktot + 31) / 32 * 32;
-  std::vector<__half> hw(static_cast<size_t>(L.Cout) * L.Kpad, __float2half(0.f));
-  for (int o = 0; o < L.Cout; ++o)
-    for (int c = 0; c < L.Cin; ++c)
-      for (int kh = 0; kh < L.K; ++kh)
-        for (int kw = 0; kw < L.K; ++kw)
-          hw[static_cast<size_t>(o) * L.Kpad + (static_cast<size_t>(kh) * L.K + kw) * L.CinPad + c] =
-              __float2half_rn(w->data[((static_cast<size_t>(o) * L.Cin + c) * L.K + kh) * L.K + kw]);
-  std::vector<float> sc(L.Cout, 1.0f), sh(L.Cout, 0.0f);
-  DIRB_TRY(dev_alloc(n, reinterpret_cast<void**>(&L.w), hw.size() * sizeof(__half)));
-  DIRB_TRY(dev_alloc(n, reinterpret_cast<void**>(&L.scale), L.Cout * sizeof(float)));
-  DIRB_TRY(dev_alloc(n, reinterpret_cast<void**>(&L.shift), L.Cout * sizeof(float)));
-  DIRB_CUDA(cudaMemcpy(L.w, hw.data(), hw.size() * sizeof(__half), cudaMemcpyHostToDevice));
-  DIRB_CUDA(cudaMemcpy(L.scale, sc.data(), L.Cout * sizeof(float), cudaMemcpyHostToDevice));
-  DIRB_CUDA(cudaMemcpy(L.shift, sh.data(), L.Cout * sizeof(float), cudaMemcpyHostToDevice));
+  if (sc_host) *sc_host = std::move(sc);
+  if (sh_host) *sh_host = std::move(sh);
   return 0;
 }
 
@@ -354,8 +329,6 @@ int dirb200_net_set_option(dirb200_net* n, const char* key, double value) {
   else if (is_global_option(k)) return dirb200_set_global_option(key, value);   // process-wide kernel selectors
   else if (k.size() == 5 && k.compare(0, 4, "mean") == 0 && k[4] >= '0' && k[4] <= '2') n->mean_std[k[4] - '0'] = static_cast<float>(value);
   else if (k.size() == 4 && k.compare(0, 3, "std") == 0 && k[3] >= '0' && k[3] <= '2') n->mean_std[3 + k[3] - '0'] = static_cast<float>(value);
-  else if (k == "stage_sched") n->stage_sched = static_cast<int>(value);
-  else if (k.size() == 4 && k.compare(0, 3, "sub") == 0 && k[3] >= '0' && k[3] <= '4') n->sub[k[3] - '0'] = static_cast<int>(value);
   else if (k == "host_chunk") n->host_chunk = std::max(1, static_cast<int>(value));
   else DIRB_REQUIRE(false, DIRB200_EKEY, "unknown net option '%s'", key);
   return 0;
@@ -420,22 +393,19 @@ int dirb200_net_finalize(dirb200_net* n) {
       blk.c2 = make_layer(p + "conv2", p + "bn2", planes, planes, 3, stride, 1);     // stride on conv2, resnet.py:58
       blk.c3 = make_layer(p + "conv3", p + "bn3", planes, planes * 4, 1, 1, 0);
       blk.has_down = (b == 0);                                                     // resnet.py:136-141
+      std::vector<float> s3, sh3;
       DIRB_TRY(pack_conv(n, blk.c1));
       DIRB_TRY(pack_conv(n, blk.c2));
-      DIRB_TRY(pack_conv(n, blk.c3));
+      DIRB_TRY(pack_conv(n, blk.c3, &s3, &sh3));
       if (blk.has_down) {
         blk.down = make_layer(p + "downsample.0", p + "downsample.1", inplanes, planes * 4, 1, stride, 0);
-        DIRB_TRY(pack_conv(n, blk.down));
+        std::vector<float> sd, shd;
+        DIRB_TRY(pack_conv(n, blk.down, &sd, &shd));
         // K-concatenated, BN-scaled weights for the fused conv3 + shortcut
         const HostTensor *w3, *wd;
         const int kcat = planes + inplanes;
         DIRB_TRY(get_tensor(n, p + "conv3.weight", &w3, static_cast<size_t>(cout) * planes));
         DIRB_TRY(get_tensor(n, p + "downsample.0.weight", &wd, static_cast<size_t>(cout) * inplanes));
-        std::vector<float> s3(cout), sh3(cout), sd(cout), shd(cout);
-        DIRB_CUDA(cudaMemcpy(s3.data(), blk.c3.scale, cout * 4, cudaMemcpyDeviceToHost));
-        DIRB_CUDA(cudaMemcpy(sh3.data(), blk.c3.shift, cout * 4, cudaMemcpyDeviceToHost));
-        DIRB_CUDA(cudaMemcpy(sd.data(), blk.down.scale, cout * 4, cudaMemcpyDeviceToHost));
-        DIRB_CUDA(cudaMemcpy(shd.data(), blk.down.shift, cout * 4, cudaMemcpyDeviceToHost));
         std::vector<__half> wc(static_cast<size_t>(cout) * kcat);
         std::vector<float> shc(cout), one(cout, 1.0f);
         for (int o = 0; o < cout; ++o) {
@@ -467,8 +437,8 @@ int dirb200_net_finalize(dirb200_net* n) {
     if (n->fpn_mode == 1) {                                                       // rmac_resnet_fpn.py:27-30
       n->fpn_lat = make_layer("conv1x5", "", n->stage_ch[4], n->stage_ch[3], 1, 1, 0);
       n->fpn_smooth = make_layer("conv3c4", "", n->stage_ch[3], n->stage_ch[3], 3, 1, 1);
-      DIRB_TRY(pack_conv_plain(n, n->fpn_lat));
-      DIRB_TRY(pack_conv_plain(n, n->fpn_smooth));
+      DIRB_TRY(pack_conv(n, n->fpn_lat));
+      DIRB_TRY(pack_conv(n, n->fpn_smooth));
     }
   } else if (n->pooling == 0) {
     const HostTensor* p;
@@ -494,7 +464,7 @@ int dirb200_net_finalize(dirb200_net* n) {
 
 static int auto_chunk(int B, int H, int W) {
   // Large chunks keep every launch at many tiles per SM (the persistent kernels lose ~1/waves to the tail);
-  // bound the activation workspace to ~24 GB of the 180 GB HBM.
+  // bound the activation workspace to ~24 GB of the 80 GB HBM.
   const double per_img = 2.0 * (static_cast<double>(H) * W * 8 + (H / 2.0) * (W / 2.0) * 64 + 5.0 * (H / 4.0) * (W / 4.0) * 256);
   int c = static_cast<int>(24e9 / per_img);
   if (c < 1) c = 1;
@@ -503,42 +473,57 @@ static int auto_chunk(int B, int H, int W) {
   return c;
 }
 
+// Resolution levels of the network: 0 = input, 1 = stem convolution output, 2 + s = output of stage s (0 maxpool,
+// 1..4 layer1..4).  The workspace, the launch schedule and the extent table of ragged batches all take their sizes
+// from level_sizes, which is what makes a ragged batch bit-identical to B = 1 forwards.
+constexpr int RG_LEVELS = 7, RG_LD = 4 * RG_LEVELS;
+
 namespace {
-// Stage schedule.  The network is cut into 5 stages: 0 = stem + maxpool, 1..4 = layer1..layer4 (+ head after 4).
-// A stage runs over the chunk in sub-chunks of sub[s] images: the tensors passed between the blocks of a stage are
-// then small enough to stay in the 50 MB L2, while the stage outputs of the whole chunk live in HBM buffers.
+struct LevelSizes {
+  int h[RG_LEVELS], w[RG_LEVELS];
+};
+
+// Activation buffers of one pass of the network over up to `chunk` images; every stage runs over the whole pass.
 struct Workspace {
-  __half* stem_ws;        // s2d / nhwc8 staging of one stem sub-chunk
-  __half* stem_out;       // stem conv output of one sub-chunk (before the maxpool)
-  __half* stage_out[4];   // outputs of stage 0..3 for the whole chunk
+  __half* stem_ws;        // s2d / nhwc8 staging of the stem input
+  __half* stem_out;       // stem conv output (before the maxpool)
+  __half* stage_out[4];   // outputs of stage 0..3
   __half* scratch[4];     // rotating tensors inside a stage
   float* head_ws;
-  int H1, W1;             // stem conv output size
-  int h[5], w[5];         // spatial size of the output of stage 0..4
-  int sub[5];
+  int chunk;
+  LevelSizes sz;          // of the slot shape H x W
 };
 }  // namespace
+
+static LevelSizes level_sizes(int H, int W) {
+  LevelSizes z;
+  z.h[0] = H;
+  z.w[0] = W;
+  for (int l = 1; l < RG_LEVELS; ++l) {
+    int h = z.h[l - 1], w = z.w[l - 1];
+    if (l == 1) { h = (h + 6 - 7) / 2 + 1; w = (w + 6 - 7) / 2 + 1; }           // stem conv 7x7/s2/p3
+    else if (l != 3) { h = (h + 2 - 3) / 2 + 1; w = (w + 2 - 3) / 2 + 1; }     // maxpool, layer2..4 (layer1: stride 1)
+    z.h[l] = h;
+    z.w[l] = w;
+  }
+  return z;
+}
 
 // Ragged batches: B pictures of sizes (h_i, w_i) in the top-left corners of B slots of one shape (H, W).  Every kernel
 // writes 0 outside a picture (what zero padding feeds its border) and the head pools over the picture's own pixels,
 // so each descriptor equals, bit for bit, the one of a B = 1 forward of the picture at its own size.  The extent table
-// holds per picture and resolution level one row {h, w, plain, block}: level 0 = input, 1 = stem convolution output,
-// 2 + s = output of stage s (0 maxpool, 1..4 layer1..4), sizes from the formulas of setup_workspace.  plain / block =
-// the K order (1 = HALO order, 0 = tap by tap) that a B = 1 forward gives a 3x3 stride-1 convolution at that level,
-// standalone / as conv2 of an identity Bottleneck (which fuse_c23 may take).  Where a pass's pictures disagree with
-// the slot's kernel choice, that convolution runs image by image in each picture's own order (ConvExt::kc_major).
-constexpr int RG_LEVELS = 7, RG_LD = 4 * RG_LEVELS;
-
+// holds per picture and resolution level one row {h, w, plain, block}: plain / block = the K order (1 = HALO order,
+// 0 = tap by tap) that a B = 1 forward gives a 3x3 stride-1 convolution at that level, standalone / as conv2 of an
+// identity Bottleneck (which fuse_c23 may take).  Where a pass's pictures disagree with the slot's kernel choice, that
+// convolution runs image by image in each picture's own order (ConvExt::kc_major).
 namespace {
 struct Ragged {
   const int* dev = nullptr;    // table rows of the pass's pictures (device)
   const int* host = nullptr;   // the same rows on the host
   bool on() const { return dev != nullptr; }
-  ConvExt at(int lvl, int b0, int nb, int slot_w) const {
-    return ConvExt{dev + static_cast<size_t>(b0) * RG_LD + 4 * lvl, RG_LD, nb, nullptr, slot_w};
-  }
-  bool all(int lvl, int col, int b0, int nb, int v) const {
-    for (int i = b0; i < b0 + nb; ++i)
+  ConvExt at(int lvl, int nb, int slot_w) const { return ConvExt{dev + 4 * lvl, RG_LD, nb, nullptr, slot_w}; }
+  bool all(int lvl, int col, int nb, int v) const {
+    for (int i = 0; i < nb; ++i)
       if (host[static_cast<size_t>(i) * RG_LD + 4 * lvl + col] != v) return false;
     return true;
   }
@@ -560,68 +545,45 @@ static void ragged_table(const dirb200_net* n, const int* hw, int B, std::vector
   t->assign(static_cast<size_t>(B) * RG_LD, 0);
   for (int i = 0; i < B; ++i) {
     int* r = t->data() + static_cast<size_t>(i) * RG_LD;
-    int h = hw[2 * i], w = hw[2 * i + 1];
+    const LevelSizes z = level_sizes(hw[2 * i], hw[2 * i + 1]);
     for (int l = 0; l < RG_LEVELS; ++l) {
-      if (l == 1) { h = (h + 6 - 7) / 2 + 1; w = (w + 6 - 7) / 2 + 1; }           // stem conv
-      else if (l == 2 || l >= 4) { h = (h + 2 - 3) / 2 + 1; w = (w + 2 - 3) / 2 + 1; }   // maxpool, layer2..4
       const int Cm = 64 << std::max(0, l - 3);   // mid channels of the identity blocks at level l (layer1 at 2 and 3)
-      r[4 * l] = h;
-      r[4 * l + 1] = w;
-      r[4 * l + 2] = halo_order_plain(n, h, w) ? 1 : 0;
-      r[4 * l + 3] = (c23_taken(n, 1, h, w, Cm) || r[4 * l + 2]) ? 1 : 0;
+      r[4 * l] = z.h[l];
+      r[4 * l + 1] = z.w[l];
+      r[4 * l + 2] = halo_order_plain(n, z.h[l], z.w[l]) ? 1 : 0;
+      r[4 * l + 3] = (c23_taken(n, 1, z.h[l], z.w[l], Cm) || r[4 * l + 2]) ? 1 : 0;
     }
   }
 }
 
 static int setup_workspace(dirb200_net* n, int chunk, int H, int W, Workspace* w) {
-  w->H1 = (H + 6 - 7) / 2 + 1; w->W1 = (W + 6 - 7) / 2 + 1;                 // stem conv
-  w->h[0] = (w->H1 + 2 - 3) / 2 + 1; w->w[0] = (w->W1 + 2 - 3) / 2 + 1;     // maxpool
-  w->h[1] = w->h[0]; w->w[1] = w->w[0];                                     // layer1: stride 1
-  for (int s = 2; s < 5; ++s) { w->h[s] = (w->h[s - 1] + 2 - 3) / 2 + 1; w->w[s] = (w->w[s - 1] + 2 - 3) / 2 + 1; }
-  // sub-chunk sizes: option "subN", else auto = enough images for ~2 tiles per SM in the stage's smallest GEMM,
-  // but not more than keeps one stage tensor around 32 MB
-  for (int s = 0; s < 5; ++s) {
-    int v = n->sub[s];
-    if (v <= 0) {
-      if (n->stage_sched == 0) {
-        v = chunk;                              // flat schedule: every stage over the whole chunk
-      } else {
-        // enough images for ~2 waves of 128-pixel tiles in the stage's narrowest GEMM
-        const double px = static_cast<double>(w->h[s]) * w->w[s];
-        v = std::max(1, static_cast<int>(ceil(2.0 * num_sms() * 128.0 / px)));
-        if (s == 0) v = std::max(v, 2);
-      }
-    }
-    w->sub[s] = std::max(1, std::min(v, chunk));
-  }
+  w->chunk = chunk;
+  w->sz = level_sizes(H, W);
+  const int* h = w->sz.h;
+  const int* wd = w->sz.w;
+  const size_t c = chunk;
   size_t off = 0;
   auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 1023) / 1024 * 1024; return o; };
-  const size_t o_sws = carve(std::max(static_cast<size_t>(w->sub[0]) * H * W * 8 * 2, stem_workspace_bytes(w->sub[0], H, W)));
-  const size_t o_stem = carve(static_cast<size_t>(w->sub[0]) * w->H1 * w->W1 * 64 * 2);
+  const size_t o_sws = carve(std::max(c * H * W * 8 * 2, stem_workspace_bytes(chunk, H, W)));
+  const size_t o_stem = carve(c * h[1] * wd[1] * 64 * 2);
   size_t o_stage[4], o_scr[4];
-  for (int s = 0; s < 4; ++s) o_stage[s] = carve(static_cast<size_t>(chunk) * w->h[s] * w->w[s] * n->stage_ch[s] * 2);
-  size_t scr = 0;   // largest tensor inside any stage = the stage's sub-chunk at the stage's INPUT resolution x output channels / or input
+  for (int s = 0; s < 4; ++s) o_stage[s] = carve(c * h[2 + s] * wd[2 + s] * n->stage_ch[s] * 2);
+  size_t scr = 0;   // largest tensor inside any stage: conv1 output at the stage's input resolution, or a block output
   for (int s = 1; s < 5; ++s) {
-    const size_t in_px = static_cast<size_t>(w->h[s - 1]) * w->w[s - 1];
-    scr = std::max(scr, static_cast<size_t>(w->sub[s]) * in_px * (n->stage_ch[s] / 4) * 2);          // conv1 output at input resolution
-    scr = std::max(scr, static_cast<size_t>(w->sub[s]) * w->h[s] * w->w[s] * n->stage_ch[s] * 2);    // block output
+    scr = std::max(scr, c * h[1 + s] * wd[1 + s] * (n->stage_ch[s] / 4) * 2);
+    scr = std::max(scr, c * h[2 + s] * wd[2 + s] * n->stage_ch[s] * 2);
   }
-  if (n->fpn)   // the merged / smoothed layer3 map of a stage-4 sub-chunk lives in a scratch tensor
-    scr = std::max(scr, static_cast<size_t>(w->sub[4]) * w->h[3] * w->w[3] * n->stage_ch[3] * 2);
+  if (n->fpn)   // the merged / smoothed layer3 map of the FPN head lives in a scratch tensor
+    scr = std::max(scr, c * h[5] * wd[5] * n->stage_ch[3] * 2);
   for (int i = 0; i < 4; ++i) o_scr[i] = carve(scr);
-  size_t head_floats = head_workspace_floats(w->sub[4], w->h[4] * w->w[4], n->stage_ch[4], n->out_dim);
+  size_t head_floats = head_workspace_floats(chunk, h[6] * wd[6], n->stage_ch[4], n->out_dim);
   if (n->fpn) {
-    const size_t partial = std::max(head_partial_floats(w->sub[4], w->h[3] * w->w[3], n->stage_ch[3]),
-                                    head_partial_floats(w->sub[4], w->h[4] * w->w[4], n->stage_ch[4]));
-    head_floats = partial + static_cast<size_t>(w->sub[4]) * (n->feat_in() + std::max(n->out_dim, n->feat_in()));
+    const size_t partial = std::max(head_partial_floats(chunk, h[5] * wd[5], n->stage_ch[3]),
+                                    head_partial_floats(chunk, h[6] * wd[6], n->stage_ch[4]));
+    head_floats = partial + c * (n->feat_in() + std::max(n->out_dim, n->feat_in()));
   }
   const size_t o_head = carve(head_floats * 4);
-  if (off > n->ws_bytes) {
-    if (n->ws) DIRB_CUDA(cudaFree(n->ws));
-    n->ws = nullptr;
-    DIRB_CUDA(cudaMalloc(&n->ws, off));
-    n->ws_bytes = off;
-  }
+  DIRB_TRY(grow_device(&n->ws, &n->ws_bytes, off));
   uint8_t* ws = static_cast<uint8_t*>(n->ws);
   w->stem_ws = reinterpret_cast<__half*>(ws + o_sws);
   w->stem_out = reinterpret_cast<__half*>(ws + o_stem);
@@ -631,187 +593,165 @@ static int setup_workspace(dirb200_net* n, int chunk, int H, int W, Workspace* w
   return 0;
 }
 
-// One pass of the network over `cb` images (NCHW fp32 on the device) -> cb descriptors.
-static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs_dev, int cb, int H, int W, float* desc_dev,
-                     __half* desc16_dev, cudaStream_t stream, const uint8_t* imgs_u8 = nullptr,
-                     const Ragged& rg = Ragged()) {
+// One pass of the network over cb <= w.chunk images on the device (NCHW fp32 imgs, or HWC uint8 imgs_u8) -> cb
+// descriptors.
+static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, const uint8_t* imgs_u8, int cb, int H, int W,
+                     float* desc_dev, __half* desc16_dev, cudaStream_t stream, const Ragged& rg) {
   const int D = n->desc_dim();
+  const int* lh = w.sz.h;   // size per level (level_sizes)
+  const int* lw = w.sz.w;
   ConvExt e0, e1;   // extents handed to one launch (ragged batches; the launchers read them on the host)
-  auto ext = [&](ConvExt& e, int lvl, int b0, int nb, int slot_w) -> const ConvExt* {
+  auto ext = [&](ConvExt& e, int lvl, int slot_w) -> const ConvExt* {
     if (!rg.on()) return nullptr;
-    e = rg.at(lvl, b0, nb, slot_w);
+    e = rg.at(lvl, cb, slot_w);
     return &e;
   };
   // 3x3 stride-1 convolution whose K order on the slot is slot_order: pictures that a B = 1 forward gives another
   // order (column col of the table) make the launch pick the order image by image
-  auto ext3 = [&](ConvExt& e, int lvl, int b0, int nb, int slot_w, int col, bool slot_order) -> const ConvExt* {
+  auto ext3 = [&](ConvExt& e, int lvl, int slot_w, int col, bool slot_order) -> const ConvExt* {
     if (!rg.on()) return nullptr;
-    e = rg.at(lvl, b0, nb, slot_w);
-    if (!rg.all(lvl, col, b0, nb, slot_order ? 1 : 0)) e.kc_major = e.hw + col;
+    e = rg.at(lvl, cb, slot_w);
+    if (!rg.all(lvl, col, cb, slot_order ? 1 : 0)) e.kc_major = e.hw + col;
     return &e;
   };
   // ---------------------------------------------------------------- stage 0: stem + maxpool
-  for (int b0 = 0; b0 < cb; b0 += w.sub[0]) {
-    const int sb = std::min(w.sub[0], cb - b0);
-    const float* img = imgs_dev ? imgs_dev + static_cast<size_t>(b0) * 3 * H * W : nullptr;
-    const uint8_t* img8 = imgs_u8 ? imgs_u8 + static_cast<size_t>(b0) * 3 * H * W : nullptr;
-    if (n->conv_impl == 1) {
-      DIRB_REQUIRE(img8 == nullptr, DIRB200_ENOTSUP, "uint8 input needs the space-to-depth stem (conv_impl 0)");
-      {
-        ProfScope ps(n, stream, 2, 0, static_cast<double>(sb) * H * W * (12 + 16));
-        DIRB_TRY(nchw_to_nhwc8(img, sb, H, W, w.stem_ws, stream));
-      }
-      DIRB_TRY(run_conv(n, n->stem, w.stem_ws, sb, H, W, nullptr, 1, w.stem_out, stream, /*force_mma=*/1));
-    } else {
-      const double flops = 2.0 * sb * w.H1 * w.W1 * 64.0 * 147.0;
-      n->last_flops += flops;
-      ProfScope ps(n, stream, 1, flops, static_cast<double>(sb) * (12.0 * H * W + 2.0 * stem_workspace_bytes(1, H, W) + 128.0 * w.H1 * w.W1), "stem s2d + 7x7/s2 3->64");
-      DIRB_TRY(stem_tc(img, sb, H, W, n->stem_w2, n->stem.scale, n->stem.shift, w.stem_ws, w.stem_out, stream, img8,
-                       n->mean_std, ext(e0, 0, b0, sb, W), ext(e1, 1, b0, sb, w.W1)));
+  if (n->conv_impl == 1) {
+    DIRB_REQUIRE(imgs_u8 == nullptr, DIRB200_ENOTSUP, "uint8 input needs the space-to-depth stem (conv_impl 0)");
+    {
+      ProfScope ps(n, stream, 2, 0, static_cast<double>(cb) * H * W * (12 + 16));
+      DIRB_TRY(nchw_to_nhwc8(imgs, cb, H, W, w.stem_ws, stream));
     }
-    ProfScope ps(n, stream, 2, 0, 2.0 * sb * 64 * (static_cast<double>(w.H1) * w.W1 + static_cast<double>(w.h[0]) * w.w[0]), "maxpool 3x3/s2");
-    DIRB_TRY(maxpool_3x3s2(w.stem_out, sb, w.H1, w.W1, 64,
-                           w.stage_out[0] + static_cast<size_t>(b0) * w.h[0] * w.w[0] * 64, stream,
-                           ext(e0, 2, b0, sb, w.w[0])));
+    DIRB_TRY(run_conv(n, n->stem, w.stem_ws, cb, H, W, nullptr, 1, w.stem_out, stream, /*force_mma=*/1));
+  } else {
+    const double flops = 2.0 * cb * lh[1] * lw[1] * 64.0 * 147.0;
+    n->last_flops += flops;
+    ProfScope ps(n, stream, 1, flops, static_cast<double>(cb) * (12.0 * H * W + 2.0 * stem_workspace_bytes(1, H, W) + 128.0 * lh[1] * lw[1]), "stem s2d + 7x7/s2 3->64");
+    DIRB_TRY(stem_tc(imgs, cb, H, W, n->stem_w2, n->stem.scale, n->stem.shift, w.stem_ws, w.stem_out, stream, imgs_u8,
+                     n->mean_std, ext(e0, 0, W), ext(e1, 1, lw[1])));
   }
-  DIRB_TRY(record_tap(n, "stem", w.stage_out[0], cb, w.h[0], w.w[0], 64, stream));
-  // ---------------------------------------------------------------- stages 1..4: layer1..layer4 (+ head)
+  {
+    ProfScope ps(n, stream, 2, 0, 2.0 * cb * 64 * (static_cast<double>(lh[1]) * lw[1] + static_cast<double>(lh[2]) * lw[2]), "maxpool 3x3/s2");
+    DIRB_TRY(maxpool_3x3s2(w.stem_out, cb, lh[1], lw[1], 64, w.stage_out[0], stream, ext(e0, 2, lw[2])));
+  }
+  DIRB_TRY(record_tap(n, "stem", w.stage_out[0], cb, lh[2], lw[2], 64, stream));
+  // ---------------------------------------------------------------- stages 1..4: layer1..layer4
+  const __half* x = w.stage_out[0];
   int first = 0;
   for (int s = 1; s < 5; ++s) {
     const int last = n->layer_end[s - 1];       // blocks [first, last)
-    const int hi = w.h[s - 1], wi = w.w[s - 1], ho = w.h[s], wo = w.w[s];
-    const __half* stage_in = w.stage_out[s - 1];
-    for (int b0 = 0; b0 < cb; b0 += w.sub[s]) {
-      const int sb = std::min(w.sub[s], cb - b0);
-      const __half* x = stage_in + static_cast<size_t>(b0) * hi * wi * n->stage_ch[s - 1];
-      int h = hi, wd = wi;
-      int lvl = 1 + s;                          // extent-table level of x
-      for (int bi = first; bi < last; ++bi) {
-        const Block& blk = n->blocks[bi];
-        const int j = bi - first;
-        const int lvl_in = lvl;
-        if ((n->basic ? blk.c1.stride : blk.c2.stride) == 2) lvl = 2 + s;   // level of the block's output
-        __half* t1 = w.scratch[0];
-        __half* t2 = w.scratch[1];
-        __half* rs = w.scratch[2];
-        __half* y = (j % 2 == 0) ? w.scratch[3] : w.scratch[2];
-        if (bi == last - 1 && s < 4) y = w.stage_out[s] + static_cast<size_t>(b0) * ho * wo * n->stage_ch[s];
-        if (n->basic) {
-          // BasicBlock, resnet.py:27-44: 3x3(stride) + BN + ReLU -> 3x3 + BN -> + (projected) x -> ReLU
-          const int st = blk.c1.stride;
-          const int h2 = (h + 2 - 3) / st + 1, w2 = (wd + 2 - 3) / st + 1;
-          DIRB_TRY(run_conv(n, blk.c1, x, sb, h, wd, nullptr, 1, t1, stream, 0,
-                            st == 1 ? ext3(e0, lvl, b0, sb, w2, 2, halo_order_plain(n, h2, w2)) : ext(e0, lvl, b0, sb, w2)));
-          const __half* res = x;
-          if (blk.has_down) {
-            DIRB_TRY(run_conv(n, blk.down, x, sb, h, wd, nullptr, 0, rs, stream, 0, ext(e0, lvl, b0, sb, w2)));
-            res = rs;
-          }
-          DIRB_TRY(run_conv(n, blk.c2, t1, sb, h2, w2, res, 1, y, stream, 0,
-                            ext3(e0, lvl, b0, sb, w2, 2, halo_order_plain(n, h2, w2))));
-          x = y;
-          h = h2;
-          wd = w2;
-          continue;
-        }
-        const int st = blk.c2.stride;
-        const int h2 = (h + 2 - 3) / st + 1, w2 = (wd + 2 - 3) / st + 1;
-        DIRB_TRY(run_conv(n, blk.c1, x, sb, h, wd, nullptr, 1, t1, stream, 0, ext(e0, lvl_in, b0, sb, wd)));
-        const bool c23 = !blk.has_down && st == 1 && c23_taken(n, sb, h, wd, blk.c2.Cin);
-        // ragged: a stride-1 conv2 in the K order of the slot's kernel choice (the fused kernel has the HALO order)
-        const ConvExt* e2 = st == 1 ? ext3(e1, lvl, b0, sb, wd, blk.has_down ? 2 : 3, c23 || halo_order_plain(n, h, wd))
-                                    : ext(e1, lvl, b0, sb, w2);
-        if (c23 && (e2 == nullptr || e2->kc_major == nullptr)) {
-          // identity block: conv2 -> conv3 (+ x) in one kernel, the conv2 output stays in shared memory
-          const int Cm = blk.c2.Cin;
-          const double flops = 2.0 * sb * h * wd * (9.0 * Cm * Cm + 4.0 * Cm * Cm);
-          const double bytes = 2.0 * (static_cast<double>(sb) * h * wd * (Cm + 8.0 * Cm) + 13.0 * Cm * Cm);   // t1 + residual + output, weights
-          n->last_flops += flops;
-          char tg[96];
-          snprintf(tg, sizeof(tg), "3x3 %d->%d + 1x1 ->%d +res fused @%dx%d", Cm, Cm, 4 * Cm, h, wd);
-          ProfScope ps(n, stream, 0, flops, bytes, tg);
-          DIRB_TRY(conv_c23(sb, h, wd, Cm, t1, blk.c2.w, blk.c2.scale, blk.c2.shift, blk.c3.w, blk.c3.scale, blk.c3.shift, x, y,
-                            stream, e2));
-          x = y;
-          continue;
-        }
-        DIRB_TRY(run_conv(n, blk.c2, t1, sb, h, wd, nullptr, 1, t2, stream, 0, e2));
+    int lvl = 1 + s;                            // level of x
+    for (int bi = first; bi < last; ++bi) {
+      const Block& blk = n->blocks[bi];
+      const int j = bi - first;
+      const int lvl_in = lvl;
+      if ((n->basic ? blk.c1.stride : blk.c2.stride) == 2) lvl = 2 + s;   // level of the block's output
+      const int h = lh[lvl_in], wd = lw[lvl_in], h2 = lh[lvl], w2 = lw[lvl];
+      __half* t1 = w.scratch[0];
+      __half* t2 = w.scratch[1];
+      __half* rs = w.scratch[2];
+      __half* y = (j % 2 == 0) ? w.scratch[3] : w.scratch[2];
+      if (bi == last - 1 && s < 4) y = w.stage_out[s];
+      if (n->basic) {
+        // BasicBlock, resnet.py:27-44: 3x3(stride) + BN + ReLU -> 3x3 + BN -> + (projected) x -> ReLU
+        DIRB_TRY(run_conv(n, blk.c1, x, cb, h, wd, nullptr, 1, t1, stream, 0,
+                          blk.c1.stride == 1 ? ext3(e0, lvl, w2, 2, halo_order_plain(n, h2, w2)) : ext(e0, lvl, w2)));
         const __half* res = x;
-        if (blk.has_down && n->fuse_ds && n->conv_impl == 0 && blk.c3.Cout % 256 == 0) {
-          const double flops = 2.0 * sb * h2 * w2 * static_cast<double>(blk.c3.Cout) * (blk.c3.Cin + blk.down.Cin);
-          const double bytes = 2.0 * (static_cast<double>(sb) * h2 * w2 * (blk.c3.Cin + blk.c3.Cout) +
-                                      static_cast<double>(sb) * h * wd * blk.down.Cin +
-                                      static_cast<double>(blk.c3.Cout) * (blk.c3.Cin + blk.down.Cin));
-          n->last_flops += flops;
-          char tbuf_[96];
-          snprintf(tbuf_, sizeof(tbuf_), "1x1 [%d|%d%s]->%d fused-shortcut @%dx%d", blk.c3.Cin, blk.down.Cin, st == 2 ? "/s2" : "", blk.c3.Cout, h2, w2);
-          ProfScope ps(n, stream, 0, flops, bytes, tbuf_);
-          DIRB_TRY(conv_fused_ds(sb, h2, w2, blk.c3.Cin, t2, h, wd, blk.down.Cin, st, x, blk.wcat, blk.c3.Cout, blk.ones,
-                                 blk.cat_shift, y, stream, ext(e0, lvl, b0, sb, w2)));
-          x = y;
-          h = h2;
-          wd = w2;
-          continue;
-        }
         if (blk.has_down) {
-          DIRB_TRY(run_conv(n, blk.down, x, sb, h, wd, nullptr, 0, rs, stream, 0, ext(e0, lvl, b0, sb, w2)));
+          DIRB_TRY(run_conv(n, blk.down, x, cb, h, wd, nullptr, 0, rs, stream, 0, ext(e0, lvl, w2)));
           res = rs;
         }
-        DIRB_TRY(run_conv(n, blk.c3, t2, sb, h2, w2, res, 1, y, stream, 0, ext(e0, lvl, b0, sb, w2)));
+        DIRB_TRY(run_conv(n, blk.c2, t1, cb, h2, w2, res, 1, y, stream, 0, ext3(e0, lvl, w2, 2, halo_order_plain(n, h2, w2))));
         x = y;
-        h = h2;
-        wd = w2;
+        continue;
       }
-      if (s == 4) {
-        const int C4 = n->stage_ch[4];
-        if (b0 + sb >= cb) DIRB_TRY(record_tap(n, "layer4", x, sb, ho, wo, C4, stream));
-        if (n->fpn) {
-          // ---- FPN head, rmac_resnet_fpn.py:52-90
-          const int C3 = n->stage_ch[3], h3 = w.h[3], w3 = w.w[3], Ct = C3 + C4;
-          const __half* x4 = w.stage_out[3] + static_cast<size_t>(b0) * h3 * w3 * C3;
-          if (n->fpn_mode == 1) {
-            // relu(conv1x5(upsample(x5))) == upsample(relu(conv1x5(x5))): the 1x1 convolution runs on the small map.
-            // x (layer4 output) sits in scratch[2] or [3]; scratch[0] / [1] are free after the last block.
-            __half* tbuf = w.scratch[0];
-            __half* x4p = w.scratch[1];
-            DIRB_TRY(run_conv(n, n->fpn_lat, x, sb, ho, wo, nullptr, 1, tbuf, stream));
-            {
-              ProfScope ps(n, stream, 2, 0, 2.0 * sb * (2.0 * h3 * w3 + static_cast<double>(ho) * wo) * C3);
-              DIRB_TRY(upsample_add(x4, tbuf, x4p, sb, h3, w3, ho, wo, C3, stream));
-            }
-            DIRB_TRY(run_conv(n, n->fpn_smooth, x4p, sb, h3, w3, nullptr, 1, tbuf, stream));
-            x4 = tbuf;
-            if (b0 + sb >= cb) DIRB_TRY(record_tap(n, "fpn_c4", x4, sb, h3, w3, C3, stream));
-          }
-          ProfScope ps(n, stream, 3, n->without_fc ? 0.0 : 2.0 * sb * static_cast<double>(Ct) * n->out_dim,
-                       2.0 * sb * (static_cast<double>(ho) * wo * C4 + static_cast<double>(h3) * w3 * C3));
-          const size_t partial_floats = std::max(head_partial_floats(w.sub[4], h3 * w3, C3), head_partial_floats(w.sub[4], ho * wo, C4));
-          float* partial = w.head_ws;
-          float* g = partial + partial_floats;
-          float* yv = g + static_cast<size_t>(w.sub[4]) * Ct;
-          DIRB_TRY(head_pool(x4, sb, h3 * w3, C3, 0, n->gem_p4, n->gem_eps, 0, partial, g, Ct, 0, stream));    // torch.cat((x4, x5), 1)
-          DIRB_TRY(head_pool(x, sb, ho * wo, C4, 0, n->gem_p, n->gem_eps, 0, partial, g, Ct, C3, stream));
-          if (n->norm_features) DIRB_TRY(l2_normalize(g, sb, Ct, 1e-12f, g, nullptr, stream));
-          DIRB_TRY(head_fc_l2(g, sb, Ct, n->without_fc ? nullptr : n->fc_w, n->without_fc ? nullptr : n->fc_b, D, yv,
-                              desc_dev + static_cast<size_t>(b0) * D,
-                              desc16_dev ? desc16_dev + static_cast<size_t>(b0) * D : nullptr, stream));
-          if (!n->without_fc) n->last_flops += 2.0 * sb * static_cast<double>(Ct) * n->out_dim;
-          continue;
-        }
-        ProfScope ps(n, stream, 3, n->without_fc ? 0.0 : 2.0 * sb * static_cast<double>(C4) * n->out_dim, 2.0 * sb * ho * wo * static_cast<double>(C4), "head pool+fc+l2");
-        if (n->center_bias > 0.0f)   // x is a scratch buffer whose only remaining reader is the pooling below
-          DIRB_TRY(center_bias(const_cast<__half*>(x), sb, ho, wo, C4, n->center_bias, stream, ext(e0, 6, b0, sb, wo)));
-        DIRB_TRY(head_pool_fc_l2(x, sb, ho * wo, C4, n->pooling, n->gem_p, n->gem_eps, n->norm_features,
-                                 n->without_fc ? nullptr : n->fc_w, n->without_fc ? nullptr : n->fc_b, D, w.head_ws,
-                                 desc_dev + static_cast<size_t>(b0) * D,
-                                 desc16_dev ? desc16_dev + static_cast<size_t>(b0) * D : nullptr, stream, n->head_bar,
-                                 ext(e0, 6, b0, sb, wo)));
-        if (!n->without_fc) n->last_flops += 2.0 * sb * static_cast<double>(C4) * n->out_dim;
+      const int st = blk.c2.stride;
+      DIRB_TRY(run_conv(n, blk.c1, x, cb, h, wd, nullptr, 1, t1, stream, 0, ext(e0, lvl_in, wd)));
+      const bool c23 = !blk.has_down && st == 1 && c23_taken(n, cb, h, wd, blk.c2.Cin);
+      // ragged: a stride-1 conv2 in the K order of the slot's kernel choice (the fused kernel has the HALO order)
+      const ConvExt* e2 = st == 1 ? ext3(e1, lvl, wd, blk.has_down ? 2 : 3, c23 || halo_order_plain(n, h, wd))
+                                  : ext(e1, lvl, w2);
+      if (c23 && (e2 == nullptr || e2->kc_major == nullptr)) {
+        // identity block: conv2 -> conv3 (+ x) in one kernel, the conv2 output stays in shared memory
+        const int Cm = blk.c2.Cin;
+        const double flops = 2.0 * cb * h * wd * (9.0 * Cm * Cm + 4.0 * Cm * Cm);
+        const double bytes = 2.0 * (static_cast<double>(cb) * h * wd * (Cm + 8.0 * Cm) + 13.0 * Cm * Cm);   // t1 + residual + output, weights
+        n->last_flops += flops;
+        char tg[96];
+        snprintf(tg, sizeof(tg), "3x3 %d->%d + 1x1 ->%d +res fused @%dx%d", Cm, Cm, 4 * Cm, h, wd);
+        ProfScope ps(n, stream, 0, flops, bytes, tg);
+        DIRB_TRY(conv_c23(cb, h, wd, Cm, t1, blk.c2.w, blk.c2.scale, blk.c2.shift, blk.c3.w, blk.c3.scale, blk.c3.shift, x, y,
+                          stream, e2));
+        x = y;
+        continue;
       }
+      DIRB_TRY(run_conv(n, blk.c2, t1, cb, h, wd, nullptr, 1, t2, stream, 0, e2));
+      if (blk.has_down && n->fuse_ds && n->conv_impl == 0 && blk.c3.Cout % 256 == 0) {
+        const double flops = 2.0 * cb * h2 * w2 * static_cast<double>(blk.c3.Cout) * (blk.c3.Cin + blk.down.Cin);
+        const double bytes = 2.0 * (static_cast<double>(cb) * h2 * w2 * (blk.c3.Cin + blk.c3.Cout) +
+                                    static_cast<double>(cb) * h * wd * blk.down.Cin +
+                                    static_cast<double>(blk.c3.Cout) * (blk.c3.Cin + blk.down.Cin));
+        n->last_flops += flops;
+        char tbuf_[96];
+        snprintf(tbuf_, sizeof(tbuf_), "1x1 [%d|%d%s]->%d fused-shortcut @%dx%d", blk.c3.Cin, blk.down.Cin, st == 2 ? "/s2" : "", blk.c3.Cout, h2, w2);
+        ProfScope ps(n, stream, 0, flops, bytes, tbuf_);
+        DIRB_TRY(conv_fused_ds(cb, h2, w2, blk.c3.Cin, t2, h, wd, blk.down.Cin, st, x, blk.wcat, blk.c3.Cout, blk.ones,
+                               blk.cat_shift, y, stream, ext(e0, lvl, w2)));
+        x = y;
+        continue;
+      }
+      const __half* res = x;
+      if (blk.has_down) {
+        DIRB_TRY(run_conv(n, blk.down, x, cb, h, wd, nullptr, 0, rs, stream, 0, ext(e0, lvl, w2)));
+        res = rs;
+      }
+      DIRB_TRY(run_conv(n, blk.c3, t2, cb, h2, w2, res, 1, y, stream, 0, ext(e0, lvl, w2)));
+      x = y;
     }
-    if (s < 4) DIRB_TRY(record_tap(n, "layer" + std::to_string(s), w.stage_out[s], cb, ho, wo, n->stage_ch[s], stream));
+    if (s < 4) DIRB_TRY(record_tap(n, "layer" + std::to_string(s), w.stage_out[s], cb, lh[2 + s], lw[2 + s], n->stage_ch[s], stream));
     first = last;
   }
+  // ---------------------------------------------------------------- head
+  const int C4 = n->stage_ch[4], ho = lh[6], wo = lw[6];
+  DIRB_TRY(record_tap(n, "layer4", x, cb, ho, wo, C4, stream));
+  if (n->fpn) {
+    // ---- FPN head, rmac_resnet_fpn.py:52-90
+    const int C3 = n->stage_ch[3], h3 = lh[5], w3 = lw[5], Ct = C3 + C4;
+    const __half* x4 = w.stage_out[3];
+    if (n->fpn_mode == 1) {
+      // relu(conv1x5(upsample(x5))) == upsample(relu(conv1x5(x5))): the 1x1 convolution runs on the small map.
+      // x (layer4 output) sits in scratch[2] or [3]; scratch[0] / [1] are free after the last block.
+      __half* tbuf = w.scratch[0];
+      __half* x4p = w.scratch[1];
+      DIRB_TRY(run_conv(n, n->fpn_lat, x, cb, ho, wo, nullptr, 1, tbuf, stream));
+      {
+        ProfScope ps(n, stream, 2, 0, 2.0 * cb * (2.0 * h3 * w3 + static_cast<double>(ho) * wo) * C3);
+        DIRB_TRY(upsample_add(x4, tbuf, x4p, cb, h3, w3, ho, wo, C3, stream));
+      }
+      DIRB_TRY(run_conv(n, n->fpn_smooth, x4p, cb, h3, w3, nullptr, 1, tbuf, stream));
+      x4 = tbuf;
+      DIRB_TRY(record_tap(n, "fpn_c4", x4, cb, h3, w3, C3, stream));
+    }
+    ProfScope ps(n, stream, 3, n->without_fc ? 0.0 : 2.0 * cb * static_cast<double>(Ct) * n->out_dim,
+                 2.0 * cb * (static_cast<double>(ho) * wo * C4 + static_cast<double>(h3) * w3 * C3));
+    const size_t partial_floats = std::max(head_partial_floats(w.chunk, h3 * w3, C3), head_partial_floats(w.chunk, ho * wo, C4));
+    float* partial = w.head_ws;
+    float* g = partial + partial_floats;
+    float* yv = g + static_cast<size_t>(w.chunk) * Ct;
+    DIRB_TRY(head_pool(x4, cb, h3 * w3, C3, 0, n->gem_p4, n->gem_eps, 0, partial, g, Ct, 0, stream));    // torch.cat((x4, x5), 1)
+    DIRB_TRY(head_pool(x, cb, ho * wo, C4, 0, n->gem_p, n->gem_eps, 0, partial, g, Ct, C3, stream));
+    if (n->norm_features) DIRB_TRY(l2_normalize(g, cb, Ct, 1e-12f, g, nullptr, stream));
+    DIRB_TRY(head_fc_l2(g, cb, Ct, n->without_fc ? nullptr : n->fc_w, n->without_fc ? nullptr : n->fc_b, D, yv, desc_dev,
+                        desc16_dev, stream));
+    if (!n->without_fc) n->last_flops += 2.0 * cb * static_cast<double>(Ct) * n->out_dim;
+    return 0;
+  }
+  ProfScope ps(n, stream, 3, n->without_fc ? 0.0 : 2.0 * cb * static_cast<double>(C4) * n->out_dim, 2.0 * cb * ho * wo * static_cast<double>(C4), "head pool+fc+l2");
+  if (n->center_bias > 0.0f)   // x is a scratch buffer whose only remaining reader is the pooling below
+    DIRB_TRY(center_bias(const_cast<__half*>(x), cb, ho, wo, C4, n->center_bias, stream, ext(e0, 6, wo)));
+  DIRB_TRY(head_pool_fc_l2(x, cb, ho * wo, C4, n->pooling, n->gem_p, n->gem_eps, n->norm_features,
+                           n->without_fc ? nullptr : n->fc_w, n->without_fc ? nullptr : n->fc_b, D, w.head_ws, desc_dev,
+                           desc16_dev, stream, n->head_bar, ext(e0, 6, wo)));
+  if (!n->without_fc) n->last_flops += 2.0 * cb * static_cast<double>(C4) * n->out_dim;
   return 0;
 }
 
@@ -821,92 +761,38 @@ static int check_forward_args(dirb200_net* n, int B, int H, int W) {
   return 0;
 }
 
-int dirb200_net_forward(dirb200_net* n, const float* imgs_dev, int B, int H, int W, float* desc_dev, void* desc16_dev,
-                        void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DIRB_REQUIRE(n && imgs_dev && desc_dev, DIRB200_EINVAL, "null argument");
-  DIRB_TRY(check_forward_args(n, B, H, W));
-  DIRB_CUDA(cudaSetDevice(n->device));
-  const int64_t launches0 = launches_total();
+// Bookkeeping of one forward call: its launch and flop counts (dirb200_net_last_launches) and, unless option
+// "profile" 2 accumulates over calls, its profile.  begin_forward returns the launch counter end_forward needs.
+static int64_t begin_forward(dirb200_net* n) {
   n->last_flops = 0;
   if (n->profile != 2) n->prof.reset();
-  const int chunk = n->chunk > 0 ? std::min(n->chunk, B) : auto_chunk(B, H, W);
-  const int D = n->desc_dim();
-  Workspace w;
-  DIRB_TRY(setup_workspace(n, chunk, H, W, &w));
-  for (int b0 = 0; b0 < B; b0 += chunk) {
-    const int cb = std::min(chunk, B - b0);
-    DIRB_TRY(run_chunk(n, w, imgs_dev + static_cast<size_t>(b0) * 3 * H * W, cb, H, W,
-                       desc_dev + static_cast<size_t>(b0) * D,
-                       desc16_dev ? static_cast<__half*>(desc16_dev) + static_cast<size_t>(b0) * D : nullptr, stream));
-  }
-  n->last_launches = launches_total() - launches0;
-  return 0;
+  return launches_total();
 }
 
-// Host buffers in, host descriptors out.  The batch is cut into chunks of `host_chunk` images; the H2D copy of
-// chunk i+1 (copy stream) overlaps the network pass over chunk i (compute stream), two device input buffers.
-static int forward_host_impl(dirb200_net* n, const void* imgs_host, int is_u8, int B, int H, int W, float* desc_host);
+static void end_forward(dirb200_net* n, int64_t launches0) { n->last_launches = launches_total() - launches0; }
 
-int dirb200_net_forward_host(dirb200_net* n, const float* imgs_host, int B, int H, int W, float* desc_host) {
-  return forward_host_impl(n, imgs_host, 0, B, H, W, desc_host);
-}
-
-int dirb200_net_forward_host_u8(dirb200_net* n, const uint8_t* imgs_host, int B, int H, int W, float* desc_host) {
-  return forward_host_impl(n, imgs_host, 1, B, H, W, desc_host);
-}
-
-int dirb200_net_forward_u8(dirb200_net* n, const uint8_t* imgs_dev, int B, int H, int W, float* desc_dev, void* desc16_dev,
-                           void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DIRB_REQUIRE(n && imgs_dev && desc_dev, DIRB200_EINVAL, "null argument");
+// Device buffers in and out, on `stream`: B images, NCHW fp32 (f32) or HWC uint8 (u8), -> B descriptors.  hw_host =
+// the pictures' sizes of a ragged batch (see Ragged), nullptr for a dense batch.
+static int forward_dev(dirb200_net* n, const float* f32, const uint8_t* u8, int B, int H, int W, const int* hw_host,
+                       float* desc_dev, __half* desc16_dev, cudaStream_t stream) {
   DIRB_TRY(check_forward_args(n, B, H, W));
-  DIRB_CUDA(cudaSetDevice(n->device));
-  const int64_t launches0 = launches_total();
-  n->last_flops = 0;
-  if (n->profile != 2) n->prof.reset();
-  const int chunk = n->chunk > 0 ? std::min(n->chunk, B) : auto_chunk(B, H, W);
-  const int D = n->desc_dim();
-  Workspace w;
-  DIRB_TRY(setup_workspace(n, chunk, H, W, &w));
-  for (int b0 = 0; b0 < B; b0 += chunk) {
-    const int cb = std::min(chunk, B - b0);
-    DIRB_TRY(run_chunk(n, w, nullptr, cb, H, W, desc_dev + static_cast<size_t>(b0) * D,
-                       desc16_dev ? static_cast<__half*>(desc16_dev) + static_cast<size_t>(b0) * D : nullptr, stream,
-                       imgs_dev + static_cast<size_t>(b0) * 3 * H * W));
-  }
-  n->last_launches = launches_total() - launches0;
-  return 0;
-}
-
-// Ragged batch: B pictures of sizes hw_host[i] in the top-left corners of slots of H x W (see RG_LD).
-static int forward_ragged_impl(dirb200_net* n, const float* slots, const uint8_t* slots_u8, int B, int H, int W,
-                               const int* hw_host, float* desc_dev, void* desc16_dev, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DIRB_REQUIRE(n && (slots || slots_u8) && hw_host && desc_dev, DIRB200_EINVAL, "null argument");
-  DIRB_TRY(check_forward_args(n, B, H, W));
-  DIRB_REQUIRE(!n->fpn, DIRB200_ENOTSUP,
-               "ragged batches do not support FPN heads (their upsampling ratio depends on each picture's size)");
-  DIRB_REQUIRE(n->conv_impl != 1, DIRB200_ENOTSUP, "ragged batches need the wgmma convolutions (conv_impl 0 or 2)");
-  for (int i = 0; i < B; ++i)
-    DIRB_REQUIRE(hw_host[2 * i] >= 32 && hw_host[2 * i] <= H && hw_host[2 * i + 1] >= 32 && hw_host[2 * i + 1] <= W,
-                 DIRB200_EINVAL, "picture %d: size %dx%d is outside [32, %d] x [32, %d]", i, hw_host[2 * i],
-                 hw_host[2 * i + 1], H, W);
   DIRB_CUDA(cudaSetDevice(n->device));
   std::vector<int> table;
-  ragged_table(n, hw_host, B, &table);
-  const size_t tbytes = table.size() * sizeof(int);
-  if (tbytes > n->ext_bytes) {
-    if (n->ext_dev) DIRB_CUDA(cudaFree(n->ext_dev));
-    n->ext_dev = nullptr;
-    DIRB_CUDA(cudaMalloc(reinterpret_cast<void**>(&n->ext_dev), tbytes));
-    n->ext_bytes = tbytes;
+  if (hw_host) {
+    DIRB_REQUIRE(!n->fpn, DIRB200_ENOTSUP,
+                 "ragged batches do not support FPN heads (their upsampling ratio depends on each picture's size)");
+    DIRB_REQUIRE(n->conv_impl != 1, DIRB200_ENOTSUP, "ragged batches need the wgmma convolutions (conv_impl 0 or 2)");
+    for (int i = 0; i < B; ++i)
+      DIRB_REQUIRE(hw_host[2 * i] >= 32 && hw_host[2 * i] <= H && hw_host[2 * i + 1] >= 32 && hw_host[2 * i + 1] <= W,
+                   DIRB200_EINVAL, "picture %d: size %dx%d is outside [32, %d] x [32, %d]", i, hw_host[2 * i],
+                   hw_host[2 * i + 1], H, W);
+    ragged_table(n, hw_host, B, &table);
+    const size_t tbytes = table.size() * sizeof(int);
+    DIRB_TRY(grow_device(reinterpret_cast<void**>(&n->ext_dev), &n->ext_bytes, tbytes));
+    // pageable source: the copy is staged before the call returns, and it is ordered before the kernels that read it
+    DIRB_CUDA(cudaMemcpyAsync(n->ext_dev, table.data(), tbytes, cudaMemcpyHostToDevice, stream));
   }
-  // pageable source: the copy is staged before the call returns, and it is ordered before the kernels that read it
-  DIRB_CUDA(cudaMemcpyAsync(n->ext_dev, table.data(), tbytes, cudaMemcpyHostToDevice, stream));
-  const int64_t launches0 = launches_total();
-  n->last_flops = 0;
-  if (n->profile != 2) n->prof.reset();
+  const int64_t launches0 = begin_forward(n);
   const int chunk = n->chunk > 0 ? std::min(n->chunk, B) : auto_chunk(B, H, W);
   const int D = n->desc_dim();
   Workspace w;
@@ -915,28 +801,49 @@ static int forward_ragged_impl(dirb200_net* n, const float* slots, const uint8_t
     const int cb = std::min(chunk, B - b0);
     const size_t img = static_cast<size_t>(b0) * 3 * H * W;
     Ragged rg;
-    rg.dev = n->ext_dev + static_cast<size_t>(b0) * RG_LD;
-    rg.host = table.data() + static_cast<size_t>(b0) * RG_LD;
-    DIRB_TRY(run_chunk(n, w, slots ? slots + img : nullptr, cb, H, W, desc_dev + static_cast<size_t>(b0) * D,
-                       desc16_dev ? static_cast<__half*>(desc16_dev) + static_cast<size_t>(b0) * D : nullptr, stream,
-                       slots_u8 ? slots_u8 + img : nullptr, rg));
+    if (hw_host) {
+      rg.dev = n->ext_dev + static_cast<size_t>(b0) * RG_LD;
+      rg.host = table.data() + static_cast<size_t>(b0) * RG_LD;
+    }
+    DIRB_TRY(run_chunk(n, w, f32 ? f32 + img : nullptr, u8 ? u8 + img : nullptr, cb, H, W,
+                       desc_dev + static_cast<size_t>(b0) * D, desc16_dev ? desc16_dev + static_cast<size_t>(b0) * D : nullptr,
+                       stream, rg));
   }
-  n->last_launches = launches_total() - launches0;
+  end_forward(n, launches0);
   return 0;
 }
 
+int dirb200_net_forward(dirb200_net* n, const float* imgs_dev, int B, int H, int W, float* desc_dev, void* desc16_dev,
+                        void* stream) {
+  DIRB_REQUIRE(n && imgs_dev && desc_dev, DIRB200_EINVAL, "null argument");
+  return forward_dev(n, imgs_dev, nullptr, B, H, W, nullptr, desc_dev, static_cast<__half*>(desc16_dev),
+                     static_cast<cudaStream_t>(stream));
+}
+
+int dirb200_net_forward_u8(dirb200_net* n, const uint8_t* imgs_dev, int B, int H, int W, float* desc_dev, void* desc16_dev,
+                           void* stream) {
+  DIRB_REQUIRE(n && imgs_dev && desc_dev, DIRB200_EINVAL, "null argument");
+  return forward_dev(n, nullptr, imgs_dev, B, H, W, nullptr, desc_dev, static_cast<__half*>(desc16_dev),
+                     static_cast<cudaStream_t>(stream));
+}
+
+// Ragged batch: B pictures of sizes hw_host[i] in the top-left corners of slots of H x W (see Ragged).
 int dirb200_net_forward_ragged_u8(dirb200_net* n, const uint8_t* slots_dev, int B, int H, int W, const int* hw_host,
                                   float* desc_dev, void* desc16_dev, void* stream) {
-  DIRB_REQUIRE(slots_dev, DIRB200_EINVAL, "null argument");
-  return forward_ragged_impl(n, nullptr, slots_dev, B, H, W, hw_host, desc_dev, desc16_dev, stream);
+  DIRB_REQUIRE(n && slots_dev && hw_host && desc_dev, DIRB200_EINVAL, "null argument");
+  return forward_dev(n, nullptr, slots_dev, B, H, W, hw_host, desc_dev, static_cast<__half*>(desc16_dev),
+                     static_cast<cudaStream_t>(stream));
 }
 
 int dirb200_net_forward_ragged(dirb200_net* n, const float* slots_dev, int B, int H, int W, const int* hw_host,
                                float* desc_dev, void* desc16_dev, void* stream) {
-  DIRB_REQUIRE(slots_dev, DIRB200_EINVAL, "null argument");
-  return forward_ragged_impl(n, slots_dev, nullptr, B, H, W, hw_host, desc_dev, desc16_dev, stream);
+  DIRB_REQUIRE(n && slots_dev && hw_host && desc_dev, DIRB200_EINVAL, "null argument");
+  return forward_dev(n, slots_dev, nullptr, B, H, W, hw_host, desc_dev, static_cast<__half*>(desc16_dev),
+                     static_cast<cudaStream_t>(stream));
 }
 
+// Host buffers in, host descriptors out.  The batch is cut into chunks; the H2D copy of chunk i+1 (copy stream)
+// overlaps the network pass over chunk i (compute stream), two device input buffers.
 static int forward_host_impl(dirb200_net* n, const void* imgs_host_, int is_u8, int B, int H, int W, float* desc_host) {
   const uint8_t* imgs_host = static_cast<const uint8_t*>(imgs_host_);
   DIRB_REQUIRE(n && imgs_host && desc_host, DIRB200_EINVAL, "null argument");
@@ -969,26 +876,14 @@ static int forward_host_impl(dirb200_net* n, const void* imgs_host_, int is_u8, 
   const size_t in_bytes = 2 * static_cast<size_t>(chunk) * img_bytes;
   const int D = n->desc_dim();
   const size_t out_bytes = static_cast<size_t>(B) * D * 4;
-  if (in_bytes > n->h2d_bytes) {
-    if (n->h2d) DIRB_CUDA(cudaFree(n->h2d));
-    n->h2d = nullptr;
-    DIRB_CUDA(cudaMalloc(reinterpret_cast<void**>(&n->h2d), in_bytes));
-    n->h2d_bytes = in_bytes;
-  }
-  if (out_bytes > n->d_desc_bytes) {
-    if (n->d_desc) DIRB_CUDA(cudaFree(n->d_desc));
-    n->d_desc = nullptr;
-    DIRB_CUDA(cudaMalloc(reinterpret_cast<void**>(&n->d_desc), out_bytes));
-    n->d_desc_bytes = out_bytes;
-  }
+  DIRB_TRY(grow_device(reinterpret_cast<void**>(&n->h2d), &n->h2d_bytes, in_bytes));
+  DIRB_TRY(grow_device(reinterpret_cast<void**>(&n->d_desc), &n->d_desc_bytes, out_bytes));
   while (n->pipe_events.size() < static_cast<size_t>(2 * nchunks)) {
     cudaEvent_t e;
     DIRB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     n->pipe_events.push_back(e);
   }
-  const int64_t launches0 = launches_total();
-  n->last_flops = 0;
-  if (n->profile != 2) n->prof.reset();
+  const int64_t launches0 = begin_forward(n);
   Workspace w;
   DIRB_TRY(setup_workspace(n, chunk, H, W, &w));
   int b0 = 0;
@@ -1001,15 +896,23 @@ static int forward_host_impl(dirb200_net* n, const void* imgs_host_, int is_u8, 
                               cudaMemcpyHostToDevice, n->copy_stream));
     DIRB_CUDA(cudaEventRecord(copied, n->copy_stream));
     DIRB_CUDA(cudaStreamWaitEvent(n->own_stream, copied, 0));
-    DIRB_TRY(run_chunk(n, w, is_u8 ? nullptr : reinterpret_cast<const float*>(dst), cb, H, W,
-                       n->d_desc + static_cast<size_t>(b0) * D, nullptr, n->own_stream, is_u8 ? dst : nullptr));
+    DIRB_TRY(run_chunk(n, w, is_u8 ? nullptr : reinterpret_cast<const float*>(dst), is_u8 ? dst : nullptr, cb, H, W,
+                       n->d_desc + static_cast<size_t>(b0) * D, nullptr, n->own_stream, Ragged()));
     DIRB_CUDA(cudaEventRecord(done, n->own_stream));
     b0 += cb;
   }
   DIRB_CUDA(cudaMemcpyAsync(desc_host, n->d_desc, out_bytes, cudaMemcpyDeviceToHost, n->own_stream));
   DIRB_CUDA(cudaStreamSynchronize(n->own_stream));
-  n->last_launches = launches_total() - launches0;
+  end_forward(n, launches0);
   return 0;
+}
+
+int dirb200_net_forward_host(dirb200_net* n, const float* imgs_host, int B, int H, int W, float* desc_host) {
+  return forward_host_impl(n, imgs_host, 0, B, H, W, desc_host);
+}
+
+int dirb200_net_forward_host_u8(dirb200_net* n, const uint8_t* imgs_host, int B, int H, int W, float* desc_host) {
+  return forward_host_impl(n, imgs_host, 1, B, H, W, desc_host);
 }
 
 // Aggregated per-class timing of the last forward run with option "profile": out[4][4] = {launches, ms, flops, bytes}

@@ -696,12 +696,8 @@ static int scratch_acquire(size_t bytes, cudaStream_t stream, void** out) {
   DevScratch& s = g_scratch[dev];
   if (!s.last_use) DIRB_CUDA(cudaEventCreateWithFlags(&s.last_use, cudaEventDisableTiming));
   if (bytes > s.bytes) {
-    if (s.ptr) DIRB_CUDA(cudaFree(s.ptr));   // synchronises the device: no earlier user is still running
-    s.ptr = nullptr;
-    s.bytes = 0;
-    const size_t want = (bytes + (size_t(1) << 20) - 1) & ~((size_t(1) << 20) - 1);
-    DIRB_CUDA(cudaMalloc(&s.ptr, want));
-    s.bytes = want;
+    // cudaFree synchronises the device: no earlier user is still running
+    DIRB_TRY(grow_device(&s.ptr, &s.bytes, (bytes + (size_t(1) << 20) - 1) & ~((size_t(1) << 20) - 1)));
   } else {
     DIRB_CUDA(cudaStreamWaitEvent(stream, s.last_use, 0));
   }

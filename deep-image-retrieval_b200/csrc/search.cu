@@ -849,6 +849,12 @@ static int sim_gemm(dirb200_index* h, int epi, const __half* q16, int Q, const _
   }
 }
 
+// Grow the search workspace to `need` bytes.  Cached query maps point into it, so they are dropped when it moves.
+static int grow_ws(dirb200_index* h, size_t need) {
+  if (need > h->ws_bytes) h->tmaps.es.clear();
+  return grow_device(&h->ws, &h->ws_bytes, need);
+}
+
 extern "C" {
 
 int dirb200_index_create(int device, int dim, dirb200_index** out) {
@@ -1022,14 +1028,7 @@ static int search_begin_seed(dirb200_index* h, const float* q32, int Q, int k, i
   const size_t o_kthk = carve(static_cast<size_t>(Q) * 4);
   const size_t o_gates = carve(8 * 4);
   const size_t o_status = carve(ST_WORDS * 8);
-  if (off > h->ws_bytes) {
-    if (h->ws) DIRB_CUDA(cudaFree(h->ws));
-    h->ws = nullptr;
-    h->ws_bytes = 0;
-    DIRB_CUDA(cudaMalloc(&h->ws, off));
-    h->ws_bytes = off;
-    h->tmaps.es.clear();                    // the cached query map pointed into the old workspace
-  }
+  DIRB_TRY(grow_ws(h, off));
   uint8_t* w = static_cast<uint8_t*>(h->ws);
   __half* q16 = reinterpret_cast<__half*>(w + o_q16);
   float* dense = reinterpret_cast<float*>(w + o_dense);
@@ -1188,12 +1187,7 @@ int dirb200_index_search(dirb200_index* h, const float* q32, int Q, int k, doubl
                          void* stream_) {
   DIRB_REQUIRE(h && q32 && scores_dev && idx_dev, DIRB200_EINVAL, "null argument");
   DIRB_REQUIRE(Q > 0, DIRB200_ENOTSUP, "need Q > 0");
-  if (static_cast<size_t>(Q) * 4 > h->sel_bytes) {
-    if (h->sel_own) cudaFree(h->sel_own);
-    h->sel_own = nullptr;
-    DIRB_CUDA(cudaMalloc(reinterpret_cast<void**>(&h->sel_own), static_cast<size_t>(Q) * 4));
-    h->sel_bytes = static_cast<size_t>(Q) * 4;
-  }
+  DIRB_TRY(grow_device(reinterpret_cast<void**>(&h->sel_own), &h->sel_bytes, static_cast<size_t>(Q) * 4));
   DIRB_TRY(dirb200_index_search_begin(h, q32, Q, k, k, h->sel_own, stream_));
   return dirb200_index_search_finish(h, q32, h->sel_own, scores_dev, idx_dev, stream_);
 }
@@ -1247,14 +1241,7 @@ int dirb200_index_rank_count(dirb200_index* h, const float* q32, int Q, const in
   const size_t o_status = carve(ST_WORDS * 8);
   const size_t o_over = carve(static_cast<size_t>(Q) * 4);
   const size_t o_qlist = carve(static_cast<size_t>(Q) * 4);
-  if (off > h->ws_bytes) {
-    if (h->ws) DIRB_CUDA(cudaFree(h->ws));
-    h->ws = nullptr;
-    h->ws_bytes = 0;
-    DIRB_CUDA(cudaMalloc(&h->ws, off));
-    h->ws_bytes = off;
-    h->tmaps.es.clear();
-  }
+  DIRB_TRY(grow_ws(h, off));
   uint8_t* w = static_cast<uint8_t*>(h->ws);
   __half* q16 = reinterpret_cast<__half*>(w + o_q16);
   float* thr = reinterpret_cast<float*>(w + o_thr);
@@ -1338,15 +1325,7 @@ int dirb200_index_count_ge(dirb200_index* h, const float* q32, int Q, const int*
   h->pend.active = false;                        // shares the search workspace
   const int64_t launches0 = launches_total();
   const int cap = h->band_cap > 0 ? h->band_cap : (1 << 20);
-  const size_t need = count_ge_ws_bytes(Q, T, cap);
-  if (need > h->ws_bytes) {
-    if (h->ws) DIRB_CUDA(cudaFree(h->ws));
-    h->ws = nullptr;
-    h->ws_bytes = 0;
-    DIRB_CUDA(cudaMalloc(&h->ws, need));
-    h->ws_bytes = need;
-    h->tmaps.es.clear();
-  }
+  DIRB_TRY(grow_ws(h, count_ge_ws_bytes(Q, T, cap)));
   CountGeArgs a;
   a.q32 = q32; a.Q = Q;
   a.db32 = h->db32; a.N = h->N; a.offset = h->offset; a.D = h->dim;

@@ -243,13 +243,7 @@ class ResNetRMAC:
             x = x.cuda(non_blocking=True)                        # common.variables, common.py:213-215
         x = x.contiguous().float()
         b, _, hgt, wid = x.shape
-        h = self._ensure(x.device.index or 0)
-        with torch.cuda.device(x.device):
-            desc = torch.empty((b, self.descriptor_dim), dtype=torch.float32, device=x.device)
-            d16 = torch.empty((b, self.descriptor_dim), dtype=torch.float16, device=x.device) if want_f16 else None
-            lib.call("dirb200_net_forward", h, C.c_void_p(x.data_ptr()), b, hgt, wid, C.c_void_p(desc.data_ptr()),
-                     C.c_void_p(d16.data_ptr()) if want_f16 else C.c_void_p(0),
-                     C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        desc, d16 = self._forward_dev("dirb200_net_forward", self._ensure(x.device.index or 0), x, hgt, wid, want_f16)
         if want_f16:
             return desc, d16
         if b == 1:
@@ -258,14 +252,26 @@ class ResNetRMAC:
 
     __call__ = forward
 
+    def _forward_dev(self, fn, h, x, hgt, wid, want_f16, *extra):
+        """Device entry point `fn` over the images of the CUDA tensor x, on the current stream of x's device; `extra`
+        goes between (B, H, W) and the outputs.  -> (B, D) fp32 descriptors, and their fp16 copy or None."""
+        b = int(x.shape[0])
+        with torch.cuda.device(x.device):
+            desc = torch.empty((b, self.descriptor_dim), dtype=torch.float32, device=x.device)
+            d16 = torch.empty((b, self.descriptor_dim), dtype=torch.float16, device=x.device) if want_f16 else None
+            lib.call(fn, h, C.c_void_p(x.data_ptr()), b, hgt, wid, *extra, C.c_void_p(desc.data_ptr()),
+                     C.c_void_p(d16.data_ptr() if want_f16 else 0), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        return desc, d16
+
+    def _forward_host(self, fn, h, a, hgt, wid):
+        out = np.empty((a.shape[0], self.descriptor_dim), dtype=np.float32)
+        lib.call(fn, h, a.ctypes.data_as(C.c_void_p), a.shape[0], hgt, wid, out.ctypes.data_as(C.c_void_p))
+        return out
+
     def forward_host(self, imgs: np.ndarray, device=0) -> np.ndarray:
         """Host NCHW fp32 array in, host descriptors out; H2D + forward + D2H inside one C call."""
         a = np.ascontiguousarray(imgs, dtype=np.float32)
-        b, _, hgt, wid = a.shape
-        h = self._ensure(device)
-        out = np.empty((b, self.descriptor_dim), dtype=np.float32)
-        lib.call("dirb200_net_forward_host", h, a.ctypes.data_as(C.c_void_p), b, hgt, wid, out.ctypes.data_as(C.c_void_p))
-        return out
+        return self._forward_host("dirb200_net_forward_host", self._ensure(device), a, a.shape[2], a.shape[3])
 
     def forward_u8(self, imgs_u8: torch.Tensor):
         """uint8 HWC CUDA tensor (B,H,W,3) -> descriptors; ToTensor + Normalize(self.preprocess) run inside the stem."""
@@ -273,10 +279,8 @@ class ResNetRMAC:
             raise TypeError("expected a (B,H,W,3) uint8 CUDA tensor")
         x = imgs_u8.contiguous()
         b, hgt, wid, _ = x.shape
-        h = self._ensure_with_preprocess(x.device.index or 0)
-        desc = torch.empty((b, self.descriptor_dim), dtype=torch.float32, device=x.device)
-        lib.call("dirb200_net_forward_u8", h, C.c_void_p(x.data_ptr()), b, hgt, wid, C.c_void_p(desc.data_ptr()),
-                 C.c_void_p(0), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        desc, _ = self._forward_dev("dirb200_net_forward_u8", self._ensure_with_preprocess(x.device.index or 0), x, hgt,
+                                    wid, False)
         return desc[0] if b == 1 else desc
 
     def forward_ragged_u8(self, imgs):
@@ -316,13 +320,8 @@ class ResNetRMAC:
             raise ValueError("need one (h, w) per slot")
         table = np.ascontiguousarray(np.asarray(hw, dtype=np.int32).reshape(b, 2))
         h = self._ensure_with_preprocess(x.device.index or 0) if u8 else self._ensure(x.device.index or 0)
-        with torch.cuda.device(x.device):
-            desc = torch.empty((b, self.descriptor_dim), dtype=torch.float32, device=x.device)
-            d16 = torch.empty((b, self.descriptor_dim), dtype=torch.float16, device=x.device) if want_f16 else None
-            lib.call("dirb200_net_forward_ragged_u8" if u8 else "dirb200_net_forward_ragged", h, C.c_void_p(x.data_ptr()),
-                     b, hgt, wid, table.ctypes.data_as(C.c_void_p), C.c_void_p(desc.data_ptr()),
-                     C.c_void_p(d16.data_ptr()) if want_f16 else C.c_void_p(0),
-                     C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        desc, d16 = self._forward_dev("dirb200_net_forward_ragged_u8" if u8 else "dirb200_net_forward_ragged", h, x, hgt,
+                                      wid, want_f16, table.ctypes.data_as(C.c_void_p))
         return (desc, d16) if want_f16 else desc
 
     def forward_u8_multiscale(self, imgs_u8: torch.Tensor, scales=(0.7, 1.0, 1.4), pooling="gem", gemp=3):
@@ -347,11 +346,8 @@ class ResNetRMAC:
     def forward_host_u8(self, imgs_u8: np.ndarray, device=0) -> np.ndarray:
         """Host uint8 HWC array (B,H,W,3) in, host descriptors out (H2D of 3 bytes/pixel instead of 12)."""
         a = np.ascontiguousarray(imgs_u8, dtype=np.uint8)
-        b, hgt, wid, _ = a.shape
-        h = self._ensure_with_preprocess(device)
-        out = np.empty((b, self.descriptor_dim), dtype=np.float32)
-        lib.call("dirb200_net_forward_host_u8", h, a.ctypes.data_as(C.c_void_p), b, hgt, wid, out.ctypes.data_as(C.c_void_p))
-        return out
+        return self._forward_host("dirb200_net_forward_host_u8", self._ensure_with_preprocess(device), a, a.shape[1],
+                                  a.shape[2])
 
     def _ensure_with_preprocess(self, device_index):
         h = self._ensure(device_index)

@@ -65,8 +65,7 @@ int dirb200_net_create(const char* arch, int device, dirb200_net** out);
  * "center_bias" b >= 0 (rmac_resnet.py:52-56); "gem_eps" (pooling.py:39, default 1e-6);
  * "mean0".."mean2", "std0".."std2": Normalize constants of the uint8 entry points (default resnet.py:110-111).
  * Scheduling: "chunk" images per pass of the network (0 = auto); "host_chunk" images per pipeline stage of
- * dirb200_net_forward_host (default 16); "stage_sched" 1 = run each stage in L2-sized sub-chunks ("sub0".."sub4"
- * images per sub-chunk of stem / layer1..4), 0 (default, faster as measured) = whole chunk per stage.
+ * dirb200_net_forward_host (default 16).
  * Implementation A/B switches: "conv_impl" 0 = persistent wgmma implicit GEMM (default), 1 = mma.sync implicit
  * GEMM (validation path), 2 = the same kernel with one tile per CTA (baseline); "fuse_ds" 1 (default) = projection
  * shortcut fused into conv3 as a K-concatenated GEMM; "fuse_c23" 0 (default) / 1 / 2 = conv2 + conv3 (+ residual) of the

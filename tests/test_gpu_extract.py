@@ -207,6 +207,26 @@ def test_uint8_input_is_bit_identical_to_fp32_input():
     assert rel_l2(d_u8, ref) < TOL
 
 
+def test_host_pipeline_over_several_chunks_is_bit_identical():
+    """The host-buffer entry points copy chunk i+1 while chunk i runs, in doubling chunks: host_chunk 4 over 23 images
+    runs chunks of 2, 2, 4, 8 and 7 images.  They give the device entry points' descriptors bit for bit.  The removed
+    sub-chunk schedule options are unknown keys."""
+    from dirb200 import lib
+    net, _ = _net("resnet50_rmac", 0)
+    u8 = synth.make_images_u8(23, 64, 96, seed=5)
+    x = synth.normalise_images(u8)
+    d = net(x.cuda()).cpu().numpy()
+    d_u8 = net.forward_u8(torch.from_numpy(u8).cuda()).cpu().numpy()
+    net.set_backend_option("host_chunk", 4)
+    assert np.array_equal(net.forward_host(x.numpy()), d)
+    assert np.array_equal(net.forward_host_u8(u8), d_u8)
+    for key, value in (("stage_sched", 1), ("sub0", 8)):
+        net, _ = _net("resnet50_rmac", 0)
+        net.set_backend_option(key, value)
+        with pytest.raises(lib.DirbError):
+            net(x[:1].cuda())
+
+
 @pytest.mark.parametrize("size", [(717, 717), (1434, 1434), (64, 48), (333, 517)], ids=lambda s: "%dx%d" % s)
 def test_odd_and_multiscale_sizes_vs_oracle(size):
     """BASELINE configs[4] scales of a 1024^2 image (Scale(0.7) -> 717, Scale(1.4) -> 1434, transforms.py:168) plus tiny
