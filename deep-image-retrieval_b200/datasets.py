@@ -50,6 +50,10 @@ class Dataset:
             img = img.resize(resize, Image.LANCZOS if np.prod(resize) < np.prod(img.size) else Image.BICUBIC)
         return img
 
+    def get_image_source(self, i):
+        """(file name, crop box or None) that get_image(i) decodes: lets the extraction decode the file itself."""
+        return self.get_filename(i), None
+
     def get_label(self, i, toint=False):
         raise NotImplementedError()
 
@@ -233,6 +237,9 @@ class ImageListROIs(Dataset):
         if resize:
             img = img.resize(resize, Image.LANCZOS if np.prod(resize) < np.prod(img.size) else Image.BICUBIC)
         return img
+
+    def get_image_source(self, i):
+        return self.get_filename(i), tuple(self.rois[i])
 
 
 class ImageListRelevants(Dataset):

@@ -50,6 +50,12 @@ SIGNATURES = {
     "dirb200_net_forward_ragged": (i32, [p, p, i32, i32, i32, p, p, p, p]),
     "dirb200_resize_bilinear_u8": (i32, [p, i32, i32, i32, i32, i32, p, p]),
     "dirb200_resize_coeffs": (i32, [i32, i32, p, p, C.POINTER(i32)]),
+    "dirb200_jpeg_probe": (i32, [p, C.c_size_t, C.POINTER(i32)]),
+    "dirb200_jpeg_decoder_create": (i32, [i32, C.POINTER(p)]),
+    "dirb200_jpeg_decoder_set_option": (i32, [p, C.c_char_p, f64]),
+    "dirb200_jpeg_decoder_decode": (i32, [p, i32, p, p, p, p, p, C.POINTER(i32), p]),
+    "dirb200_jpeg_debug_coefficients": (i32, [p, i32, p, C.c_size_t, C.POINTER(i32), p]),
+    "dirb200_jpeg_decoder_destroy": (i32, [p]),
     "dirb200_net_debug_stage": (i32, [p, C.c_char_p, p, C.c_size_t, C.POINTER(i32), p]),
     "dirb200_net_profile": (i32, [p, C.POINTER(f64)]),
     "dirb200_net_profile_table": (i32, [p, p, C.c_size_t, C.POINTER(C.c_size_t)]),

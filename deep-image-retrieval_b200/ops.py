@@ -134,6 +134,92 @@ def resize_coeffs(in_size, out_size):
     return bounds, kk
 
 
+def _bytes_ptr(buf):
+    """(pointer, size, keep-alive) of a host byte buffer: a uint8 CPU tensor, bytes or a numpy array."""
+    if isinstance(buf, torch.Tensor):
+        t = buf.contiguous()
+        return t.data_ptr(), t.numel(), t
+    a = np.ascontiguousarray(np.frombuffer(buf, np.uint8) if isinstance(buf, (bytes, bytearray, memoryview)) else buf,
+                             dtype=np.uint8)
+    return a.ctypes.data, a.size, a
+
+
+def jpeg_probe(buf):
+    """Host-only header parse of a JPEG held in memory -> (status, info).  status 0: the GPU decoder takes it;
+    DIRB200_ENOTSUP (-2): a JPEG it does not take; DIRB200_EINVAL (-1): not a (complete) JPEG.  info = dict(height,
+    width, components, h_samp, v_samp, restart_interval, color, scan_bytes) as far as the header was read."""
+    ptr, n, keep = _bytes_ptr(buf)
+    info = (C.c_int * 8)()
+    status = lib.raw("dirb200_jpeg_probe")(C.c_void_p(ptr), n, info)
+    del keep
+    keys = ("height", "width", "components", "h_samp", "v_samp", "restart_interval", "color", "scan_bytes")
+    return status, dict(zip(keys, list(info)))
+
+
+class JpegDecoder:
+    """Batched baseline-JPEG decoder on one GPU, byte-identical to np.array(Image.open(f).convert("RGB"))."""
+
+    def __init__(self, device=None, subseq_bits=None):
+        self.device = torch.cuda.current_device() if device is None else int(device)
+        h = C.c_void_p()
+        lib.call("dirb200_jpeg_decoder_create", self.device, C.byref(h))
+        self._h = h
+        self.last_rounds = 0
+        if subseq_bits is not None:
+            self.set_option("subseq_bits", subseq_bits)
+
+    def set_option(self, key, value):
+        lib.call("dirb200_jpeg_decoder_set_option", self._h, key.encode(), float(value))
+
+    def decode(self, bufs):
+        """List of JPEG files in host memory (uint8 CPU tensors, bytes or arrays) -> (list of (h, w, 3) uint8 CUDA
+        tensors, bool list ok).  One upload for the whole list.  ok[i] False: file i was refused by the header parser
+        or its entropy-coded data did not decode cleanly; its tensor is then undefined (decode it with PIL)."""
+        n = len(bufs)
+        if n == 0:
+            return [], []
+        held = [_bytes_ptr(b) for b in bufs]
+        shapes, offs, total = [], [], 0
+        for ptr, size, _ in held:
+            info = (C.c_int * 8)()
+            st = lib.raw("dirb200_jpeg_probe")(C.c_void_p(ptr), size, info)
+            h, w = (info[0], info[1]) if st == 0 else (0, 0)
+            shapes.append((h, w))
+            offs.append(total)
+            total += h * w * 3
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.device(dev):
+            out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+            status = torch.empty(n, dtype=torch.int32, device=dev)
+            ptrs = (C.c_void_p * n)(*[p for p, _, _ in held])
+            sizes = (C.c_size_t * n)(*[s for _, s, _ in held])
+            offsets = (C.c_int64 * n)(*offs)
+            rounds = C.c_int()
+            lib.call("dirb200_jpeg_decoder_decode", self._h, n, ptrs, sizes, _ptr(out), offsets, _ptr(status), C.byref(rounds),
+                     _stream())
+            self.last_rounds = rounds.value
+            ok = (status.cpu().numpy() == 0).tolist()
+        del held
+        imgs = [out[o:o + h * w * 3].view(h, w, 3) for o, (h, w) in zip(offs, shapes)]
+        return imgs, ok
+
+    def debug_coefficients(self, image):
+        """int16 (nblocks, 64) coefficients of image `image` of the last decode (natural order, MCU order, DC
+        prediction applied)."""
+        nb = C.c_int()
+        lib.call("dirb200_jpeg_debug_coefficients", self._h, int(image), C.c_void_p(0), 0, C.byref(nb), _stream())
+        out = torch.empty((nb.value, 64), dtype=torch.int16, device=torch.device("cuda", self.device))
+        lib.call("dirb200_jpeg_debug_coefficients", self._h, int(image), _ptr(out), out.numel() * 2, C.byref(nb),
+                 _stream())
+        return out
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h is not None and h.value:
+            lib.raw("dirb200_jpeg_decoder_destroy")(h)
+            self._h = None
+
+
 def maxpool_3x3s2(x):
     _chk(x, torch.float16, "x")
     b, h, w, c = x.shape

@@ -153,17 +153,72 @@ def _ragged_window(net, imgs, batch_size):
     return torch.cat(out, dim=0)
 
 
-class _RawImages(torch.utils.data.Dataset):
-    """Decoded images as uint8 HWC tensors (the decode stays on CPU workers; everything after it runs on the GPU)."""
+# Baseline JPEGs are decoded on the GPU (ops.JpegDecoder, byte-identical to PIL) in calls of one window of images:
+# the ragged window, or JPEG_WINDOW images when images go through the network one at a time.  False: PIL decodes
+# every file on the loader workers.
+GPU_JPEG = True
+JPEG_WINDOW = 16
 
-    def __init__(self, dataset):
-        self.dataset = dataset
+
+def _image_source(dataset):
+    """dataset.get_image_source where get_image is exactly the decode (+ ROI crop) that it describes, else None (a
+    dataset that overrides get_image keeps its own decode)."""
+    if isinstance(dataset, _RowRange):
+        return dataset.get_image_source if _image_source(dataset.dataset) else None
+    if type(dataset).get_image in (datasets.Dataset.get_image, datasets.ImageListROIs.get_image):
+        return dataset.get_image_source
+    return None
+
+
+def crop_u8(x, box):
+    """Image.crop(box) of a uint8 HWC tensor: PIL rounds the box with round() (half to even) and fills 0 outside."""
+    x0, y0, x1, y1 = (int(round(v)) for v in box)
+    h, w = int(x.shape[0]), int(x.shape[1])
+    if (x0, y0, x1, y1) == (0, 0, w, h):
+        return x
+    out = x.new_zeros((max(y1 - y0, 0), max(x1 - x0, 0), 3))
+    sy0, sy1, sx0, sx1 = max(y0, 0), min(y1, h), max(x0, 0), min(x1, w)
+    if sy1 > sy0 and sx1 > sx0:
+        out[sy0 - y0:sy1 - y0, sx0 - x0:sx1 - x0] = x[sy0:sy1, sx0:sx1]
+    return out
+
+
+class _RawImages(torch.utils.data.Dataset):
+    """Images for the GPU preprocessing path, as (data, is_jpeg, crop box).  With a source (_image_source), a file the
+    GPU decoder takes comes back as its bytes (uint8 tensor) and its crop box; anything else is decoded here with
+    PIL, as uint8 HWC pixels (crop applied)."""
+
+    def __init__(self, dataset, source=None):
+        self.dataset, self.source = dataset, source
 
     def __len__(self):
         return len(self.dataset)
 
     def __getitem__(self, i):
-        return torch.from_numpy(np.array(self.dataset.get_image(i).convert("RGB"), dtype=np.uint8))
+        if self.source is not None:
+            fname, box = self.source(i)
+            with open(fname, "rb") as f:
+                data = f.read()
+            if ops.jpeg_probe(data)[0] == 0:
+                return torch.frombuffer(bytearray(data), dtype=torch.uint8), True, box
+        return torch.from_numpy(np.array(self.dataset.get_image(i).convert("RGB"), dtype=np.uint8)), False, None
+
+
+def _decode_window(items, first, dataset, decoder):
+    """Loader items of images first, first + 1, ... -> their uint8 HWC pixels on the GPU.  The JPEGs go through one
+    decoder call; a file whose data does not decode cleanly there is decoded again with PIL."""
+    imgs = [None] * len(items)
+    jpeg = [k for k, it in enumerate(items) if it[1]]
+    if jpeg:
+        dec, ok = decoder.decode([items[k][0] for k in jpeg])
+        for k, x, good in zip(jpeg, dec, ok):
+            if good:
+                imgs[k] = crop_u8(x, items[k][2]) if items[k][2] is not None else x
+    for k, it in enumerate(items):
+        if imgs[k] is None:
+            px = it[0] if not it[1] else torch.from_numpy(np.array(dataset.get_image(first + k).convert("RGB"), np.uint8))
+            imgs[k] = px.cuda(non_blocking=True)
+    return imgs
 
 
 def extract_image_features(dataset, transforms, net, ret_imgs=False, same_size=False, flip=None,
@@ -186,28 +241,39 @@ def extract_image_features(dataset, transforms, net, ret_imgs=False, same_size=F
     if hasattr(net, "eval"):
         net.eval()
     if scale is not None:
-        loader = torch.utils.data.DataLoader(_RawImages(dataset), batch_size=None, shuffle=False,
+        source = _image_source(dataset) if GPU_JPEG else None
+        decoder = ops.JpegDecoder() if source is not None else None
+        loader = torch.utils.data.DataLoader(_RawImages(dataset, source), batch_size=None, shuffle=False,
                                              num_workers=max(0, threads if threads > 1 else 0), pin_memory=True)
-        img_feats, pending = [], []
-        for img in tqdm.tqdm(loader, desc, total=len(dataset)):
-            x = img.cuda(non_blocking=True)
-            if flip and flip.pop(0):
-                x = x.flip(1)                            # horizontal flip (imgs[i].flip(2) on CHW, test_dir.py:70-72)
-            h, w = int(x.shape[0]), int(x.shape[1])
-            oh, ow = int(0.5 + scale * h), int(0.5 + scale * w)          # Scale.get_params, transforms.py:168
-            x = x.unsqueeze(0).contiguous()
-            if (oh, ow) != (h, w) and min(oh, ow) != min(h, w):          # Scale.__call__: can_upscale / can_downscale
-                x = ops.resize_bilinear_u8(x, (oh, ow))
-            if ragged:
-                pending.append(x[0])
-                if len(pending) == window:
-                    img_feats.append(_ragged_window(net, pending, group))
-                    pending = []
-                continue
-            d = net.forward_u8(x)
-            img_feats.append(d.unsqueeze(0) if d.dim() == 1 else d)
-        if pending:
-            img_feats.append(_ragged_window(net, pending, group))
+        img_feats, items, done = [], [], 0
+        step = window if ragged else (JPEG_WINDOW if decoder is not None else 1)
+
+        def run(items, first):
+            pending = []
+            for x in _decode_window(items, first, dataset, decoder):
+                if flip and flip.pop(0):
+                    x = x.flip(1)                        # horizontal flip (imgs[i].flip(2) on CHW, test_dir.py:70-72)
+                h, w = int(x.shape[0]), int(x.shape[1])
+                oh, ow = int(0.5 + scale * h), int(0.5 + scale * w)      # Scale.get_params, transforms.py:168
+                x = x.unsqueeze(0).contiguous()
+                if (oh, ow) != (h, w) and min(oh, ow) != min(h, w):      # Scale.__call__: can_upscale / can_downscale
+                    x = ops.resize_bilinear_u8(x, (oh, ow))
+                if ragged:
+                    pending.append(x[0])
+                    continue
+                d = net.forward_u8(x)
+                img_feats.append(d.unsqueeze(0) if d.dim() == 1 else d)
+            if pending:
+                img_feats.append(_ragged_window(net, pending, group))
+
+        for item in tqdm.tqdm(loader, desc, total=len(dataset)):
+            items.append(item)
+            if len(items) == step:
+                run(items, done)
+                done += len(items)
+                items = []
+        if items:
+            run(items, done)
         return torch.cat(img_feats, dim=0)
     loader = get_loader(dataset, trf_chain=transforms, preprocess=net.preprocess, iscuda=iscuda, output=["img"],
                         batch_size=batch_size, threads=threads, shuffle=False)
@@ -468,6 +534,9 @@ class _RowRange:
 
     def get_image(self, i, resize=None):
         return self.dataset.get_image(self.start + i, resize=resize)
+
+    def get_image_source(self, i):
+        return self.dataset.get_image_source(self.start + i)
 
 
 def extract_to_store(db, net, trfs, store_path, pooling="mean", gemp=3, whiten=None, threads=8, batch_size=16,

@@ -115,6 +115,34 @@ int dirb200_net_forward_ragged(dirb200_net* net, const float* slots_dev, int B, 
  * call with kk_out == NULL to query ksize). */
 int dirb200_resize_bilinear_u8(const uint8_t* in_dev, int B, int H, int W, int Ho, int Wo, uint8_t* out_dev, void* stream);
 int dirb200_resize_coeffs(int in_size, int out_size, int* bounds_out, int* kk_out, int* ksize_out);
+/* ------------------------------------------------------------------ baseline JPEG decoding
+ * Replaces Image.open(f).convert("RGB") (dirtorch/datasets/dataset.py:52, dirtorch/datasets/generic.py:246) for
+ * baseline JPEGs: the RGB pixels equal, byte for byte, what PIL (libjpeg-turbo, default ISLOW IDCT, fancy upsampling)
+ * returns.  Supported: 8-bit baseline / extended-sequential Huffman, one interleaved scan of all components, 1 component
+ * (grey, replicated to RGB) or 3 with luma sampling 1x1, 2x1 or 2x2 and chroma 1x1, any restart interval.
+ * dirb200_jpeg_probe (host only) parses the markers: info = {height, width, components, luma h-sampling, luma
+ * v-sampling, restart interval, colour (0 YCbCr, 1 RGB, 2 grey), entropy-coded bytes}; returns 0 if the decoder takes
+ * the file, DIRB200_ENOTSUP for a well-formed JPEG it does not (progressive, arithmetic, 12-bit, CMYK, multi-scan,
+ * other sampling, DNL, Huffman tables with an all-ones code) and DIRB200_EINVAL for anything else (not a JPEG,
+ * truncated, malformed).
+ * The decoder handle owns pinned staging and device workspace, grown on demand.  dirb200_jpeg_decoder_decode decodes n images
+ * (host buffers data_host[i] of sizes_host[i] bytes) in one upload: image i goes to out_dev + out_offsets_host[i] as
+ * (h, w, 3) uint8 and status_dev[i] (device int32) is 0 when it was decoded; non-zero: the probe's code for files the
+ * host parser refused, or a positive mask (1 marker in the scan, 2 restart markers, 4 block count of a restart segment, 8 invalid code)
+ * when the entropy-coded data does not decode cleanly - the caller decodes such a file with PIL.  rounds_out (may be
+ * NULL) = synchronisation rounds that changed a state.  Waits on the stream once per four synchronisation rounds.
+ * Option "subseq_bits" (default 1024, multiple of 32 in [64, 2^20]): bits per subsequence of the parallel Huffman
+ * decode.  dirb200_jpeg_debug_coefficients copies image `image` of the last decode's coefficients, int16 [nblocks][64]
+ * in natural order, blocks in MCU order, DC prediction applied (dst_dev = NULL: *nblocks only). */
+int dirb200_jpeg_probe(const uint8_t* data, size_t size, int info[8]);
+typedef struct dirb200_jpeg_decoder dirb200_jpeg_decoder;
+int dirb200_jpeg_decoder_create(int device, dirb200_jpeg_decoder** out);
+int dirb200_jpeg_decoder_set_option(dirb200_jpeg_decoder* dec, const char* key, double value);
+int dirb200_jpeg_decoder_decode(dirb200_jpeg_decoder* dec, int n, const uint8_t* const* data_host, const size_t* sizes_host,
+                        uint8_t* out_dev, const int64_t* out_offsets_host, int* status_dev, int* rounds_out, void* stream);
+int dirb200_jpeg_debug_coefficients(dirb200_jpeg_decoder* dec, int image, int16_t* dst_dev, size_t capacity, int* nblocks,
+                                    void* stream);
+int dirb200_jpeg_decoder_destroy(dirb200_jpeg_decoder* dec);
 /* Debug tap (needs option "debug_taps"): copy the NHWC fp16 activation after stage `what` ("stem","layer1".."layer4")
  * of the LAST chunk of the last forward into dst_dev (capacity in bytes); returns its dims as {n,h,w,c}. */
 int dirb200_net_debug_stage(dirb200_net* net, const char* what, void* dst_dev, size_t capacity, int dims[4],
