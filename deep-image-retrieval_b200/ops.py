@@ -391,14 +391,18 @@ class Index:
     def __init__(self, db32: torch.Tensor, index_offset: int = 0, db16: torch.Tensor = None, check_norms: bool = True):
         """check_norms: the exactness of the top-k rests on |fp16-path score - exact score| <= eps16 = 1.2e-3, which is
         derived for UNIT-NORM rows and queries (what pooling / whitening / query expansion produce).  Rows with larger
-        norms are refused here instead of silently returning an inexact list; pass check_norms=False and set option
-        'eps16' to 1.2e-3 * max|q| * max|row| to search un-normalised data."""
+        norms are refused here instead of silently returning an inexact list.  To search un-normalised data, either
+        scale queries and rows to unit norm (the order does not change), or pass check_norms=False and set option
+        'eps16' to 1.2e-3 * max|q| * max|row| + 2^-24 * sqrt(D) * (max|q| + max|row|) (norms of queries and rows, D the
+        dimension): below 2^-14 fp16 is subnormal and rounds to an absolute 2^-25 per entry, which the first term
+        alone does not cover for small norms.  Every entry must stay below fp16's largest value, 65504."""
         _chk(db32, torch.float32, "db32")
         if check_norms and db32.shape[0]:
             worst = float(torch.linalg.vector_norm(db32, dim=1).max())
             if worst > 1.0 + 1e-3:
                 raise ValueError("database rows are not unit-norm (max norm %.4g): the exact-top-k error bound assumes |row| <= 1; "
-                                 "normalise them, or pass check_norms=False and set option 'eps16' accordingly" % worst)
+                                 "normalise them, or pass check_norms=False and set option 'eps16' to 1.2e-3*max|q|*max|row| "
+                                 "+ 2^-24*sqrt(D)*(max|q| + max|row|) (entries below 65504)" % worst)
         self.db32 = db32
         self.n, self.dim = db32.shape
         if db16 is None:                      # an empty shard (more ranks than rows) has nothing to convert
