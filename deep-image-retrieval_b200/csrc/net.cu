@@ -629,6 +629,7 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
     DIRB_TRY(stem_tc(imgs, cb, H, W, n->stem_w2, n->stem.scale, n->stem.shift, w.stem_ws, w.stem_out, stream, imgs_u8,
                      n->mean_std, ext(e0, 0, W), ext(e1, 1, lw[1])));
   }
+  DIRB_TRY(record_tap(n, "stem_conv", w.stem_out, cb, lh[1], lw[1], 64, stream));
   {
     ProfScope ps(n, stream, 2, 0, 2.0 * cb * 64 * (static_cast<double>(lh[1]) * lw[1] + static_cast<double>(lh[2]) * lw[2]), "maxpool 3x3/s2");
     DIRB_TRY(maxpool_3x3s2(w.stem_out, cb, lh[1], lw[1], 64, w.stage_out[0], stream, ext(e0, 2, lw[2])));
@@ -651,21 +652,29 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
       __half* rs = w.scratch[2];
       __half* y = (j % 2 == 0) ? w.scratch[3] : w.scratch[2];
       if (bi == last - 1 && s < 4) y = w.stage_out[s];
+      // debug taps of this block: "layerL.B" (its output) and "layerL.B.conv1" / ".conv2" / ".down" (L = s, B = j, as
+      // in the state-dict keys)
+      const std::string tp = "layer" + std::to_string(s) + "." + std::to_string(j);
+      const int cm = blk.c1.Cout, cout = n->stage_ch[s];
       if (n->basic) {
         // BasicBlock, resnet.py:27-44: 3x3(stride) + BN + ReLU -> 3x3 + BN -> + (projected) x -> ReLU
         DIRB_TRY(run_conv(n, blk.c1, x, cb, h, wd, nullptr, 1, t1, stream, 0,
                           blk.c1.stride == 1 ? ext3(e0, lvl, w2, 2, halo_order_plain(n, h2, w2)) : ext(e0, lvl, w2)));
+        DIRB_TRY(record_tap(n, tp + ".conv1", t1, cb, h2, w2, cm, stream));
         const __half* res = x;
         if (blk.has_down) {
           DIRB_TRY(run_conv(n, blk.down, x, cb, h, wd, nullptr, 0, rs, stream, 0, ext(e0, lvl, w2)));
+          DIRB_TRY(record_tap(n, tp + ".down", rs, cb, h2, w2, cout, stream));
           res = rs;
         }
         DIRB_TRY(run_conv(n, blk.c2, t1, cb, h2, w2, res, 1, y, stream, 0, ext3(e0, lvl, w2, 2, halo_order_plain(n, h2, w2))));
+        DIRB_TRY(record_tap(n, tp, y, cb, h2, w2, cout, stream));
         x = y;
         continue;
       }
       const int st = blk.c2.stride;
       DIRB_TRY(run_conv(n, blk.c1, x, cb, h, wd, nullptr, 1, t1, stream, 0, ext(e0, lvl_in, wd)));
+      DIRB_TRY(record_tap(n, tp + ".conv1", t1, cb, h, wd, cm, stream));
       const bool c23 = !blk.has_down && st == 1 && c23_taken(n, cb, h, wd, blk.c2.Cin);
       // ragged: a stride-1 conv2 in the K order of the slot's kernel choice (the fused kernel has the HALO order)
       const ConvExt* e2 = st == 1 ? ext3(e1, lvl, wd, blk.has_down ? 2 : 3, c23 || halo_order_plain(n, h, wd))
@@ -681,10 +690,12 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
         ProfScope ps(n, stream, 0, flops, bytes, tg);
         DIRB_TRY(conv_c23(cb, h, wd, Cm, t1, blk.c2.w, blk.c2.scale, blk.c2.shift, blk.c3.w, blk.c3.scale, blk.c3.shift, x, y,
                           stream, e2));
+        DIRB_TRY(record_tap(n, tp, y, cb, h, wd, cout, stream));
         x = y;
         continue;
       }
       DIRB_TRY(run_conv(n, blk.c2, t1, cb, h, wd, nullptr, 1, t2, stream, 0, e2));
+      DIRB_TRY(record_tap(n, tp + ".conv2", t2, cb, h2, w2, cm, stream));
       if (blk.has_down && n->fuse_ds && n->conv_impl == 0 && blk.c3.Cout % 256 == 0) {
         const double flops = 2.0 * cb * h2 * w2 * static_cast<double>(blk.c3.Cout) * (blk.c3.Cin + blk.down.Cin);
         const double bytes = 2.0 * (static_cast<double>(cb) * h2 * w2 * (blk.c3.Cin + blk.c3.Cout) +
@@ -696,15 +707,18 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
         ProfScope ps(n, stream, 0, flops, bytes, tbuf_);
         DIRB_TRY(conv_fused_ds(cb, h2, w2, blk.c3.Cin, t2, h, wd, blk.down.Cin, st, x, blk.wcat, blk.c3.Cout, blk.ones,
                                blk.cat_shift, y, stream, ext(e0, lvl, w2)));
+        DIRB_TRY(record_tap(n, tp, y, cb, h2, w2, cout, stream));
         x = y;
         continue;
       }
       const __half* res = x;
       if (blk.has_down) {
         DIRB_TRY(run_conv(n, blk.down, x, cb, h, wd, nullptr, 0, rs, stream, 0, ext(e0, lvl, w2)));
+        DIRB_TRY(record_tap(n, tp + ".down", rs, cb, h2, w2, cout, stream));
         res = rs;
       }
       DIRB_TRY(run_conv(n, blk.c3, t2, cb, h2, w2, res, 1, y, stream, 0, ext(e0, lvl, w2)));
+      DIRB_TRY(record_tap(n, tp, y, cb, h2, w2, cout, stream));
       x = y;
     }
     if (s < 4) DIRB_TRY(record_tap(n, "layer" + std::to_string(s), w.stage_out[s], cb, lh[2 + s], lw[2 + s], n->stage_ch[s], stream));
@@ -723,10 +737,12 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
       __half* tbuf = w.scratch[0];
       __half* x4p = w.scratch[1];
       DIRB_TRY(run_conv(n, n->fpn_lat, x, cb, ho, wo, nullptr, 1, tbuf, stream));
+      DIRB_TRY(record_tap(n, "fpn_lat", tbuf, cb, ho, wo, C3, stream));
       {
         ProfScope ps(n, stream, 2, 0, 2.0 * cb * (2.0 * h3 * w3 + static_cast<double>(ho) * wo) * C3);
         DIRB_TRY(upsample_add(x4, tbuf, x4p, cb, h3, w3, ho, wo, C3, stream));
       }
+      DIRB_TRY(record_tap(n, "fpn_merge", x4p, cb, h3, w3, C3, stream));
       DIRB_TRY(run_conv(n, n->fpn_smooth, x4p, cb, h3, w3, nullptr, 1, tbuf, stream));
       x4 = tbuf;
       DIRB_TRY(record_tap(n, "fpn_c4", x4, cb, h3, w3, C3, stream));

@@ -357,7 +357,9 @@ class ResNetRMAC:
         return h
 
     def debug_stage(self, what):
-        """NHWC fp16 activation after 'stem' / 'layer1'..'layer4' of the last chunk of the last forward."""
+        """NHWC fp16 activation `what` of the last chunk of the last forward (option 'debug_taps' 1): 'stem_conv',
+        'stem', 'layerL.B.conv1' / '.conv2' / '.down', 'layerL.B', 'layer1'..'layer4', 'fpn_lat', 'fpn_merge',
+        'fpn_c4' (see dirb200_net_debug_stage in include/dirb200.h)."""
         dims = (C.c_int * 4)()
         dev = torch.device("cuda", self._handle_device)
         buf = torch.empty(1 << 28, dtype=torch.uint8, device=dev)

@@ -143,8 +143,12 @@ int dirb200_jpeg_decoder_decode(dirb200_jpeg_decoder* dec, int n, const uint8_t*
 int dirb200_jpeg_debug_coefficients(dirb200_jpeg_decoder* dec, int image, int16_t* dst_dev, size_t capacity, int* nblocks,
                                     void* stream);
 int dirb200_jpeg_decoder_destroy(dirb200_jpeg_decoder* dec);
-/* Debug tap (needs option "debug_taps"): copy the NHWC fp16 activation after stage `what` ("stem","layer1".."layer4")
- * of the LAST chunk of the last forward into dst_dev (capacity in bytes); returns its dims as {n,h,w,c}. */
+/* Debug tap (needs option "debug_taps"): copy the NHWC fp16 activation `what` of the LAST chunk of the last forward
+ * into dst_dev (capacity in bytes); returns its dims as {n,h,w,c}.  Names: "stem_conv" (stem convolution, before the
+ * maxpool), "stem" (after it), "layerL.B.conv1" / "layerL.B.conv2" / "layerL.B.down" (outputs of block B of layer L,
+ * L = 1..4, as in the state-dict keys; conv2 only where it reaches memory, i.e. not inside conv_c23, and down only
+ * where the projection shortcut is not fused into conv3), "layerL.B" (block output), "layer1".."layer4" (stage
+ * outputs), and for FPN heads "fpn_lat" (conv1x5), "fpn_merge" (after the upsample-add) and "fpn_c4" (conv3c4). */
 int dirb200_net_debug_stage(dirb200_net* net, const char* what, void* dst_dev, size_t capacity, int dims[4],
                             void* stream);
 /* Per-class CUDA-event timing of the last forward run with option "profile" = 1: out16 = 4 rows of
