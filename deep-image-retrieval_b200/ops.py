@@ -261,7 +261,19 @@ def pool_scales(xs, pooling="mean", gemp=3, l2=True):
     return out
 
 
+def center_bias(feat, b):
+    """In place on an NHWC fp16 map: feat *= 1 + bilinear(align_corners=True) resize of the 4x4 map holding b on its
+    central 2x2 (rmac_resnet.py:52-56).  Returns feat."""
+    _chk(feat, torch.float16, "feat")
+    n, h, w, c = feat.shape
+    lib.call("dirb200_center_bias", _ptr(feat), n, h, w, c, float(b), _stream())
+    return feat
+
+
 def l2_normalize(x, eps=1e-12, want_f16=False):
+    """Rows x / max(||x||, eps) in fp32 (eps 0: x / ||x||, NaN for a zero row), optionally with an fp16 copy equal to
+    out.half().  The sum of squares is fp32: rows need 2^-63 < ||x|| < 2^64.  Below, the squares underflow (such a row
+    is below any eps > 0 and comes out x / eps); above, the sum overflows and the row comes out 0."""
     _chk(x, torch.float32, "x")
     n, d = x.shape
     out = torch.empty_like(x)

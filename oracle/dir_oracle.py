@@ -91,9 +91,9 @@ def gem(x, p, eps=1e-6):
     return x.clamp(min=eps).pow(p).mean(dim=(2, 3)).pow(1.0 / p)
 
 
-def center_bias_map(b, h, w):
+def center_bias_map(b, h, w, dtype=torch.float32):
     """1 + bilinear(align_corners=True) resize to (h, w) of the 4x4 map with b on its central 2x2, rmac_resnet.py:52-55."""
-    m = torch.zeros(1, 1, 4, 4)
+    m = torch.zeros(1, 1, 4, 4, dtype=dtype)
     m[0, 0, 1:3, 1:3] = float(b)
     return F.interpolate(1 + m, size=(h, w), mode="bilinear", align_corners=True)
 

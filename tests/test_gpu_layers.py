@@ -5,18 +5,17 @@ import pytest
 import torch
 
 import layer_model as LM
+import post_model as PM
 import synthdata as synth
-from oracle import dir_oracle as O
-from conftest import rel_l2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
 
-def _net(arch, sd, chunk, **opts):
+def _net(arch, sd, chunk, model_kw=None, **opts):
     from dirb200 import nets, ops
     ops.require_gpu(0)
-    net = nets.create_model(arch)
+    net = nets.create_model(arch, **(model_kw or {}))
     net.load_state_dict(sd)
     net.eval()
     for k, v in dict(debug_taps=1, fuse_c23=0, chunk=chunk, **opts).items():
@@ -34,17 +33,35 @@ def _taps(net):
     return tap
 
 
-def _head_check(arch, sd, tap, d):
-    """The head from the layer4 (and FPN layer3) taps in fp64 vs the descriptors: 2e-5 rel."""
-    sd64 = {k: v.double() for k, v in sd.items() if v.is_floating_point()}
-    x5 = tap("layer4").double().cpu().permute(0, 3, 1, 2)
+def _head_check(arch, sd, tap, d, center_bias=0.0):
+    """The head from the layer4 (and FPN fpn_c4) taps against the end-to-end bound of tests/post_model.py: every phase's
+    bound propagated to the descriptor.  center_bias > 0: the taps precede it, so the head input is the fp64 x * m with
+    the fp16 rounding of the center-bias output (one fp16 ulp plus its own bound) as input uncertainty."""
+    w, b = sd["fc.weight"].to(DEV), sd["fc.bias"].to(DEV)
+
+    def flat(t):
+        return t.reshape(t.shape[0], -1, t.shape[-1])
+
+    x5 = tap("layer4")
     if "_fpn" in arch:
-        x4 = tap("fpn_c4").double().cpu().permute(0, 3, 1, 2)
-        v = torch.cat([O.gem(x4, sd["adpoolc4.p"].item()), O.gem(x5, sd["adpoolx5.p"].item())], dim=1)
-        ref = torch.nn.functional.normalize(torch.nn.functional.linear(v, sd64["fc.weight"], sd64["fc.bias"]), dim=-1)
+        parts = [PM.head_partial_ref(flat(tap(n)), "gem", sd[k].item(), 1e-6) for n, k in (("fpn_c4", "adpoolc4.p"),
+                                                                                         ("layer4", "adpoolx5.p"))]
+        hw = [flat(tap("fpn_c4")).shape[1], flat(x5).shape[1]]
+        pooled = [PM.head_pool_final_ref(P, n, "gem", sd[k].item(), False, eP)
+                  for (P, eP), n, k in zip(parts, hw, ("adpoolc4.p", "adpoolx5.p"))]
+        g, eg = torch.cat([v[0] for v in pooled], 1), torch.cat([v[1] for v in pooled], 1)
+        y, ey = PM.head_fc_ref(g, w, b, eg)
+        ref, bound = PM.l2_ref(y, ey, eps=1e-12)
     else:
-        ref = O.head(x5, sd64, squeeze=False)
-    assert rel_l2(d.reshape(ref.shape).cpu().numpy(), ref.numpy()) < 2e-5
+        e_in = None
+        x = x5
+        if center_bias > 0:
+            x, e_cb = PM.center_bias_ref(x5, center_bias)
+            e_in = flat(e_cb + PM.ulp16(x * (1 + 2.0 ** -10)))
+        ref, bound = PM.head_e2e(flat(x), "gem", sd["adpool.p"].item(), 1e-6, False, w, b, e_in)
+    c = PM.check("head", d.reshape(ref.shape), ref, bound)
+    print("HEAD %s: ratio %.4f" % (arch, c.ratio))
+    assert c.ok, c.worst
 
 
 def _report(case, reps, expected):
@@ -58,10 +75,10 @@ def _report(case, reps, expected):
     assert not bad, "\n".join("%s: %d / %d elements outside the bound; %s" % (r.name, r.n_fail, r.n, r.worst) for r in bad[:12])
 
 
-def _case(case, arch, sd, x, *, u8=None, head=True, **opts):
+def _case(case, arch, sd, x, *, u8=None, head=True, center_bias=0.0, **opts):
     """Forward x (NCHW fp32) or u8 (B,H,W,3) with taps on, check every launch, the exact operators and the head."""
     B = (u8 if u8 is not None else x).shape[0]
-    net = _net(arch, sd, B, **opts)
+    net = _net(arch, sd, B, model_kw=dict(center_bias=center_bias) if center_bias else None, **opts)
     if u8 is not None:
         d = net.forward_u8(torch.from_numpy(u8).to(DEV))
         x16 = LM.stem_input_u8(u8)
@@ -74,7 +91,7 @@ def _case(case, arch, sd, x, *, u8=None, head=True, **opts):
     reps, _ = LM.check_network(tap, sd, arch, x16.to(DEV), fuse_ds=fuse_ds, conv_impl=impl, device=DEV)
     _report(case, reps, LM.expected_launches(arch, fuse_ds=fuse_ds, conv_impl=impl))
     if head:
-        _head_check(arch, sd, tap, d)
+        _head_check(arch, sd, tap, d, center_bias)
     return net, tap
 
 
@@ -116,6 +133,12 @@ def test_r50_unfused_shortcut():
     """fuse_ds 0: the projection shortcut as its own launch (tap 'down') and conv3 with that residual."""
     _case("r50_fuse_ds0", "resnet50_rmac", synth.make_state_dict("resnet50_rmac", seed=4), synth.make_images(2, 160, 192, seed=9),
           fuse_ds=0)
+
+
+def test_r50_center_bias_head():
+    """center_bias > 0 runs on the layer4 map after its tap: the head is checked against center_bias applied to it."""
+    _case("r50_center_bias", "resnet50_rmac", synth.make_state_dict("resnet50_rmac", seed=10), synth.make_images(2, 250, 190, seed=16),
+          center_bias=1.5)
 
 
 def test_r18_basic_block():
