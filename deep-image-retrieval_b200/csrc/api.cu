@@ -55,6 +55,15 @@ int dirb200_stem_conv(const float* imgs_dev, int B, int H, int W, const void* w2
   return stem_tc(imgs_dev, B, H, W, CH16(w2_dev), scale_dev, shift_dev, H16(ws_dev), H16(out_dev), ST(stream));
 }
 
+int dirb200_stem_pool(const void* imgs_dev, int is_u8, int B, int H, int W, const float* mean_std_host, const void* w2_dev,
+                      const float* scale_dev, const float* shift_dev, void* out_dev, void* stem_dev, void* stream) {
+  DIRB_REQUIRE(imgs_dev && w2_dev && scale_dev && shift_dev && out_dev && (!is_u8 || mean_std_host), DIRB200_EINVAL,
+               "null argument");
+  DIRB_REQUIRE(B > 0 && H > 0 && W > 0, DIRB200_EINVAL, "bad shape");
+  return stem_pool(is_u8 ? nullptr : static_cast<const float*>(imgs_dev), is_u8 ? static_cast<const uint8_t*>(imgs_dev) : nullptr,
+                   mean_std_host, B, H, W, CH16(w2_dev), scale_dev, shift_dev, H16(out_dev), H16(stem_dev), ST(stream));
+}
+
 int dirb200_maxpool_3x3s2(const void* in_dev, int B, int H, int W, int C, void* out_dev, void* stream) {
   DIRB_REQUIRE(in_dev && out_dev && B > 0 && H > 0 && W > 0, DIRB200_EINVAL, "bad arguments");
   return maxpool_3x3s2(CH16(in_dev), B, H, W, C, H16(out_dev), ST(stream));

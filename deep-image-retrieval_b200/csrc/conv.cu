@@ -7,8 +7,11 @@
 // :115-118 (stem).  BatchNorm (eval) is folded by the caller into scale = gamma/sqrt(var+eps), shift = beta-mean*scale.
 #include "conv.h"
 
+#include <algorithm>
+
 #include "conv_c23.cuh"
 #include "conv_pers.cuh"
+#include "conv_stem.cuh"
 
 namespace dirb {
 
@@ -397,6 +400,57 @@ int stem_tc(const float* imgs, int B, int H, int W, const __half* w2, const floa
   DIRB_CUDA(cudaGetLastError());
   const ConvShape s{B, Hs, Wo, 64, 64, 4, 1, 1, 0};      // 4x1 over the row-expanded tensor: Ho = Hs - 3, Wo
   return conv_tc(s, s2d_ws, w2, scale, shift, nullptr, 1, out, stream, out_ext);
+}
+
+int stem_pool(const float* imgs, const uint8_t* imgs_u8, const float* mean_std, int B, int H, int W, const __half* w2,
+              const float* scale, const float* shift, __half* out, __half* stem_out, cudaStream_t stream,
+              const ConvExt* in_ext, const ConvExt* stem_ext, const ConvExt* pool_ext) {
+  DIRB_REQUIRE((imgs != nullptr) != (imgs_u8 != nullptr) && (imgs_u8 == nullptr || mean_std != nullptr), DIRB200_EINVAL,
+               "the fused stem takes fp32 images or uint8 images with their mean / std");
+  DIRB_REQUIRE((in_ext == nullptr) == (stem_ext == nullptr) && (in_ext == nullptr) == (pool_ext == nullptr) &&
+                   (in_ext == nullptr || (in_ext->ld == stem_ext->ld && in_ext->ld == pool_ext->ld)),
+               DIRB200_EINVAL, "the fused stem needs the extents of all three levels of one table");
+  DIRB_REQUIRE(3 * static_cast<int64_t>(H) * W < (int64_t(1) << 31), DIRB200_ENOTSUP, "image of %d x %d pixels too large", H, W);
+  StemPoolParams p{};
+  p.imgs = imgs;
+  p.imgs_u8 = imgs_u8;
+  if (imgs_u8 != nullptr) {
+    p.m0 = mean_std[0]; p.m1 = mean_std[1]; p.m2 = mean_std[2];
+    p.s0 = mean_std[3]; p.s1 = mean_std[4]; p.s2 = mean_std[5];
+  }
+  p.w2 = w2;
+  p.scale = scale;
+  p.shift = shift;
+  p.out = out;
+  p.stem_out = stem_out;
+  int Hs, Ws;
+  stem_dims(H, W, &p.Ho, &p.Wo, &Hs, &Ws);
+  p.H = H;
+  p.W = W;
+  p.Hp = (p.Ho + 2 - 3) / 2 + 1;
+  p.Wp = (p.Wo + 2 - 3) / 2 + 1;
+  p.tiles_x = static_cast<int>(ceil_div(p.Wp, SP_PT));
+  p.tiles_y = static_cast<int>(ceil_div(p.Hp, SP_PT));
+  const int64_t total = static_cast<int64_t>(p.tiles_x) * p.tiles_y * B;
+  DIRB_REQUIRE(total > 0 && total < (int64_t(1) << 31), DIRB200_ENOTSUP, "tile count %lld out of range", (long long)total);
+  p.total_tiles = static_cast<int>(total);
+  if (in_ext != nullptr) {
+    p.ext0 = in_ext->hw;
+    p.ext1 = stem_ext->hw;
+    p.ext2 = pool_ext->hw;
+    p.ext_ld = in_ext->ld;
+  }
+  constexpr int smem = StemPoolSmem::TOTAL;
+  auto kern = imgs_u8 != nullptr ? stem_pool_kernel<true> : stem_pool_kernel<false>;
+  static std::atomic<uint64_t> attr_done{0};
+  if (first_launch_on_device(attr_done)) {
+    DIRB_CUDA(cudaFuncSetAttribute(stem_pool_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    DIRB_CUDA(cudaFuncSetAttribute(stem_pool_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  }
+  const int64_t grid = std::min<int64_t>(total, 2 * num_sms());   // two CTAs per SM (__launch_bounds__ of the kernel)
+  DIRB_CUDA(launch_pdl(kern, dim3(static_cast<unsigned>(grid)), dim3(SP_THREADS), smem, stream, p));
+  count_launch();
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------ mma.sync path

@@ -58,6 +58,13 @@ size_t stem_workspace_bytes(int B, int H, int W);
 int stem_tc(const float* imgs, int B, int H, int W, const __half* w2, const float* scale, const float* shift,
             __half* s2d_ws, __half* out, cudaStream_t stream, const uint8_t* imgs_u8 = nullptr,
             const float* mean_std = nullptr, const ConvExt* in_ext = nullptr, const ConvExt* out_ext = nullptr);
+// The stem and the 3x3/s2 max-pool after it in one kernel (conv_stem.cuh), bit-identical to stem_tc + maxpool_3x3s2:
+// fp32 imgs, or uint8 imgs_u8 with mean_std, -> out NHWC fp16 (B,Hp,Wp,64).  stem_out (optional) receives the stem
+// map (B,Ho,Wo,64) before pooling.  Ragged batch: the pictures' extents in the input, the stem map and the pooled map
+// (rows of one table, one stride).
+int stem_pool(const float* imgs, const uint8_t* imgs_u8, const float* mean_std, int B, int H, int W, const __half* w2,
+              const float* scale, const float* shift, __half* out, __half* stem_out, cudaStream_t stream,
+              const ConvExt* in_ext = nullptr, const ConvExt* stem_ext = nullptr, const ConvExt* pool_ext = nullptr);
 // OIHW fp32 [64][3][7][7] -> [64][256] fp16 (host).
 void pack_stem_w2(const float* w_oihw, __half* out);
 int maxpool_3x3s2(const __half* in, int B, int H, int W, int C, __half* out, cudaStream_t stream,

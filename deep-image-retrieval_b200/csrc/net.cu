@@ -105,6 +105,7 @@ struct dirb200_net {
   Profiler prof;
   float mean_std[6] = {0.485f, 0.456f, 0.406f, 0.229f, 0.224f, 0.225f};   // preprocess of resnet.py:110-111
   int fuse_ds = 1;                // fuse the projection shortcut into conv3 of block 0 (wgmma path only)
+  int fuse_stem = 1;              // stem conv + maxpool as one kernel reading the images (conv_impl 0 / 2)
   int fuse_c23 = 0;               // conv2 + conv3 (+ residual) of the identity blocks as one kernel (conv_c23.cuh):
                                   // 0 off, 1 where every SM gets several tiles, 2 wherever the kernel supports the shape
   // trunk / head variants (rmac_resnet.py:74-88, rmac_resnet_fpn.py:92-110)
@@ -326,6 +327,7 @@ int dirb200_net_set_option(dirb200_net* n, const char* key, double value) {
   }
   else if (k == "fuse_ds") n->fuse_ds = value != 0;
   else if (k == "fuse_c23") n->fuse_c23 = static_cast<int>(value);
+  else if (k == "fuse_stem") n->fuse_stem = value != 0;
   else if (is_global_option(k)) return dirb200_set_global_option(key, value);   // process-wide kernel selectors
   else if (k.size() == 5 && k.compare(0, 4, "mean") == 0 && k[4] >= '0' && k[4] <= '2') n->mean_std[k[4] - '0'] = static_cast<float>(value);
   else if (k.size() == 4 && k.compare(0, 3, "std") == 0 && k[3] >= '0' && k[3] <= '2') n->mean_std[3 + k[3] - '0'] = static_cast<float>(value);
@@ -485,8 +487,8 @@ struct LevelSizes {
 
 // Activation buffers of one pass of the network over up to `chunk` images; every stage runs over the whole pass.
 struct Workspace {
-  __half* stem_ws;        // s2d / nhwc8 staging of the stem input
-  __half* stem_out;       // stem conv output (before the maxpool)
+  __half* stem_ws;        // s2d / nhwc8 staging of the stem input (unfused stem only, else null)
+  __half* stem_out;       // stem conv output (before the maxpool; unfused stem or debug taps only, else null)
   __half* stage_out[4];   // outputs of stage 0..3
   __half* scratch[4];     // rotating tensors inside a stage
   float* head_ws;
@@ -556,6 +558,9 @@ static void ragged_table(const dirb200_net* n, const int* hw, int B, std::vector
   }
 }
 
+// Whether the stem and its maxpool run as one kernel (stem_pool); the mma.sync stem of conv_impl 1 has no fused form.
+static bool stem_fused(const dirb200_net* n) { return n->fuse_stem && n->conv_impl != 1; }
+
 static int setup_workspace(dirb200_net* n, int chunk, int H, int W, Workspace* w) {
   w->chunk = chunk;
   w->sz = level_sizes(H, W);
@@ -564,8 +569,10 @@ static int setup_workspace(dirb200_net* n, int chunk, int H, int W, Workspace* w
   const size_t c = chunk;
   size_t off = 0;
   auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 1023) / 1024 * 1024; return o; };
-  const size_t o_sws = carve(std::max(c * H * W * 8 * 2, stem_workspace_bytes(chunk, H, W)));
-  const size_t o_stem = carve(c * h[1] * wd[1] * 64 * 2);
+  // the fused stem reads the images and writes the pooled map: neither intermediate exists
+  const bool unfused = !stem_fused(n);
+  const size_t o_sws = carve(unfused ? std::max(c * H * W * 8 * 2, stem_workspace_bytes(chunk, H, W)) : 0);
+  const size_t o_stem = carve(unfused || n->debug_taps ? c * h[1] * wd[1] * 64 * 2 : 0);
   size_t o_stage[4], o_scr[4];
   for (int s = 0; s < 4; ++s) o_stage[s] = carve(c * h[2 + s] * wd[2 + s] * n->stage_ch[s] * 2);
   size_t scr = 0;   // largest tensor inside any stage: conv1 output at the stage's input resolution, or a block output
@@ -585,8 +592,8 @@ static int setup_workspace(dirb200_net* n, int chunk, int H, int W, Workspace* w
   const size_t o_head = carve(head_floats * 4);
   DIRB_TRY(grow_device(&n->ws, &n->ws_bytes, off));
   uint8_t* ws = static_cast<uint8_t*>(n->ws);
-  w->stem_ws = reinterpret_cast<__half*>(ws + o_sws);
-  w->stem_out = reinterpret_cast<__half*>(ws + o_stem);
+  w->stem_ws = unfused ? reinterpret_cast<__half*>(ws + o_sws) : nullptr;
+  w->stem_out = unfused || n->debug_taps ? reinterpret_cast<__half*>(ws + o_stem) : nullptr;
   for (int s = 0; s < 4; ++s) w->stage_out[s] = reinterpret_cast<__half*>(ws + o_stage[s]);
   for (int i = 0; i < 4; ++i) w->scratch[i] = reinterpret_cast<__half*>(ws + o_scr[i]);
   w->head_ws = reinterpret_cast<float*>(ws + o_head);
@@ -600,7 +607,7 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
   const int D = n->desc_dim();
   const int* lh = w.sz.h;   // size per level (level_sizes)
   const int* lw = w.sz.w;
-  ConvExt e0, e1;   // extents handed to one launch (ragged batches; the launchers read them on the host)
+  ConvExt e0, e1, e2;   // extents handed to one launch (ragged batches; the launchers read them on the host)
   auto ext = [&](ConvExt& e, int lvl, int slot_w) -> const ConvExt* {
     if (!rg.on()) return nullptr;
     e = rg.at(lvl, cb, slot_w);
@@ -615,7 +622,16 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
     return &e;
   };
   // ---------------------------------------------------------------- stage 0: stem + maxpool
-  if (n->conv_impl == 1) {
+  if (stem_fused(n)) {
+    const double flops = 2.0 * cb * lh[1] * lw[1] * 64.0 * 147.0;
+    n->last_flops += flops;
+    // bytes: the images once, the pooled map once, the weights
+    const double bytes = static_cast<double>(cb) * ((imgs_u8 ? 3.0 : 12.0) * H * W + 128.0 * lh[2] * lw[2]) + 64.0 * 256 * 2;
+    ProfScope ps(n, stream, 1, flops, bytes, "stem 7x7/s2 3->64 + maxpool 3x3/s2 fused");
+    DIRB_TRY(stem_pool(imgs, imgs_u8, n->mean_std, cb, H, W, n->stem_w2, n->stem.scale, n->stem.shift, w.stage_out[0],
+                       n->debug_taps ? w.stem_out : nullptr, stream, ext(e0, 0, W), ext(e1, 1, lw[1]), ext(e2, 2, lw[2])));
+    DIRB_TRY(record_tap(n, "stem_conv", w.stem_out, cb, lh[1], lw[1], 64, stream));
+  } else if (n->conv_impl == 1) {
     DIRB_REQUIRE(imgs_u8 == nullptr, DIRB200_ENOTSUP, "uint8 input needs the space-to-depth stem (conv_impl 0)");
     {
       ProfScope ps(n, stream, 2, 0, static_cast<double>(cb) * H * W * (12 + 16));
@@ -629,8 +645,8 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
     DIRB_TRY(stem_tc(imgs, cb, H, W, n->stem_w2, n->stem.scale, n->stem.shift, w.stem_ws, w.stem_out, stream, imgs_u8,
                      n->mean_std, ext(e0, 0, W), ext(e1, 1, lw[1])));
   }
-  DIRB_TRY(record_tap(n, "stem_conv", w.stem_out, cb, lh[1], lw[1], 64, stream));
-  {
+  if (!stem_fused(n)) {
+    DIRB_TRY(record_tap(n, "stem_conv", w.stem_out, cb, lh[1], lw[1], 64, stream));
     ProfScope ps(n, stream, 2, 0, 2.0 * cb * 64 * (static_cast<double>(lh[1]) * lw[1] + static_cast<double>(lh[2]) * lw[2]), "maxpool 3x3/s2");
     DIRB_TRY(maxpool_3x3s2(w.stem_out, cb, lh[1], lw[1], 64, w.stage_out[0], stream, ext(e0, 2, lw[2])));
   }

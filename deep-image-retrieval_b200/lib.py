@@ -67,6 +67,7 @@ SIGNATURES = {
     "dirb200_stem_workspace_bytes": (C.c_size_t, [i32, i32, i32]),
     "dirb200_stem_pack_weight": (i32, [p, p]),
     "dirb200_stem_conv": (i32, [p, i32, i32, i32, p, p, p, p, p, p]),
+    "dirb200_stem_pool": (i32, [p, i32, i32, i32, i32, p, p, p, p, p, p, p]),
     "dirb200_maxpool_3x3s2": (i32, [p, i32, i32, i32, i32, p, p]),
     "dirb200_head_workspace_floats": (C.c_size_t, [i32, i32, i32, i32]),
     "dirb200_head_pool_fc_l2": (i32, [p, i32, i32, i32, i32, f32, f32, i32, p, p, i32, p, p, p, p]),

@@ -112,6 +112,32 @@ def stem_conv(x_nchw, w_oihw, scale, shift):
     return out
 
 
+def stem_pool(x, w_oihw, scale, shift, mean_std=None, stem_map=False):
+    """Stem conv 7x7/s2/p3 + BN + ReLU + maxpool 3x3/s2 as one kernel: NCHW fp32 (B,3,H,W), or HWC uint8 (B,H,W,3)
+    with mean_std = (mean[3], std[3]), -> NHWC fp16 (B,Hp,Wp,64); with stem_map also the stem map (B,Ho,Wo,64)."""
+    u8 = x.dtype == torch.uint8
+    _chk(x, torch.uint8 if u8 else torch.float32, "x")
+    if u8:
+        b, h, w, c = x.shape
+        ms = np.ascontiguousarray(np.asarray(mean_std, dtype=np.float32).reshape(6))
+    else:
+        b, c, h, w = x.shape
+        ms = None
+    assert c == 3 and tuple(w_oihw.shape) == (64, 3, 7, 7)
+    wh = np.ascontiguousarray(w_oihw.detach().cpu().numpy().astype(np.float32))
+    w2 = np.empty((64, 256), dtype=np.float16)
+    lib.call("dirb200_stem_pack_weight", wh.ctypes.data_as(C.c_void_p), w2.ctypes.data_as(C.c_void_p))
+    w2d = torch.from_numpy(w2).to(x.device)
+    ho, wo = (h + 6 - 7) // 2 + 1, (w + 6 - 7) // 2 + 1
+    hp, wp = (ho - 1) // 2 + 1, (wo - 1) // 2 + 1
+    out = torch.empty((b, hp, wp, 64), dtype=torch.float16, device=x.device)
+    stem = torch.empty((b, ho, wo, 64), dtype=torch.float16, device=x.device) if stem_map else None
+    lib.call("dirb200_stem_pool", _ptr(x), int(u8), b, h, w, None if ms is None else ms.ctypes.data_as(C.c_void_p), _ptr(w2d),
+             _ptr(_chk(scale, torch.float32, "scale")), _ptr(_chk(shift, torch.float32, "shift")), _ptr(out), _ptr(stem),
+             _stream())
+    return (out, stem) if stem_map else out
+
+
 def resize_bilinear_u8(x_u8, size):
     """uint8 HWC CUDA tensor (B,H,W,3) -> (B,Ho,Wo,3), byte-identical to PIL Image.resize((Wo,Ho), BILINEAR)."""
     _chk(x_u8, torch.uint8, "x_u8")

@@ -70,7 +70,8 @@ int dirb200_net_create(const char* arch, int device, dirb200_net** out);
  * GEMM (validation path), 2 = the same kernel with one tile per CTA (baseline); "fuse_ds" 1 (default) = projection
  * shortcut fused into conv3 as a K-concatenated GEMM; "fuse_c23" 0 (default) / 1 / 2 = conv2 + conv3 (+ residual) of the
  * identity blocks with 64 / 128 / 256 mid channels as one kernel (dirb200_conv_c23): never / where every SM gets at least
- * two tiles / wherever the kernel supports the shape.  PROCESS-WIDE (they select kernels, not handle state; set them
+ * two tiles / wherever the kernel supports the shape; "fuse_stem" 1 (default) = stem convolution + maxpool as one kernel
+ * (dirb200_stem_pool; conv_impl 0 and 2), 0 = space-to-depth, convolution and maxpool as three launches.  PROCESS-WIDE (they select kernels, not handle state; set them
  * once, not concurrently with a running forward): the global options above.
  * Diagnostics: "debug_taps" 1 = keep copies of the stage outputs for dirb200_net_debug_stage; "profile" 1 = time
  * every launch with CUDA events (dirb200_net_profile). */
@@ -191,6 +192,12 @@ size_t dirb200_stem_workspace_bytes(int B, int H, int W);
 int dirb200_stem_pack_weight(const float* w_oihw_host, void* w2_host);
 int dirb200_stem_conv(const float* imgs_dev, int B, int H, int W, const void* w2_dev, const float* scale_dev,
                       const float* shift_dev, void* ws_dev, void* out_dev, void* stream);
+/* The stem and the max-pool after it (resnet.py:115-119) in one kernel that reads the images and writes the pooled map,
+ * bit-identical to dirb200_stem_conv + dirb200_maxpool_3x3s2.  imgs_dev NCHW fp32 (B,3,H,W) (is_u8 0) or HWC uint8
+ * (B,H,W,3) (is_u8 1, ToTensor + Normalize with mean_std_host = {mean[3], std[3]}); w2_dev as for dirb200_stem_conv;
+ * out_dev NHWC fp16 (B,Hp,Wp,64); stem_dev (may be NULL) receives the stem map (B,Ho,Wo,64) before pooling. */
+int dirb200_stem_pool(const void* imgs_dev, int is_u8, int B, int H, int W, const float* mean_std_host, const void* w2_dev,
+                      const float* scale_dev, const float* shift_dev, void* out_dev, void* stem_dev, void* stream);
 /* MaxPool2d(3, stride 2, pad 1) on NHWC fp16.  resnet.py:119,161. */
 int dirb200_maxpool_3x3s2(const void* in_dev, int B, int H, int W, int C, void* out_dev, void* stream);
 /* Global pooling + (L2 over C) + FC + L2: rmac_resnet.py:59-68, pooling.py:38-40.
