@@ -80,14 +80,27 @@ static int set_total_tiles(ConvPersParams& p, int64_t total) {
   return 0;
 }
 
+template <int BN, int STAGES, bool HALO, bool PP>
+static int launch_conv_pers_mode(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR,
+                                 const CUtensorMap& tmO, const ConvPersParams& p, int grid_limit, cudaStream_t stream) {
+  if (p.ext != nullptr)
+    return conv_pers_launch<BN, STAGES, PERS_EPI_CONV, HALO, true, PP>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
+  return conv_pers_launch<BN, STAGES, PERS_EPI_CONV, HALO, false, PP>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
+}
+
 // Convolution epilogue on the persistent kernel; the RAGGED instantiation when the launch carries image extents.
+// When every CTA gets at least three tiles the consumer warpgroups ping-pong (one's epilogue runs under the other's
+// MMAs).  With one tile per CTA ping-pong would leave the whole epilogue to 128 threads; with two there is a single
+// overlap per CTA, and on an H100 the B = 1 forwards (layer1 / layer2 at 2-3 tiles per CTA) ran slower than
+// cooperative, while B = 64 was as fast as with a threshold of two.  Both modes give bit-identical outputs.
 template <int BN, int STAGES, bool HALO>
 static int launch_conv_pers(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO,
                             ConvPersParams& p, int64_t total, int grid_limit, cudaStream_t stream) {
   DIRB_TRY(set_total_tiles(p, total));
-  if (p.ext != nullptr)
-    return conv_pers_launch<BN, STAGES, PERS_EPI_CONV, HALO, true>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
-  return conv_pers_launch<BN, STAGES, PERS_EPI_CONV, HALO>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
+  const int64_t grid = std::min<int64_t>(total, grid_limit);
+  if (total >= 3 * grid)
+    return launch_conv_pers_mode<BN, STAGES, HALO, true>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
+  return launch_conv_pers_mode<BN, STAGES, HALO, false>(tmA, tmB, tmR, tmO, p, grid_limit, stream);
 }
 
 template <int CM>

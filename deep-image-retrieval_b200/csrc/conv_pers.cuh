@@ -10,6 +10,8 @@
 //                   scale/shift (+ residual) (+ ReLU) -> fp16 into 128-byte-swizzled staging buffers (one per 64
 //                   channels) and one thread TMA-stores them (the store clips ragged edges by itself).  The residual tile
 //                   is TMA-loaded into the same staging buffers when the tile starts, so it lands during the main loop.
+//                   When every CTA gets three tiles or more, the convolution epilogue runs in ping-pong mode instead: each
+//                   consumer warpgroup takes whole tiles, alternately, and its epilogue overlaps the other's MMAs (PP).
 //
 // HALO mode (3x3 / stride 1 / pad 1, 8 x 16 output pixels per tile): per 64-channel block ONE 5-D TMA box brings the
 // 10 x 18 input patch (zero padding from out-of-bounds fill) into a patch ring, channel-chunk-major without swizzle, and
@@ -87,7 +89,9 @@ __device__ __forceinline__ bool row_in_extent(const ConvPersParams& p, int m_til
 
 // HALO (3x3 / stride 1 / pad 1, 8 x 16 output tiles): the ring holds weight tiles only; per 64-channel block ONE TMA box
 // brings the 10 x 18 input patch into a separate ring of NP patch slots, and the nine taps read it as shifted views.
-template <int BN, int STAGES, int EPI = 0, bool HALO = false>
+// PP (ping-pong consumers, convolution epilogue only): each consumer warpgroup has its own staging buffers, residual
+// barrier and mainloop-handover barrier.
+template <int BN, int STAGES, int EPI = 0, bool HALO = false, bool PP = false>
 struct ConvPersSmem {
   static constexpr int A_BYTES = HALO ? 0 : 128 * 128;
   static constexpr int B_BYTES = BN * 128;
@@ -99,9 +103,12 @@ struct ConvPersSmem {
   static constexpr int PATCH_OFF = STAGES * STAGE_BYTES;
   static constexpr int STG_CHUNK = 128 * 128;                        // 128 rows x 64 channels fp16
   static constexpr int STG_OFF = PATCH_OFF + NP * PATCH_BYTES;
-  static constexpr int STG_BYTES = (EPI == 0) ? (BN / 64) * STG_CHUNK : 0;   // staging exists only for the conv epilogue
+  static constexpr int NWG_STG = PP ? 2 : 1;                         // staging sets: one per warpgroup in ping-pong
+  static constexpr int WG_STG_BYTES = (EPI == 0) ? (BN / 64) * STG_CHUNK : 0;  // staging exists only for the conv epilogue
+  static constexpr int STG_BYTES = NWG_STG * WG_STG_BYTES;
   static constexpr int BAR_OFF = STG_OFF + STG_BYTES;
-  static constexpr int NUM_BARS = 2 * STAGES + 2 * NP + 1;           // ring full / empty, patch full / empty, residual
+  // ring full / empty, patch full / empty, residual (per staging set), ping-pong mainloop handover (2)
+  static constexpr int NUM_BARS = 2 * STAGES + 2 * NP + NWG_STG + (PP ? 2 : 0);
   static constexpr int TOTAL = BAR_OFF + 8 * NUM_BARS + 1024;        // + alignment slack
 };
 
@@ -144,14 +151,42 @@ __device__ __forceinline__ void store_dense_pair(const ConvPersParams& p, int64_
 }
 
 // RAGGED: the launch carries an extent table (ConvPersParams::ext); dense launches compile without its code.
-template <int BN, int STAGES, int EPI, bool HALO, bool RAGGED>
+//
+// PP selects the consumer mode of the convolution epilogue:
+//   false (cooperative)  both consumer warpgroups work on every tile, warpgroup w on rows 64w .. 64w+63; the tensor cores
+//                        idle while the two run the epilogue together.
+//   true  (ping-pong)    warpgroup w takes every other CTA-local tile (tile i -> warpgroup i & 1) and holds the whole
+//                        128 x BN tile as acc[2][BN/2]; half h issues exactly the wgmmas that warpgroup h issues in the
+//                        cooperative mode and runs its epilogue for rows 64h .. 64h+63, so the output is bit-identical.
+//                        One warpgroup's epilogue runs under the other's main loop.
+// Invariants of the ping-pong mode (tests/pingpong_model.py checks them on a model of the barriers):
+//   1. ring parity: the main loops are handed over in tile order through mma_done[2] - only one warpgroup waits on the
+//      operand / patch rings at a time, so no waiter is ever two phases ahead of a slot's barrier (try_wait.parity would
+//      pass on the stale phase and the MMAs would read the wrong operands, with no hang and no trap).  Every consumer
+//      WARP arrives (count 4, lane 0 after the warp's last full-barrier wait of the tile): wgmma synchronises a warp,
+//      not a warpgroup, so one leader's arrival would not prove that its sibling warps have passed their own mma_done
+//      wait - with k_iters == 1 a sibling could lag while the partner completes the barrier twice, and then wait on a
+//      parity that never comes back;
+//   2. slot counters at CTA-local tile i: g = i * k_iters (HALO: g = i * 9 * cin_blocks, gp = i * cin_blocks) - every
+//      tile of a launch has the same number of k-iterations, kc_major only reorders them;
+//   3. the ring-empty and patch-empty barriers expect one arrival per fill (template constant, not a launch parameter);
+//   4. each warpgroup owns its staging buffers, residual barrier, bulk-store groups and 128-thread named barrier;
+//   5. a warpgroup may get one tile fewer: its partner's last mma_done arrival then has no waiter, which an mbarrier
+//      allows;
+//   6. setmaxnreg moves registers from the producer warpgroup (40) to the consumers (232): 128 x 40 + 256 x 232 <= 64 K.
+template <int BN, int STAGES, int EPI, bool HALO, bool RAGGED, bool PP>
 __global__ void __launch_bounds__(PERS_THREADS, 1)
 conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO,
                  const ConvPersParams p) {
-  using L = ConvPersSmem<BN, STAGES, EPI, HALO>;
+  using L = ConvPersSmem<BN, STAGES, EPI, HALO, PP>;
   constexpr int CHUNKS = BN / 64;
+  constexpr int NH = PP ? 2 : 1;                    // 64-row accumulator halves per consumer warpgroup
+  constexpr uint32_t EMPTY_ARRIVALS = PP ? 1 : 2;   // consumer warpgroups that read each fill (invariant 3)
+  constexpr uint32_t MMA_DONE_ARRIVALS = 4;         // one per warp of the handing-over warpgroup (invariant 1)
   static_assert(!HALO || EPI == PERS_EPI_CONV, "the halo mode is a convolution");
+  static_assert(!PP || EPI == PERS_EPI_CONV, "the ping-pong mode is a convolution epilogue");
+  static_assert(!PP || 128 * 40 + 256 * 232 <= 65536, "register file exceeded");
   if (EPI != PERS_EPI_CONV && p.gate != nullptr) {   // uniform over the grid: nothing has been set up yet
     pdl_wait();
     if (*reinterpret_cast<const volatile int*>(p.gate) == 0) return;
@@ -163,7 +198,8 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* pfull_bar = empty_bar + STAGES;
   uint64_t* pempty_bar = pfull_bar + L::NP;
-  uint64_t* res_bar = pempty_bar + L::NP;
+  uint64_t* res_bar = pempty_bar + L::NP;           // [NWG_STG]
+  uint64_t* mma_done = res_bar + L::NWG_STG;        // [2], ping-pong only
   uint8_t* patch = smem + L::PATCH_OFF;
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
@@ -178,13 +214,17 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (EPI == PERS_EPI_F32) { tma_prefetch_desc(&tmR); tma_prefetch_desc(&tmO); }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);               // one arrival per consumer warpgroup
+      mbar_init(&empty_bar[s], EMPTY_ARRIVALS);  // one arrival per consumer warpgroup reading the fill
     }
     for (int s = 0; s < L::NP; ++s) {
       mbar_init(&pfull_bar[s], 1);
-      mbar_init(&pempty_bar[s], 2);
+      mbar_init(&pempty_bar[s], EMPTY_ARRIVALS);
     }
-    mbar_init(res_bar, 1);
+    for (int w = 0; w < L::NWG_STG; ++w) mbar_init(&res_bar[w], 1);
+    if constexpr (PP) {
+      mbar_init(&mma_done[0], MMA_DONE_ARRIVALS);
+      mbar_init(&mma_done[1], MMA_DONE_ARRIVALS);
+    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -192,6 +232,7 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   pdl_wait();                // everything below reads tensors written by the previous kernel of the stream
 
   if (warp < 4) {
+    if constexpr (PP) setmaxnreg_dec<40>();        // all four producer warps, including the three that return at once
     if (threadIdx.x == 0) {
       // ------------------------------------------------------------ A/B producer
       uint32_t g = 0;  // ring slot counter, runs across tiles
@@ -255,28 +296,56 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 
   // ---------------------------------------------------------------- consumers
-  const int wg = (warp >> 2) - 1;                  // 0 / 1: accumulator rows 64*wg ..
+  if constexpr (PP) setmaxnreg_inc<232>();         // the whole 128 x BN accumulator tile lives in each warpgroup
+  // cooperative: accumulator rows 64*wg ..; ping-pong: the CTA-local tiles i with i & 1 == wg, all 128 rows
+  const int wg = (warp >> 2) - 1;
   const int ctid = static_cast<int>(threadIdx.x) - 128;
-  const bool leader = ctid == 0;
-  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: r0 and r0 + 8
+  const bool leader = PP ? (ctid & 127) == 0 : ctid == 0;   // issues the residual loads and the output stores
+  const int half0 = PP ? 0 : wg;                   // first 64-row half of the tile in this warpgroup's accumulators
+  const int r0 = half0 * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: r0 + 64 * half and + 8
   const int t4 = lane & 3;
-  float acc[BN / 2];
+  // invariant 4: per-warpgroup staging buffers, residual barrier and named barrier (ID 0 is __syncthreads)
+  uint8_t* stg_w = stg + (PP ? wg * L::WG_STG_BYTES : 0);
+  uint64_t* res_w = res_bar + (PP ? wg : 0);
+  const int epi_bar = PP ? 1 + wg : 1;
+  const int epi_threads = PP ? 128 : PERS_CONSUMER_THREADS;
+  float acc[NH][BN / 2];
 #pragma unroll
-  for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+  for (int h = 0; h < NH; ++h)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
 
-  uint32_t g = 0, i = 0, gp = 0;
-  for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++i) {
+  uint32_t g = 0, i = PP ? wg : 0, gp = 0;
+  for (int t = blockIdx.x + (PP ? wg * static_cast<int>(gridDim.x) : 0); t < p.total_tiles;
+       t += (PP ? 2 : 1) * gridDim.x, i += PP ? 2 : 1) {
     const TileCoord c = decode_tile(p, t);
+    const uint32_t jw = PP ? i >> 1 : i;             // tiles this warpgroup has finished: the residual barrier's phase
+    // ragged batches: bit 2 * hf + h = this thread's row r0 + 64 * hf + 8 * h lies inside its image (decided before the
+    // main loop, where the previous tile's accumulators are dead)
+    uint32_t keep = 0;
+#pragma unroll
+    for (int hf = 0; hf < NH; ++hf)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (!RAGGED || row_in_extent(p, c.m_tile, c.wo0, c.ho0, c.n0, r0 + 64 * hf + 8 * h)) keep |= 1u << (2 * hf + h);
     if (EPI == PERS_EPI_CONV && p.has_res && leader) {
       // the residual tile goes into the staging buffers once the previous tile's stores have finished reading them
+      // (bulk groups belong to the thread that committed them: each warpgroup's leader waits for its own stores)
       bulk_wait_read<0>();
-      mbar_expect_tx(res_bar, CHUNKS * L::STG_CHUNK);
+      mbar_expect_tx(res_w, CHUNKS * L::STG_CHUNK);
       for (int ch = 0; ch < CHUNKS; ++ch) {
         if (p.a_spatial)
-          tma_load_4d(stg + ch * L::STG_CHUNK, &tmR, res_bar, c.n_tile * BN + ch * 64, c.wo0, c.ho0, c.n0);
+          tma_load_4d(stg_w + ch * L::STG_CHUNK, &tmR, res_w, c.n_tile * BN + ch * 64, c.wo0, c.ho0, c.n0);
         else
-          tma_load_2d(stg + ch * L::STG_CHUNK, &tmR, res_bar, c.n_tile * BN + ch * 64, c.m_tile * 128);
+          tma_load_2d(stg_w + ch * L::STG_CHUNK, &tmR, res_w, c.n_tile * BN + ch * 64, c.m_tile * 128);
       }
+    }
+    if constexpr (PP) {
+      // invariant 2: this tile's first ring (and patch) slot; every tile has k_iters = taps * cin_blocks k-iterations
+      g = i * static_cast<uint32_t>(k_iters);
+      gp = i * static_cast<uint32_t>(p.cin_blocks);
+      // invariant 1: the partner warpgroup has passed every full-barrier wait of tile i - 1
+      if (i > 0) mbar_wait(&mma_done[wg ^ 1], ((i - 1) >> 1) & 1);
     }
 
     // ------------------------------------------------------------ main loop
@@ -292,18 +361,27 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const int s = g % STAGES;
           const int kh = tap / 3, kw = tap - 3 * (tap / 3);
           mbar_wait(&full_bar[s], (g / STAGES) & 1);
-          const uint64_t adesc = gmma_desc_noswizzle(pa + ((wg * 8 + kh) * HALO_W + kw) * 16, L::PATCH_CHUNK, HALO_W * 16);
+          uint64_t adesc[NH];
+#pragma unroll
+          for (int h = 0; h < NH; ++h)
+            adesc[h] = gmma_desc_noswizzle(pa + (((half0 + h) * 8 + kh) * HALO_W + kw) * 16, L::PATCH_CHUNK, HALO_W * 16);
           const uint64_t bdesc = gmma_desc_sw128(smem_u32(smem + s * L::STAGE_BYTES));
 #pragma unroll
-          for (int j = 0; j < BN / 2; ++j) fence_operand(acc[j]);
+          for (int h = 0; h < NH; ++h)
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) fence_operand(acc[h][j]);
           wgmma_fence();
 #pragma unroll
           for (int k = 0; k < 4; ++k)
-            wgmma_f16<BN>(acc, adesc + ((2 * k * L::PATCH_CHUNK) >> 4), bdesc + 2 * k, (kc | tap | k) != 0);
+#pragma unroll
+            for (int h = 0; h < NH; ++h)
+              wgmma_f16<BN>(acc[h], adesc[h] + ((2 * k * L::PATCH_CHUNK) >> 4), bdesc + 2 * k, (kc | tap | k) != 0);
           wgmma_commit();
           wgmma_wait<1>();                          // the previous group is done: hand back its weight slot (and patch)
 #pragma unroll
-          for (int j = 0; j < BN / 2; ++j) fence_operand(acc[j]);
+          for (int h = 0; h < NH; ++h)
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) fence_operand(acc[h][j]);
           if ((kc | tap) != 0 && (ctid & 127) == 0) {
             mbar_arrive(&empty_bar[(g - 1) % STAGES]);
             if (prev_last) mbar_arrive(&pempty_bar[(gp - 1) % L::NP]);
@@ -311,9 +389,12 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           prev_last = tap == 8;
         }
       }
+      if (PP && lane == 0) mbar_arrive(&mma_done[wg]);   // this warp is done waiting: the partner may start
       wgmma_wait<0>();
 #pragma unroll
-      for (int j = 0; j < BN / 2; ++j) fence_operand(acc[j]);
+      for (int h = 0; h < NH; ++h)
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) fence_operand(acc[h][j]);
       if ((ctid & 127) == 0) {
         mbar_arrive(&empty_bar[(g - 1) % STAGES]);
         mbar_arrive(&pempty_bar[(gp - 1) % L::NP]);
@@ -323,76 +404,87 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int s = g % STAGES;
       mbar_wait(&full_bar[s], (g / STAGES) & 1);
       const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
-      const uint64_t adesc = gmma_desc_sw128(sa + wg * 64 * 128);
+      uint64_t adesc[NH];
+#pragma unroll
+      for (int h = 0; h < NH; ++h) adesc[h] = gmma_desc_sw128(sa + (half0 + h) * 64 * 128);
       const uint64_t bdesc = gmma_desc_sw128(sa + L::A_BYTES);
 #pragma unroll
-      for (int j = 0; j < BN / 2; ++j) fence_operand(acc[j]);
+      for (int h = 0; h < NH; ++h)
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) fence_operand(acc[h][j]);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_f16<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (it | k) != 0);
+      for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int h = 0; h < NH; ++h) wgmma_f16<BN>(acc[h], adesc[h] + 2 * k, bdesc + 2 * k, (it | k) != 0);
       wgmma_commit();
       wgmma_wait<1>();                              // the previous slot's MMAs are done: hand it back
 #pragma unroll
-      for (int j = 0; j < BN / 2; ++j) fence_operand(acc[j]);
+      for (int h = 0; h < NH; ++h)
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) fence_operand(acc[h][j]);
       if (it > 0 && (ctid & 127) == 0) mbar_arrive(&empty_bar[(g - 1) % STAGES]);
     }
     if constexpr (!HALO) {
+      if (PP && lane == 0) mbar_arrive(&mma_done[wg]);   // this warp is done waiting: the partner may start
       wgmma_wait<0>();
 #pragma unroll
-      for (int j = 0; j < BN / 2; ++j) fence_operand(acc[j]);
+      for (int h = 0; h < NH; ++h)
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) fence_operand(acc[h][j]);
       if (k_iters > 0 && (ctid & 127) == 0) mbar_arrive(&empty_bar[(g - 1) % STAGES]);
     }
 
     // ------------------------------------------------------------ epilogue
     if (EPI == PERS_EPI_CONV) {
       if (p.has_res) {
-        mbar_wait(res_bar, i & 1);                  // residual tile has landed in the staging buffers
+        mbar_wait(res_w, jw & 1);                   // residual tile has landed in the staging buffers
       } else {
         if (leader) bulk_wait_read<0>();            // the previous tile's stores have left the staging buffers
-        named_bar_sync(1, PERS_CONSUMER_THREADS);
+        named_bar_sync(epi_bar, epi_threads);
       }
-      const uint32_t stg_addr = smem_u32(stg);
-      bool keep[2] = {true, true};
-      if constexpr (RAGGED) {
-        keep[0] = row_in_extent(p, c.m_tile, c.wo0, c.ho0, c.n0, r0);
-        keep[1] = row_in_extent(p, c.m_tile, c.wo0, c.ho0, c.n0, r0 + 8);
-      }
+      // this thread's rows r0 + 64 * hf + 8 * h all share r0 & 7, so their 128-byte swizzle (16-byte unit j ^ (r & 7)) is
+      // the same and the rows differ by immediate offsets
+      const uint32_t stg_addr = smem_u32(stg_w) + r0 * 128 + t4 * 4;
+      const int rsw = r0 & 7;
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int col = j * 8 + 2 * t4;
         const float2 sc = __ldg(reinterpret_cast<const float2*>(p.scale + c.n_tile * BN + col));
         const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + c.n_tile * BN + col));
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = r0 + 8 * h;
-          const uint32_t sp = stg_addr + (j >> 3) * L::STG_CHUNK + r * 128 + ((((j & 7) ^ (r & 7))) << 4) + t4 * 4;
-          float v0 = fmaf(acc[4 * j + 2 * h], sc.x, sh.x);
-          float v1 = fmaf(acc[4 * j + 2 * h + 1], sc.y, sh.y);
-          if (p.has_res) {
-            uint32_t rv;
-            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(rv) : "r"(sp));
-            const float2 f = unpack_h2(rv);
-            v0 += f.x;
-            v1 += f.y;
+        for (int hf = 0; hf < NH; ++hf) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t sp = stg_addr + (j >> 3) * L::STG_CHUNK + (64 * hf + 8 * h) * 128 + (((j & 7) ^ rsw) << 4);
+            float v0 = fmaf(acc[hf][4 * j + 2 * h], sc.x, sh.x);
+            float v1 = fmaf(acc[hf][4 * j + 2 * h + 1], sc.y, sh.y);
+            if (p.has_res) {
+              uint32_t rv;
+              asm volatile("ld.shared.u32 %0, [%1];" : "=r"(rv) : "r"(sp));
+              const float2 f = unpack_h2(rv);
+              v0 += f.x;
+              v1 += f.y;
+            }
+            if (p.relu) {
+              v0 = fmaxf(v0, 0.f);
+              v1 = fmaxf(v1, 0.f);
+            }
+            if (RAGGED && !((keep >> (2 * hf + h)) & 1)) {                     // ragged batch: outside the image = zero padding of the next layer
+              v0 = 0.f;
+              v1 = 0.f;
+            }
+            asm volatile("st.shared.u32 [%0], %1;" ::"r"(sp), "r"(pack_h2(v0, v1)) : "memory");
           }
-          if (p.relu) {
-            v0 = fmaxf(v0, 0.f);
-            v1 = fmaxf(v1, 0.f);
-          }
-          if (RAGGED && !keep[h]) {                           // ragged batch: outside the image = zero padding of the next layer
-            v0 = 0.f;
-            v1 = 0.f;
-          }
-          asm volatile("st.shared.u32 [%0], %1;" ::"r"(sp), "r"(pack_h2(v0, v1)) : "memory");
         }
       }
       fence_proxy_async_smem();                     // generic-proxy smem writes -> visible to the TMA engine
-      named_bar_sync(1, PERS_CONSUMER_THREADS);
+      named_bar_sync(epi_bar, epi_threads);
       if (leader) {
         for (int ch = 0; ch < CHUNKS; ++ch) {
           const int col0 = c.n_tile * BN + ch * 64;
-          if (p.a_spatial) tma_store_4d(&tmO, stg + ch * L::STG_CHUNK, col0, c.wo0, c.ho0, c.n0);
-          else tma_store_2d(&tmO, stg + ch * L::STG_CHUNK, col0, c.m_tile * 128);
+          if (p.a_spatial) tma_store_4d(&tmO, stg_w + ch * L::STG_CHUNK, col0, c.wo0, c.ho0, c.n0);
+          else tma_store_2d(&tmO, stg_w + ch * L::STG_CHUNK, col0, c.m_tile * 128);
         }
         bulk_commit();
       }
@@ -410,8 +502,8 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             const int col = c.n_tile * BN + j * 8 + 2 * t4;
-            cnt += (acc[4 * j + 2 * h] >= t_q && col < p.N) ? 1 : 0;
-            cnt += (acc[4 * j + 2 * h + 1] >= t_q && col + 1 < p.N) ? 1 : 0;
+            cnt += (acc[0][4 * j + 2 * h] >= t_q && col < p.N) ? 1 : 0;
+            cnt += (acc[0][4 * j + 2 * h + 1] >= t_q && col + 1 < p.N) ? 1 : 0;
           }
           int incl = cnt;
 #pragma unroll
@@ -430,7 +522,7 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                const float v = acc[4 * j + 2 * h + e];
+                const float v = acc[0][4 * j + 2 * h + e];
                 const int col = c.n_tile * BN + j * 8 + 2 * t4 + e;
                 if (v >= t_q && col < p.N) {
                   if (pos < p.cand_cap)
@@ -450,8 +542,8 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
             for (int j = 4 * gi; j < 4 * gi + 4; ++j) {
               const int col = c.n_tile * BN + j * 8 + 2 * t4;
-              m = (col < p.N) ? fmaxf(m, acc[4 * j + 2 * h]) : m;
-              m = (col + 1 < p.N) ? fmaxf(m, acc[4 * j + 2 * h + 1]) : m;
+              m = (col < p.N) ? fmaxf(m, acc[0][4 * j + 2 * h]) : m;
+              m = (col + 1 < p.N) ? fmaxf(m, acc[0][4 * j + 2 * h + 1]) : m;
             }
             m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
             m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
@@ -462,7 +554,7 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           for (int j = 0; j < BN / 8; ++j) {
             const int col = c.n_tile * BN + j * 8 + 2 * t4;
             if (col >= p.N) continue;
-            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            float v0 = acc[0][4 * j + 2 * h], v1 = acc[0][4 * j + 2 * h + 1];
             if (EPI == PERS_EPI_F32 && p.scale != nullptr) {
               v0 *= __ldg(p.scale + col);
               if (col + 1 < p.N) v1 *= __ldg(p.scale + col + 1);
@@ -476,12 +568,12 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (EPI == PERS_EPI_CONV && leader) bulk_wait<0>();     // all output bytes written before the CTA retires
 }
 
-template <int BN, int STAGES, int EPI, bool HALO = false, bool RAGGED = false>
+template <int BN, int STAGES, int EPI, bool HALO = false, bool RAGGED = false, bool PP = false>
 int conv_pers_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO,
                      const ConvPersParams& p, int num_sms, cudaStream_t stream) {
-  using L = ConvPersSmem<BN, STAGES, EPI, HALO>;
+  using L = ConvPersSmem<BN, STAGES, EPI, HALO, PP>;
   static_assert(L::TOTAL <= 232448, "shared memory budget exceeded");
-  auto kern = conv_pers_kernel<BN, STAGES, EPI, HALO, RAGGED>;
+  auto kern = conv_pers_kernel<BN, STAGES, EPI, HALO, RAGGED, PP>;
   static std::atomic<uint64_t> attr_done{0};
   if (first_launch_on_device(attr_done))
     DIRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
