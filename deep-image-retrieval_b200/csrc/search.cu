@@ -462,6 +462,106 @@ __global__ void __launch_bounds__(FIN_THREADS) search_finish_kernel(
   if (x.world > 0) x_signal_when_all_blocks_done(x, 1, X_OFF_FLIST, epoch);
 }
 
+// Phase 2 for k > 1024 (the deep path).  The survivors, their exact scores (exact_dot_warp) and their order are those
+// of search_finish_kernel, but they live in global memory and each step runs over many blocks per query:
+//   deep_compact_kernel   survivors (fp16-path score >= max(sel, kth_k) - band) -> surv_row[q][cap2], surv_cnt[q]
+//   deep_rescore_kernel   one warp per survivor: exact score -> surv_sc[q][cap2]
+//   deep_run_sort_kernel  runs of DEEP_RUN survivors bitonic-sorted in shared memory -> (score, global index) in place
+//   merge_runs_kernel     rank-based merge of the sorted runs, first k entries (also dirb200_topk_merge at large G*k)
+constexpr int DEEP_RUN = 2048;
+
+__global__ void deep_compact_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cnt, int cap,
+                                    const float* __restrict__ kth_k, const float* __restrict__ sel, float band,
+                                    int* __restrict__ surv_row, int* __restrict__ surv_cnt, int cap2,
+                                    unsigned long long* __restrict__ status) {
+  const int q = blockIdx.y;
+  const int n = min(cnt[q], cap);
+  const float t2 = fmaxf(sel[q], kth_k[q]) - band;
+  const unsigned long long* c = cand + static_cast<int64_t>(q) * cap;
+  const int lane = threadIdx.x & 31;
+  const int n_round = (n + 31) & ~31;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += gridDim.x * blockDim.x) {
+    bool keep = false;
+    int row = 0;
+    if (i < n) {
+      const unsigned long long e = c[i];
+      keep = __uint_as_float(static_cast<uint32_t>(e >> 32)) >= t2;
+      row = static_cast<int>(e & 0xffffffffu);
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, keep);
+    int base = 0;
+    if (lane == 0 && m) base = atomicAdd(surv_cnt + q, __popc(m));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (keep) {
+      const int pos = base + __popc(m & ((1u << lane) - 1u));
+      if (pos < cap2) surv_row[static_cast<int64_t>(q) * cap2 + pos] = row;
+      else atomicOr(status + ST_ERR, 2ull);
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(status + ST_CAND, static_cast<unsigned long long>(n));
+}
+
+__global__ void deep_rescore_kernel(const float* __restrict__ q32, const float* __restrict__ db32, int D,
+                                    const int* __restrict__ surv_row, const int* __restrict__ surv_cnt, int cap2,
+                                    double* __restrict__ surv_sc) {
+  const int q = blockIdx.y;
+  const int ns = min(surv_cnt[q], cap2);
+  const int wpb = blockDim.x >> 5, lane = threadIdx.x & 31;
+  const int64_t o = static_cast<int64_t>(q) * cap2;
+  for (int w = blockIdx.x * wpb + (threadIdx.x >> 5); w < ns; w += gridDim.x * wpb) {
+    const double acc = exact_dot_warp(q32 + static_cast<int64_t>(q) * D, db32 + static_cast<int64_t>(surv_row[o + w]) * D, D, lane);
+    if (lane == 0) surv_sc[o + w] = acc;
+  }
+}
+
+// Block x sorts run x of query y by (score desc, row asc) and writes it back as (score, global index); the tail of the
+// last run becomes (-inf, -1), which the merge treats as empty.  Runs past the survivor count are never read.
+__global__ void __launch_bounds__(FIN_THREADS) deep_run_sort_kernel(const int* __restrict__ surv_row,
+                                                                    const int* __restrict__ surv_cnt, int cap2,
+                                                                    int64_t offset, double* __restrict__ surv_sc,
+                                                                    int64_t* __restrict__ run_ix,
+                                                                    unsigned long long* __restrict__ status) {
+  __shared__ double sc[DEEP_RUN];
+  __shared__ int ix[DEEP_RUN];
+  const int q = blockIdx.y;
+  const int ns = min(surv_cnt[q], cap2);
+  const int base = blockIdx.x * DEEP_RUN;
+  if (base >= ns) return;                                  // uniform over the block
+  const int n = min(DEEP_RUN, ns - base);
+  const int64_t o = static_cast<int64_t>(q) * cap2 + base;
+  int P = 2;
+  while (P < n) P <<= 1;
+  for (int i = threadIdx.x; i < P; i += FIN_THREADS) {
+    const bool ok = i < n;
+    sc[i] = ok ? surv_sc[o + i] : -INFINITY;
+    ix[i] = ok ? surv_row[o + i] : INT_MAX;
+  }
+  __syncthreads();
+  for (int size = 2; size <= P; size <<= 1) {
+    for (int st = size >> 1; st > 0; st >>= 1) {
+      for (int i = threadIdx.x; i < P / 2; i += FIN_THREADS) {
+        const int lo = 2 * i - (i & (st - 1));
+        const int hi = lo + st;
+        const bool up = ((lo & size) == 0);
+        const double va = sc[lo], vb = sc[hi];
+        const int ia = ix[lo], ib = ix[hi];
+        const bool a_first = (va > vb) || (va == vb && ia < ib);
+        if (a_first != up) {
+          sc[lo] = vb; sc[hi] = va;
+          ix[lo] = ib; ix[hi] = ia;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  for (int i = threadIdx.x; i < DEEP_RUN; i += FIN_THREADS) {
+    const bool ok = i < n;
+    surv_sc[o + i] = ok ? sc[i] : -INFINITY;
+    run_ix[o + i] = ok ? static_cast<int64_t>(ix[i]) + offset : -1;
+  }
+  if (threadIdx.x == 0) atomicAdd(status + ST_SURV, static_cast<unsigned long long>(n));
+}
+
 // Exact dense scores for small evaluation sets: grid (ceil(N/8), ceil(Q/4)), warp = one db row x 4 queries.
 __global__ void scores_exact_kernel(const float* __restrict__ q, int Q, const float* __restrict__ db, int64_t N, int D,
                                     float* __restrict__ out) {
@@ -492,33 +592,42 @@ __global__ void scores_exact_kernel(const float* __restrict__ q, int Q, const fl
 
 // alpha query expansion: out_i = normalize(q_i + sum_j db[idx_ij] * s_ij^alpha)   (test_dir.py:38-42; the mean's
 // 1/(k+1) cancels in the normalisation).  partial: un-normalised neighbour sum only.
+// The neighbours are taken in chunks of AQE_CHUNK weights held in shared memory; between chunks the running sums wait in
+// `out` (fp32, as in the register), so every element sees the same fmaf sequence whatever the chunking.
+constexpr int AQE_CHUNK = 2048;
 __global__ void aqe_kernel(const float* __restrict__ q, int D, const float* __restrict__ db, const int64_t* __restrict__ nn,
                            const double* __restrict__ ns, int k, double alpha, int partial, int64_t row_offset,
                            int64_t n_rows, float* __restrict__ out) {
-  extern __shared__ float wts[];  // [k] weights, then [k] local rows (as int64 pairs of floats)
+  extern __shared__ float wts[];  // [chunk] weights, then [chunk] local rows (as int64 pairs of floats)
   __shared__ float sh[32];
-  int64_t* rows = reinterpret_cast<int64_t*>(wts + ((k + 1) & ~1));
+  const int kc = min(k, AQE_CHUNK);
+  int64_t* rows = reinterpret_cast<int64_t*>(wts + ((kc + 1) & ~1));
   const int i = blockIdx.x;
-  for (int j = threadIdx.x; j < k; j += blockDim.x) {
-    int64_t r = nn[static_cast<int64_t>(i) * k + j];
-    if (r >= 0 && (partial || n_rows > 0)) {         // sharded: global index -> local row of this shard, or "not mine"
-                                                     // (partial sums are per shard by definition, also for an EMPTY shard)
-      r -= row_offset;
-      if (r < 0 || r >= n_rows) r = -1;
-    }
-    rows[j] = r;
-    wts[j] = (r >= 0) ? static_cast<float>(pow(ns[static_cast<int64_t>(i) * k + j], alpha)) : 0.f;
-  }
-  __syncthreads();
   float ss = 0.f;
-  for (int c = threadIdx.x; c < D; c += blockDim.x) {
-    float acc = partial ? 0.f : q[static_cast<int64_t>(i) * D + c];
-    for (int j = 0; j < k; ++j) {
-      const int64_t r = rows[j];
-      if (r >= 0) acc += db[r * D + c] * wts[j];
+  for (int j0 = 0; j0 < k; j0 += AQE_CHUNK) {
+    const int nj = min(AQE_CHUNK, k - j0);
+    if (j0 > 0) __syncthreads();                     // the previous chunk's weights are no longer read
+    for (int j = threadIdx.x; j < nj; j += blockDim.x) {
+      int64_t r = nn[static_cast<int64_t>(i) * k + j0 + j];
+      if (r >= 0 && (partial || n_rows > 0)) {       // sharded: global index -> local row of this shard, or "not mine"
+                                                     // (partial sums are per shard by definition, also for an EMPTY shard)
+        r -= row_offset;
+        if (r < 0 || r >= n_rows) r = -1;
+      }
+      rows[j] = r;
+      wts[j] = (r >= 0) ? static_cast<float>(pow(ns[static_cast<int64_t>(i) * k + j0 + j], alpha)) : 0.f;
     }
-    out[static_cast<int64_t>(i) * D + c] = acc;
-    ss += acc * acc;
+    __syncthreads();
+    const bool last = j0 + AQE_CHUNK >= k;
+    for (int c = threadIdx.x; c < D; c += blockDim.x) {
+      float acc = (j0 > 0) ? out[static_cast<int64_t>(i) * D + c] : (partial ? 0.f : q[static_cast<int64_t>(i) * D + c]);
+      for (int j = 0; j < nj; ++j) {
+        const int64_t r = rows[j];
+        if (r >= 0) acc += db[r * D + c] * wts[j];
+      }
+      out[static_cast<int64_t>(i) * D + c] = acc;
+      if (last) ss += acc * acc;
+    }
   }
   if (!partial) {
     for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
@@ -735,6 +844,47 @@ __global__ void __launch_bounds__(1024) merge_lists_kernel(const double* in_scor
   }
 }
 
+// The same rank-based merge with the runs read from global memory, one thread per entry, for merges that do not fit in
+// shared memory: run g of query q holds L entries at g * run_stride + q * q_stride, ordered (score desc, index asc), empty
+// entries (index -1) only at its tail.  cnt != nullptr: query q has only ceil(min(cnt[q], cnt_cap) / L) runs.  An entry
+// at position j >= k of its own run cannot reach the first k, so only the first min(L, k) entries of a run take part.
+// The output must already hold (-inf, -1): every entry that ranks below k overwrites exactly one slot.
+__global__ void merge_runs_kernel(const double* __restrict__ in_score, const int64_t* __restrict__ in_idx, int G, int L,
+                                  int64_t run_stride, int64_t q_stride, const int* __restrict__ cnt, int cnt_cap, int Q,
+                                  int k, double* __restrict__ out_score, int64_t* __restrict__ out_idx) {
+  const int Lk = min(L, k);
+  const int64_t e = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  for (int q = blockIdx.y; q < Q; q += gridDim.y) {
+    const int Gq = cnt ? (min(cnt[q], cnt_cap) + L - 1) / L : G;
+    if (e >= static_cast<int64_t>(Gq) * Lk) continue;
+    const int g = static_cast<int>(e / Lk), j = static_cast<int>(e - static_cast<int64_t>(g) * Lk);
+    const double* sq = in_score + static_cast<int64_t>(q) * q_stride;
+    const int64_t* iq = in_idx + static_cast<int64_t>(q) * q_stride;
+    const double se = __ldcg(sq + g * run_stride + j);
+    const int64_t ie = __ldcg(iq + g * run_stride + j);
+    if (ie < 0) continue;
+    int rank = j;
+    for (int h = 0; h < Gq && rank < k; ++h) {
+      if (h == g) continue;
+      const double* hs = sq + h * run_stride;
+      const int64_t* hi = iq + h * run_stride;
+      int lo = 0, hi_ = Lk;                     // first position of run h that does NOT come before (se, ie)
+      while (lo < hi_) {
+        const int mid = (lo + hi_) >> 1;
+        const int64_t im = __ldcg(hi + mid);
+        const double sm = __ldcg(hs + mid);
+        const bool before = im >= 0 && (sm > se || (sm == se && im < ie));
+        if (before) lo = mid + 1; else hi_ = mid;
+      }
+      rank += lo;
+    }
+    if (rank < k) {
+      out_score[static_cast<int64_t>(q) * k + rank] = se;
+      out_idx[static_cast<int64_t>(q) * k + rank] = ie;
+    }
+  }
+}
+
 }  // namespace
 }  // namespace dirb
 
@@ -770,6 +920,7 @@ struct dirb200_index {
   int band_cap = 0;          // dirb200_index_count_ge: band-list capacity (0 = 1 << 20 entries)
   int retries = 1;           // gated retry passes enqueued after the first filter pass (device-side predicate)
   int deferred = 0;          // 1 = search calls never synchronise; the caller collects the status (dirb200_index_check)
+  double ws_budget = 4.0 * (1 << 30);   // search workspace bound in bytes: sets the largest query block (search_max_queries)
   // workspaces (grown on demand)
   void* ws = nullptr;
   size_t ws_bytes = 0;
@@ -800,6 +951,11 @@ struct dirb200_index {
     int64_t S_ld = 0;
     bool small = false;
     int ks = 0;
+    // deep path (k > 1024): survivors in global memory
+    int* surv_row = nullptr;
+    int* surv_cnt = nullptr;
+    double* surv_sc = nullptr;
+    int64_t* run_ix = nullptr;
   } pend;
   TmapCache tmaps;
   int profile = 0;                 // option "profile": time the phases of a search with CUDA events
@@ -893,6 +1049,7 @@ int dirb200_index_set_option(dirb200_index* h, const char* key, double value) {
   else if (k == "band_cap") h->band_cap = std::max(0, static_cast<int>(value));
   else if (k == "retries") h->retries = std::max(0, std::min(4, static_cast<int>(value)));
   else if (k == "deferred_check") h->deferred = value != 0;
+  else if (k == "ws_budget") h->ws_budget = std::max(0.0, value);
   else DIRB_REQUIRE(false, DIRB200_EKEY, "unknown index option '%s'", key);
   return 0;
 }
@@ -909,7 +1066,8 @@ int dirb200_index_check(dirb200_index* h) {
   h->stats[2] = static_cast<int64_t>(h->h_status[ST_SURV]);
   h->stats[3] = static_cast<int64_t>(h->h_status[ST_RETRIES]);
   if (h->profile && h->pend.mark_i >= 2) {
-    for (int i = 0; i + 1 < h->pend.mark_i && i < 8; ++i) {
+    for (double& v : h->phase_ms) v = 0;
+    for (int i = 0; i + 1 < h->pend.mark_i && i < 9; ++i) {
       float ms = 0;
       cudaEventElapsedTime(&ms, h->ev[i], h->ev[i + 1]);
       h->phase_ms[i] = ms;
@@ -970,15 +1128,97 @@ static void mark_phase(dirb200_index* h, cudaStream_t stream) {
 // candidate selection, gated retries).  seed2 != nullptr: the seed half also writes the k_shard-th seed bound of every
 // query there - what a shard contributes to the MIN over the shards that tightens the filter threshold of the sharded
 // search (thr_min_kernel, issued between the halves by dirb200_index_search_sharded_phase).
+// Sizes of a search of depth k on this shard; none depends on Q.
+constexpr int DEEP_K = 1024;        // k above this takes the deep finish (survivors in global memory)
+constexpr int K_MAX = 1 << 27;      // keeps the per-query buffer sizes (2k, 8k entries) in int
+struct SearchSizes {
+  int64_t S = 0, S_ld = 0;
+  bool small = false, gmax = false, deep = false;
+  int cap = 0, cap2 = 0;
+};
+static SearchSizes search_sizes(const dirb200_index* h, int k) {
+  SearchSizes z;
+  const int64_t N = h->N;
+  int64_t S = h->sample_rows > 0 ? h->sample_rows : std::max<int64_t>(8192, ceil_div(N, 16));
+  S = std::min<int64_t>(std::min<int64_t>(S, 65536), N);
+  S = std::max<int64_t>(S, std::min<int64_t>(N, 4 * static_cast<int64_t>(k)));
+  const bool small = (N <= S);
+  if (small) S = N;
+  // at least k groups of 32 rows; k > 1024: 2k groups, so that the bound is the median group maximum, as with the
+  // 2048 groups of the default sample at k = 1024 (with only k groups it is the smallest one: ~20 % of the rows pass)
+  const int64_t groups = (k > DEEP_K ? 2 : 1) * static_cast<int64_t>(k);
+  if (!small && S / 32 < groups) S = std::min<int64_t>(N, std::max<int64_t>(S, 32 * groups));
+  // seed threshold from group maxima (1/32 of the dense traffic) whenever there are at least k groups; otherwise the
+  // seed scores are dense (all N rows when 32 k >= N)
+  z.gmax = !small && (S / 32 >= k);
+  z.small = small;
+  z.S = S;
+  z.S_ld = ceil_div(z.gmax ? ceil_div(S, 32) : S, 128) * 128;   // dense row stride (16-byte aligned rows)
+  const double expect = z.small ? (2.0 * k + 64) : (1.5 * k * static_cast<double>(N) / S);
+  int cap = static_cast<int>(std::min<double>(std::max<double>(4096, 4 * expect), std::max<double>(1 << 18, 8.0 * k)));
+  if (h->cand_cap > 0) cap = std::max(h->cand_cap, 2 * k);
+  z.cap = (cap + 255) / 256 * 256;
+  z.deep = k > DEEP_K;
+  // survivors: the shallow finish sorts up to cap2 of them in shared memory; the deep one keeps 2k (at most N) in
+  // global memory, whole runs of DEEP_RUN
+  z.cap2 = z.deep ? static_cast<int>(ceil_div(std::min<int64_t>(2 * static_cast<int64_t>(k), N), DEEP_RUN) * DEEP_RUN)
+                  : (k > 256 ? 2048 : 1024);
+  return z;
+}
+
+// Byte offsets of the search workspace for Q queries.
+struct SearchLayout {
+  size_t q16 = 0, dense = 0, thr = 0, cnt = 0, cand = 0, kthk = 0, gates = 0, status = 0;
+  size_t surv_row = 0, surv_cnt = 0, surv_sc = 0, run_ix = 0, total = 0;
+};
+static SearchLayout search_layout(const dirb200_index* h, const SearchSizes& z, int Q) {
+  SearchLayout L;
+  size_t off = 0;
+  auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
+  const size_t q = static_cast<size_t>(Q);
+  L.q16 = carve(q * h->dim * 2);
+  L.dense = carve(q * z.S_ld * 4);
+  L.thr = carve(q * 4);
+  L.cnt = carve(q * 4);
+  L.cand = carve(q * z.cap * 8);
+  L.kthk = carve(q * 4);
+  L.gates = carve(8 * 4);
+  L.status = carve(ST_WORDS * 8);
+  if (z.deep) {
+    L.surv_row = carve(q * z.cap2 * 4);
+    L.surv_cnt = carve(q * 4);
+    L.surv_sc = carve(q * z.cap2 * 8);
+    L.run_ix = carve(q * z.cap2 * 8);
+  }
+  L.total = off;
+  return L;
+}
+
+// Largest query block whose workspace fits option ws_budget (at least 1).  Launches with a grid row per query (the
+// dense compaction of the small path, the deep finish) limit it to 65535.
+static int search_max_queries(const dirb200_index* h, int k) {
+  if (h->N == 0) return 1 << 30;              // an empty shard has no workspace
+  const SearchSizes z = search_sizes(h, k);
+  int lo = 1, hi = (z.small || z.deep) ? 65535 : (1 << 30);
+  while (lo < hi) {
+    const int mid = lo + (hi - lo + 1) / 2;
+    if (static_cast<double>(search_layout(h, z, mid).total) <= h->ws_budget) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
 static int search_begin_seed(dirb200_index* h, const float* q32, int Q, int k, int k_shard, float* sel_dev, cudaStream_t stream,
                              float* seed2) {
   DIRB_REQUIRE(h && q32 && sel_dev, DIRB200_EINVAL, "null argument");
   DIRB_REQUIRE(h->has_db, DIRB200_ESTATE, "index has no database attached");
-  DIRB_REQUIRE(Q > 0 && k > 0 && k <= 1024, DIRB200_ENOTSUP, "need 0 < Q and 0 < k <= 1024 (got Q=%d k=%d)", Q, k);
+  DIRB_REQUIRE(Q > 0 && k > 0 && k <= K_MAX, DIRB200_ENOTSUP, "need 0 < Q and 0 < k <= %d (got Q=%d k=%d)", K_MAX, Q, k);
   DIRB_REQUIRE(k_shard >= 1 && k_shard <= k, DIRB200_EINVAL, "k_shard must be in [1, k]");
+  const int q_max = search_max_queries(h, k);
+  DIRB_REQUIRE(Q <= q_max, DIRB200_ENOTSUP,
+               "a search of depth k=%d takes at most %d queries per call within option ws_budget=%.0f bytes (got Q=%d; "
+               "dirb200_index_search_max_queries)", k, q_max, h->ws_budget, Q);
   DIRB_CUDA(cudaSetDevice(h->device));
   DIRB_TRY(dirb200_index_check(h));          // an uncollected error of the previous search must not get lost
-  const int D = h->dim;
   const int64_t N = h->N;
   auto& P = h->pend;
   P = dirb200_index::Pending();
@@ -998,46 +1238,33 @@ static int search_begin_seed(dirb200_index* h, const float* q32, int Q, int k, i
     DIRB_CUDA(cudaGetLastError());
     return 0;
   }
-  // ---- sizes
-  int64_t S = h->sample_rows > 0 ? h->sample_rows : std::max<int64_t>(8192, ceil_div(N, 16));
-  S = std::min<int64_t>(std::min<int64_t>(S, 65536), N);
-  S = std::max<int64_t>(S, std::min<int64_t>(N, 4 * k));
-  const bool small = (N <= S);
-  if (small) S = N;
-  if (!small && S / 32 < k) S = std::min<int64_t>(N, std::max<int64_t>(S, 32 * static_cast<int64_t>(k)));
-  // seed threshold from group maxima (1/32 of the dense traffic) whenever there are at least k groups
-  const bool use_gmax = !small && (S / 32 >= k);
-  const int64_t S_ld = ceil_div(S, 128) * 128;   // dense row stride (16-byte aligned rows)
-  const double expect = small ? (2.0 * k + 64) : (1.5 * k * static_cast<double>(N) / S);
-  int cap = static_cast<int>(std::min<double>(std::max<double>(4096, 4 * expect), 1 << 18));
-  if (h->cand_cap > 0) cap = std::max(h->cand_cap, 2 * k);
-  cap = (cap + 255) / 256 * 256;
+  // ---- sizes, workspace carve-up
+  const SearchSizes z = search_sizes(h, k);
+  const int64_t S = z.S, S_ld = z.S_ld;
+  const bool small = z.small, use_gmax = z.gmax;
   const float band = static_cast<float>(2.0 * h->eps16);
   P.S = S;
-  P.cap = cap;
+  P.cap = z.cap;
+  P.cap2 = z.cap2;
   P.band = band;
-
-  // ---- workspace carve-up
-  size_t off = 0;
-  auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-  const size_t o_q16 = carve(static_cast<size_t>(Q) * D * 2);
-  const size_t o_dense = carve(static_cast<size_t>(Q) * S_ld * 4);
-  const size_t o_thr = carve(static_cast<size_t>(Q) * 4);
-  const size_t o_cnt = carve(static_cast<size_t>(Q) * 4);
-  const size_t o_cand = carve(static_cast<size_t>(Q) * cap * 8);
-  const size_t o_kthk = carve(static_cast<size_t>(Q) * 4);
-  const size_t o_gates = carve(8 * 4);
-  const size_t o_status = carve(ST_WORDS * 8);
-  DIRB_TRY(grow_ws(h, off));
+  const SearchLayout L = search_layout(h, z, Q);
+  DIRB_TRY(grow_ws(h, L.total));
   uint8_t* w = static_cast<uint8_t*>(h->ws);
-  __half* q16 = reinterpret_cast<__half*>(w + o_q16);
-  float* dense = reinterpret_cast<float*>(w + o_dense);
-  float* thr = reinterpret_cast<float*>(w + o_thr);
-  int* gates = reinterpret_cast<int*>(w + o_gates);
-  P.cnt = reinterpret_cast<int*>(w + o_cnt);
-  P.cand = reinterpret_cast<unsigned long long*>(w + o_cand);
-  P.kth_k = reinterpret_cast<float*>(w + o_kthk);
-  P.status = reinterpret_cast<unsigned long long*>(w + o_status);
+  __half* q16 = reinterpret_cast<__half*>(w + L.q16);
+  float* dense = reinterpret_cast<float*>(w + L.dense);
+  float* thr = reinterpret_cast<float*>(w + L.thr);
+  int* gates = reinterpret_cast<int*>(w + L.gates);
+  P.cnt = reinterpret_cast<int*>(w + L.cnt);
+  P.cand = reinterpret_cast<unsigned long long*>(w + L.cand);
+  P.kth_k = reinterpret_cast<float*>(w + L.kthk);
+  P.status = reinterpret_cast<unsigned long long*>(w + L.status);
+  if (z.deep) {
+    P.surv_row = reinterpret_cast<int*>(w + L.surv_row);
+    P.surv_cnt = reinterpret_cast<int*>(w + L.surv_cnt);
+    P.surv_sc = reinterpret_cast<double*>(w + L.surv_sc);
+    P.run_ix = reinterpret_cast<int64_t*>(w + L.run_ix);
+  }
+  const int D = h->dim;
   int* cnt = P.cnt;
 
   mark_phase(h, stream);  // 0
@@ -1160,12 +1387,40 @@ static int search_finish_impl(dirb200_index* h, const float* q32, const float* s
     h->stats[4] = launches_total() - P.launches0;
     return 0;
   }
-  const size_t smem = static_cast<size_t>(cap2) * 12;
-  search_finish_kernel<<<Q, FIN_THREADS, smem, stream>>>(P.cand, P.cnt, P.cap, P.kth_k, sel_dev, P.band, q32, h->db32, h->dim,
-                                                         cap2, h->offset, k, scores_dev, idx_dev, P.status, px);
-  count_launch();
-  DIRB_CUDA(cudaGetLastError());
-  mark_phase(h, stream);  // 7: survivors + exact re-scoring + sort
+  if (P.surv_row != nullptr) {              // deep path, k > 1024 (never through peer memory: exchange windows hold k <= 1024)
+    DIRB_REQUIRE(px.world == 0, DIRB200_ENOTSUP, "peer-exchange search needs k <= 1024");
+    const int64_t sms = num_sms();
+    DIRB_CUDA(cudaMemsetAsync(P.surv_cnt, 0, static_cast<size_t>(Q) * 4, stream));
+    const unsigned gc = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(8 * sms, Q), ceil_div(P.cap, 256))));
+    deep_compact_kernel<<<dim3(gc, Q), 256, 0, stream>>>(P.cand, P.cnt, P.cap, P.kth_k, sel_dev, P.band, P.surv_row, P.surv_cnt,
+                                                         cap2, P.status);
+    count_launch();
+    mark_phase(h, stream);  // 7: survivor compaction
+    const unsigned gr = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(32 * sms, Q), ceil_div(cap2, 8))));
+    deep_rescore_kernel<<<dim3(gr, Q), 256, 0, stream>>>(q32, h->db32, h->dim, P.surv_row, P.surv_cnt, cap2, P.surv_sc);
+    count_launch();
+    mark_phase(h, stream);  // 8: exact re-scoring
+    const int runs = cap2 / DEEP_RUN;
+    deep_run_sort_kernel<<<dim3(runs, Q), FIN_THREADS, 0, stream>>>(P.surv_row, P.surv_cnt, cap2, h->offset, P.surv_sc, P.run_ix,
+                                                                    P.status);
+    count_launch();
+    const int64_t n = static_cast<int64_t>(Q) * k;
+    fill_empty_result_kernel<<<static_cast<unsigned>(ceil_div(n, 256)), 256, 0, stream>>>(scores_dev, idx_dev, n);
+    count_launch();
+    const int64_t elems = static_cast<int64_t>(runs) * std::min(DEEP_RUN, k);
+    merge_runs_kernel<<<dim3(static_cast<unsigned>(ceil_div(elems, 256)), Q), 256, 0, stream>>>(
+        P.surv_sc, P.run_ix, runs, DEEP_RUN, DEEP_RUN, cap2, P.surv_cnt, cap2, Q, k, scores_dev, idx_dev);
+    count_launch();
+    DIRB_CUDA(cudaGetLastError());
+    mark_phase(h, stream);  // 9: run sort + merge
+  } else {
+    const size_t smem = static_cast<size_t>(cap2) * 12;
+    search_finish_kernel<<<Q, FIN_THREADS, smem, stream>>>(P.cand, P.cnt, P.cap, P.kth_k, sel_dev, P.band, q32, h->db32, h->dim,
+                                                           cap2, h->offset, k, scores_dev, idx_dev, P.status, px);
+    count_launch();
+    DIRB_CUDA(cudaGetLastError());
+    mark_phase(h, stream);  // 7: survivors + exact re-scoring + sort
+  }
   h->status_cap2 = cap2;
   h->status_band = P.band;
   h->stats[0] = P.S;
@@ -1182,14 +1437,31 @@ int dirb200_index_search_finish(dirb200_index* h, const float* q32, const float*
   return search_finish_impl(h, q32, sel_dev, scores_dev, idx_dev, static_cast<cudaStream_t>(stream_), PeerX{}, nullptr);
 }
 
-// Single-shard search = phase 1 with k_shard = k followed directly by phase 2.
+int dirb200_index_search_max_queries(dirb200_index* h, int k, int* q_max) {
+  DIRB_REQUIRE(h && q_max, DIRB200_EINVAL, "null argument");
+  DIRB_REQUIRE(h->has_db, DIRB200_ESTATE, "index has no database attached");
+  DIRB_REQUIRE(k > 0 && k <= K_MAX, DIRB200_ENOTSUP, "need 0 < k <= %d (got k=%d)", K_MAX, k);
+  *q_max = search_max_queries(h, k);
+  return 0;
+}
+
+// Single-shard search = phase 1 with k_shard = k followed directly by phase 2, in blocks of at most
+// dirb200_index_search_max_queries queries (one block unless Q * k outgrows option ws_budget).
 int dirb200_index_search(dirb200_index* h, const float* q32, int Q, int k, double* scores_dev, int64_t* idx_dev,
                          void* stream_) {
   DIRB_REQUIRE(h && q32 && scores_dev && idx_dev, DIRB200_EINVAL, "null argument");
   DIRB_REQUIRE(Q > 0, DIRB200_ENOTSUP, "need Q > 0");
-  DIRB_TRY(grow_device(reinterpret_cast<void**>(&h->sel_own), &h->sel_bytes, static_cast<size_t>(Q) * 4));
-  DIRB_TRY(dirb200_index_search_begin(h, q32, Q, k, k, h->sel_own, stream_));
-  return dirb200_index_search_finish(h, q32, h->sel_own, scores_dev, idx_dev, stream_);
+  int qb = Q;
+  if (h->has_db && k > 0 && k <= K_MAX) qb = std::min(Q, search_max_queries(h, k));   // (bad arguments: _begin reports them)
+  DIRB_TRY(grow_device(reinterpret_cast<void**>(&h->sel_own), &h->sel_bytes, static_cast<size_t>(qb) * 4));
+  for (int q0 = 0; q0 < Q; q0 += qb) {
+    const int nb = std::min(qb, Q - q0);
+    const float* qq = q32 + static_cast<int64_t>(q0) * h->dim;
+    const int64_t o = static_cast<int64_t>(q0) * k;
+    DIRB_TRY(dirb200_index_search_begin(h, qq, nb, k, k, h->sel_own, stream_));
+    DIRB_TRY(dirb200_index_search_finish(h, qq, h->sel_own, scores_dev + o, idx_dev + o, stream_));
+  }
+  return 0;
 }
 
 // ---- rank counting (see the kernels above): exact scores of the labelled rows + number of rows ranking before them
@@ -1344,10 +1616,21 @@ int dirb200_topk_merge(const double* scores_dev, const int64_t* idx_dev, int G, 
                        double* out_scores_dev, int64_t* out_idx_dev, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DIRB_REQUIRE(scores_dev && idx_dev && out_scores_dev && out_idx_dev, DIRB200_EINVAL, "null argument");
-  DIRB_REQUIRE(G >= 1 && Q >= 1 && k >= 1 && static_cast<int64_t>(G) * k <= 4096, DIRB200_ENOTSUP,
-               "merge supports G*k <= 4096 (got G=%d k=%d)", G, k);
+  DIRB_REQUIRE(G >= 1 && Q >= 1 && k >= 1, DIRB200_EINVAL, "need G, Q, k >= 1 (got G=%d Q=%d k=%d)", G, Q, k);
   // shard g holds [Q][k] at element offset g*shard_stride, each list already ordered: rank-based merge, read in place
   if (shard_stride <= 0) shard_stride = static_cast<int64_t>(Q) * k;
+  const int64_t n64 = static_cast<int64_t>(G) * k;
+  if (n64 > 4096) {                          // the lists do not fit in shared memory: merge straight from global memory
+    const int64_t qk = static_cast<int64_t>(Q) * k;
+    fill_empty_result_kernel<<<static_cast<unsigned>(ceil_div(qk, 256)), 256, 0, stream>>>(out_scores_dev, out_idx_dev, qk);
+    count_launch();
+    DIRB_REQUIRE(ceil_div(n64, 256) < (int64_t(1) << 31), DIRB200_ENOTSUP, "G*k too large (G=%d k=%d)", G, k);
+    merge_runs_kernel<<<dim3(static_cast<unsigned>(ceil_div(n64, 256)), std::min(Q, 65535)), 256, 0, stream>>>(
+        scores_dev, idx_dev, G, k, shard_stride, k, nullptr, 0, Q, k, out_scores_dev, out_idx_dev);
+    count_launch();
+    DIRB_CUDA(cudaGetLastError());
+    return 0;
+  }
   const int n = G * k;
   const int threads = std::min(1024, (n + 31) / 32 * 32);
   merge_lists_kernel<<<Q, threads, static_cast<size_t>(n) * 16, stream>>>(scores_dev, idx_dev, G, k, shard_stride, out_scores_dev,
@@ -1557,9 +1840,9 @@ int dirb200_aqe_expand(const float* q_dev, int Q, int D, const float* db32_dev, 
   DIRB_REQUIRE(q_dev && nn_idx_dev && nn_scores_dev && out_dev && (db32_dev || (partial && n_rows == 0)), DIRB200_EINVAL,
                "null argument");
   DIRB_REQUIRE(k >= 1 && alpha >= 0, DIRB200_EINVAL, "k and alpha must be non-negative (test_dir.py:25)");
-  DIRB_REQUIRE(k <= 2048, DIRB200_ENOTSUP, "at most 2048 neighbours per query (got %d)", k);
   if (Q == 0) return 0;
-  const size_t smem = static_cast<size_t>((k + 1) & ~1) * 4 + static_cast<size_t>(k) * 8;
+  const int kc = std::min(k, AQE_CHUNK);
+  const size_t smem = static_cast<size_t>((kc + 1) & ~1) * 4 + static_cast<size_t>(kc) * 8;
   aqe_kernel<<<Q, 256, smem, stream>>>(q_dev, D, db32_dev, nn_idx_dev, nn_scores_dev, k, alpha, partial, row_offset,
                                        n_rows, out_dev);
   count_launch();

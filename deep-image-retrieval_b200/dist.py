@@ -59,6 +59,7 @@ class ShardedIndex:
         self.local = ops.Index(db32_local, index_offset=row_offset, db16=db16_local)
         self.local.set_option("retries", 2)      # a rank cannot re-run alone (collectives): one more gated retry pass up front
         self.xchg = None                         # peer-memory exchange window (enable_peer_exchange)
+        self._qmax = {}                          # k -> query block of the collective path (_max_queries)
         # row counts of all shards (one small all-gather at construction, not on the search path): the selection depth
         # of the two-phase search depends on them, see shard_quota
         world = dist.get_world_size(group) if dist.is_initialized() else 1
@@ -141,15 +142,29 @@ class ShardedIndex:
             if check:
                 self.local.check()
             return out
-        sel = self.local.search_begin(q32, k, k_shard)
-        dist.all_reduce(sel, op=dist.ReduceOp.MIN, group=self.group)
-        packed = torch.empty((2, q32.shape[0], k), dtype=torch.int64, device=q32.device)
-        self.local.search_finish(q32, k, sel, out=packed)
-        gathered = all_gather_packed(packed, self.group)
-        out = self.ops.topk_merge_packed(gathered, k)
+        qb = self._max_queries(k)
+        parts = []
+        for q0 in range(0, q32.shape[0], qb):               # query blocks whose workspace fits every shard's budget
+            qc = q32[q0:q0 + qb].contiguous()
+            sel = self.local.search_begin(qc, k, k_shard)
+            dist.all_reduce(sel, op=dist.ReduceOp.MIN, group=self.group)
+            packed = torch.empty((2, qc.shape[0], k), dtype=torch.int64, device=q32.device)
+            self.local.search_finish(qc, k, sel, out=packed)
+            gathered = all_gather_packed(packed, self.group)
+            parts.append(self.ops.topk_merge_packed(gathered, k))
+        out = parts[0] if len(parts) == 1 else (torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts]))
         if check:
             self.local.check()
         return out
+
+    def _max_queries(self, k: int) -> int:
+        """Query block of a depth-k search: the smallest search_max_queries(k) over the shards (one MIN all-reduce the
+        first time each k is seen; every rank calls search() with the same k, so the ranks fill the cache in step)."""
+        if k not in self._qmax:
+            t = torch.tensor([self.local.search_max_queries(k)], dtype=torch.int64, device=self.local.db32.device)
+            dist.all_reduce(t, op=dist.ReduceOp.MIN, group=self.group)
+            self._qmax[k] = int(t.item())
+        return self._qmax[k]
 
     def check(self):
         """Status of the last search(check=False)."""

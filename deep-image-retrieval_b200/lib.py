@@ -80,6 +80,7 @@ SIGNATURES = {
     "dirb200_index_set_db": (i32, [p, p, p, i64, i64]),
     "dirb200_index_set_option": (i32, [p, C.c_char_p, f64]),
     "dirb200_index_search": (i32, [p, p, i32, i32, p, p, p]),
+    "dirb200_index_search_max_queries": (i32, [p, i32, C.POINTER(C.c_int)]),
     "dirb200_index_search_begin": (i32, [p, p, i32, i32, i32, p, p]),
     "dirb200_index_search_finish": (i32, [p, p, p, p, p, p]),
     "dirb200_index_check": (i32, [p]),

@@ -483,6 +483,12 @@ class Index:
                 self.set_option("cand_cap", 0)
         return scores, idx
 
+    def search_max_queries(self, k: int) -> int:
+        """Most queries one search_begin of depth k takes within option 'ws_budget' (search() splits larger Q itself)."""
+        out = C.c_int()
+        lib.call("dirb200_index_search_max_queries", self._h, int(k), C.byref(out))
+        return int(out.value)
+
     def search_begin(self, q32: torch.Tensor, k: int, k_shard: int):
         """Phase 1 of a sharded search -> sel (Q,) fp32: local k_shard-th best fp16-path score (MIN-reduce it)."""
         _chk(q32, torch.float32, "q32")
@@ -589,7 +595,10 @@ class Index:
         arr = (C.c_double * 9)()
         lib.call("dirb200_index_last_profile", self._h, arr)
         names = ["prep", "seed_gemm", "seed_kth", "filter_gemm", "cand_select", "retry_gates", "finish"]
-        return {n: float(arr[i]) for i, n in enumerate(names)}
+        out = {n: float(arr[i]) for i, n in enumerate(names)}
+        if arr[7] or arr[8]:                        # k > 1024: the finish in three steps
+            out.update(finish=arr[6] + arr[7] + arr[8], finish_compact=arr[6], finish_rescore=arr[7], finish_sort=arr[8])
+        return out
 
     def close(self):
         if self._h:

@@ -55,10 +55,6 @@ def expand_descriptors(descs, db=None, alpha=0, k=0, q_block=4096, to_numpy=True
     assert k >= 0 and alpha >= 0, "k and alpha must be non-negative"
     if k == 0:
         return descs
-    if k + (db is None) > 1024:
-        # the reference expands with any k (a full argsort per query); the exact top-k search returns at most 1024 rows
-        raise ValueError("query expansion / database augmentation with more than %d neighbours is not supported "
-                         "(dirb200_index_search returns at most 1024 rows per query); got k=%d" % (1024 - (db is None), k))
     dim = np.shape(descs)[1]
     pad = (-dim) % 64                      # the tensor-core search wants D % 64 == 0; zero columns change no score
 
@@ -322,7 +318,7 @@ def _aps_from_topk(db, qdescs, bdescs, k):
     pad = (-dim) % 64
     f = lambda a: torch.nn.functional.pad(_dev_f32(a), (0, pad)).contiguous() if pad else _dev_f32(a)
     qd, bd = f(qdescs), f(bdescs)
-    k = min(k, bd.shape[0], 1024)
+    k = min(k, bd.shape[0])
     _, idx = ops.Index(bd).search(qd, k)
     idx = idx.cpu().numpy()
     aps = []
@@ -619,10 +615,13 @@ def test_dir_main(argv=None):
     parser.add_argument("--save-feats", type=str, default="", help="path to output features")
     parser.add_argument("--load-feats", type=str, default="", help="path to load features from")
     parser.add_argument("--gpu", type=int, default=0, nargs="+", help="GPU ids")
-    parser.add_argument("--aqe", type=float, nargs="+", help="alpha-query expansion parameters: k alpha")
-    parser.add_argument("--adba", type=float, nargs="+", help="alpha-database augmentation parameters: k alpha")
+    parser.add_argument("--aqe", type=float, nargs="+",
+                        help="alpha-query expansion parameters: k alpha (any k: the k nearest rows come from the exact top-k search)")
+    parser.add_argument("--adba", type=float, nargs="+",
+                        help="alpha-database augmentation parameters: k alpha (any k; with k >= the number of rows every other row is a neighbour)")
     parser.add_argument("--rank-topk", type=int, default=0,
-                        help="(extension) rank with the exact top-k search (k <= 1024) instead of the dense score matrix")
+                        help="(extension) rank with the exact top-k search (any k; queries whose positives lie deeper fall "
+                             "back to their dense score row) instead of the dense score matrix")
     parser.add_argument("--dense-scores", action="store_true",
                         help="(extension) force the reference's literal matmul + per-query sort instead of GPU rank counts")
     args = parser.parse_args(argv)

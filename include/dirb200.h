@@ -245,14 +245,22 @@ int dirb200_index_set_db(dirb200_index* idx, const float* db32_dev, const void* 
  * retry passes enqueued after the filter pass (default 1; they return at once unless a list overflowed);
  * "deferred_check" = 1: search calls never synchronise the host, the caller collects the status with
  * dirb200_index_check (it is also collected at the start of the next search); "profile"; "count_eps" / "band_cap":
- * see dirb200_index_count_ge. */
+ * see dirb200_index_count_ge; "ws_budget": bytes of search workspace a call may use (default 4 GiB), which sets the
+ * largest query block (dirb200_index_search_max_queries). */
 int dirb200_index_set_option(dirb200_index* idx, const char* key, double value);
-/* q32_dev [Q][dim] fp32.  Outputs (device): scores_dev [Q][k] fp64 exact scores, idx_dev [Q][k] int64.
- * If N < k the tail is filled with score -inf / index -1.  Everything is enqueued on `stream`; the call then waits
- * once for the status block (overflow that the device-side retries could not resolve -> DIRB200_EOVERFLOW) unless
- * option "deferred_check" is set. */
+/* q32_dev [Q][dim] fp32, any Q >= 1, 1 <= k <= 2^27.  Outputs (device): scores_dev [Q][k] fp64 exact scores, idx_dev
+ * [Q][k] int64.  If N < k the tail is filled with score -inf / index -1.  k <= 1024 re-scores and sorts the survivors
+ * of each query in shared memory (at most 1024 survivors for k <= 256, 2048 above); k > 1024 keeps them in global
+ * memory (at most min(2k, N) per query) and orders them with sorted runs and a rank-based merge.  Queries run in blocks
+ * of dirb200_index_search_max_queries(k).  Everything is enqueued on `stream`; the call then waits once per block for
+ * the status block (overflow that the device-side retries could not resolve, or more survivors than the limit above ->
+ * DIRB200_EOVERFLOW) unless option "deferred_check" is set. */
 int dirb200_index_search(dirb200_index* idx, const float* q32_dev, int Q, int k, double* scores_dev,
                          int64_t* idx_dev, void* stream);
+/* Largest Q that one dirb200_index_search_begin of depth k accepts: its workspace (fp16 queries, seed scores, candidate
+ * and survivor lists, all proportional to Q and growing with k) must fit option "ws_budget".  At least 1; at most 65535
+ * when the search keeps one grid row per query (k > 1024, or N within the dense seed sample). */
+int dirb200_index_search_max_queries(dirb200_index* idx, int k, int* q_max);
 /* The same search in two phases, for a database sharded over several GPUs.  Phase 1 runs the tensor-core passes and
  * writes to sel_dev[Q] (caller-owned) the local min(k_shard, N_local)-th best fp16-path score per query (+inf for an
  * empty shard).  The caller MIN-reduces sel_dev over the shards (ncclAllReduce, 4*Q bytes): shard g holds
@@ -261,7 +269,8 @@ int dirb200_index_search(dirb200_index* idx, const float* q32_dev, int Q, int k,
  * satisfies it when every shard holds at least that many rows; with small shards use a larger value (k always
  * works; deep-image-retrieval_b200/dist.py: shard_quota picks the smallest valid one from the shard sizes).  The
  * tight bound lets each shard re-score only ~1.4 * k / shards rows instead of ~1.4 * k.  Phase 2 re-scores the rows
- * within the band of max(sel_dev[q], local k-th) exactly and returns the shard's ordered list. */
+ * within the band of max(sel_dev[q], local k-th) exactly and returns the shard's ordered list.  Limits as for
+ * dirb200_index_search, except that _begin refuses Q > dirb200_index_search_max_queries(k) with DIRB200_ENOTSUP. */
 int dirb200_index_search_begin(dirb200_index* idx, const float* q32_dev, int Q, int k, int k_shard, float* sel_dev,
                                void* stream);
 int dirb200_index_search_finish(dirb200_index* idx, const float* q32_dev, const float* sel_dev, double* scores_dev,
@@ -274,7 +283,8 @@ int dirb200_index_check(dirb200_index* idx);
 int dirb200_index_last_stats(dirb200_index* idx, int64_t stats[5]);
 /* With option "profile" = 1: CUDA-event milliseconds of the phases of the last search (valid after its status was
  * collected), out9[0..6] = {query fp16 conversion + clears, seed GEMM, seed k-th select, filter GEMM, candidate k-th
- * select, gated retry passes (+ any cross-shard exchange between the phases), survivors + exact re-scoring + sort}. */
+ * select, gated retry passes (+ any cross-shard exchange between the phases), survivors + exact re-scoring + sort};
+ * for k > 1024 out9[6..8] = {survivor compaction, exact re-scoring, run sort + merge}. */
 int dirb200_index_last_profile(dirb200_index* idx, double out9[9]);
 int dirb200_index_destroy(dirb200_index* idx);
 
@@ -315,7 +325,8 @@ int dirb200_index_count_ge(dirb200_index* idx, const float* q32_dev, int Q, cons
  * dirb200_index_search outputs: each list ordered best first, empty slots = index -1 at the tail, no row in two
  * lists) into the global top-k with the same ordering rule.  Shard g's [Q][k] block starts
  * shard_stride elements after shard g-1's (0 = dense [G][Q][k]); a packed all-gather buffer [G][2][Q][k] uses
- * shard_stride = 2*Q*k with idx_dev = scores_dev + Q*k. */
+ * shard_stride = 2*Q*k with idx_dev = scores_dev + Q*k.  Any G and k: up to G*k = 4096 the lists of a query are merged
+ * in shared memory, beyond that straight from global memory (same rank-based merge, same result). */
 int dirb200_topk_merge(const double* scores_dev, const int64_t* idx_dev, int G, int Q, int k, int64_t shard_stride,
                        double* out_scores_dev, int64_t* out_idx_dev, void* stream);
 /* Sharded search over PEER MEMORY (one process per GPU of one NVLink / NVSwitch box; the reference's analogue of a
@@ -354,7 +365,8 @@ int dirb200_scores_exact(const float* q_dev, int Q, const float* db_dev, int64_t
  * n_rows > 0): the indices are GLOBAL and db32_dev holds the rows [row_offset, row_offset+n_rows) of a sharded
  * database; neighbours owned by other shards are skipped (an EMPTY shard, n_rows == 0 with partial != 0, owns none and
  * may pass db32_dev = NULL).  Otherwise (partial == 0 and n_rows <= 0) the indices are plain rows of db32_dev.
- * partial != 0 writes the un-normalised SUM over the owned neighbours only, for a cross-GPU all-reduce. */
+ * partial != 0 writes the un-normalised SUM over the owned neighbours only, for a cross-GPU all-reduce.  Any k >= 1:
+ * the weights are taken 2048 at a time, and every output element accumulates its neighbours in list order. */
 int dirb200_aqe_expand(const float* q_dev, int Q, int D, const float* db32_dev, const int64_t* nn_idx_dev,
                        const double* nn_scores_dev, int k, double alpha, int partial, int64_t row_offset, int64_t n_rows,
                        float* out_dev, void* stream);
