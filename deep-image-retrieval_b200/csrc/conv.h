@@ -94,4 +94,9 @@ int f32_to_f16(const float* x, int64_t n, __half* out, cudaStream_t stream);
 int whiten(const float* x, int64_t N, int D, const float* comp, const float* mean, const float* colscale, int Dout,
            int l2norm, float* y, __half* y16, cudaStream_t stream);
 
+// Per-device scratch buffer kept for the life of the process (ops.cu): acquire grows it to `bytes` and orders `stream`
+// after the previous user; release marks the end of this stream's use.
+int scratch_acquire(size_t bytes, cudaStream_t stream, void** out);
+int scratch_release(cudaStream_t stream);
+
 }  // namespace dirb

@@ -688,7 +688,7 @@ DevScratch g_scratch[64];
 std::mutex g_scratch_mu;
 }  // namespace
 
-static int scratch_acquire(size_t bytes, cudaStream_t stream, void** out) {
+int scratch_acquire(size_t bytes, cudaStream_t stream, void** out) {
   int dev = 0;
   DIRB_CUDA(cudaGetDevice(&dev));
   DIRB_REQUIRE(dev >= 0 && dev < 64, DIRB200_ENOTSUP, "device index %d out of range", dev);
@@ -705,7 +705,7 @@ static int scratch_acquire(size_t bytes, cudaStream_t stream, void** out) {
   return 0;
 }
 
-static int scratch_release(cudaStream_t stream) {
+int scratch_release(cudaStream_t stream) {
   int dev = 0;
   DIRB_CUDA(cudaGetDevice(&dev));
   std::lock_guard<std::mutex> lock(g_scratch_mu);

@@ -101,6 +101,10 @@ SIGNATURES = {
     "dirb200_index_search_sharded_phase": (i32, [p, p, i32, p, i32, i32, i32, p, p, p]),
     "dirb200_scores_exact": (i32, [p, i32, p, i64, i32, p, p]),
     "dirb200_aqe_expand": (i32, [p, i32, i32, p, p, p, i32, f64, i32, i64, i64, p, p]),
+    # the statistics of sklearn's PCA.fit (_pca.py, _fit_full): the column sums behind mean_, and the centred Gram that
+    # replaces the covariance_eigh branch's X^T X - n m m^T
+    "dirb200_col_sums_f64": (i32, [p, i64, i32, p, p]),
+    "dirb200_gram_f64": (i32, [p, i64, i32, p, p, p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -344,6 +344,56 @@ def scores_exact(q, db):
     return out
 
 
+def _pad4(x):
+    """(N,D) fp32 -> (N,D') with D' = D rounded up to a multiple of 4 (zero columns), and D."""
+    d = x.shape[1]
+    pad = (-d) % 4
+    return (torch.nn.functional.pad(x, (0, pad)).contiguous() if pad else x), d
+
+
+def col_sums_f64(x, out=None):
+    """Column sums of x (N,D) fp32 CUDA in fp64, in a fixed order (bit-identical on every run).  out: optional (D,)
+    fp64 CUDA buffer the sums are ADDED to (rows fed in chunks); returned."""
+    _chk(x, torch.float32, "x")
+    xp, d = _pad4(x)
+    if out is None:
+        out = torch.zeros(d, dtype=torch.float64, device=x.device)
+    _chk(out, torch.float64, "out")
+    if tuple(out.shape) != (d,):
+        raise ValueError("out must have shape (%d,)" % d)
+    buf = out if xp.shape[1] == d else torch.nn.functional.pad(out, (0, xp.shape[1] - d)).contiguous()
+    lib.call("dirb200_col_sums_f64", _ptr(xp), xp.shape[0], xp.shape[1], _ptr(buf), _stream())
+    if buf is not out:
+        out.copy_(buf[:d])
+    return out
+
+
+def gram_f64(x, mean, out=None):
+    """Centred Gram matrix G += (x - mean)^T (x - mean), fp64 (D,D), the centring done in fp64; x (N,D) fp32, mean (D,)
+    fp64, CUDA.  out: optional (D,D) fp64 CUDA buffer the Gram is ADDED to (rows fed in chunks); returned.  Any D up
+    to 8064: other D than multiples of 4 go through zero columns (zero mean), which add nothing."""
+    _chk(x, torch.float32, "x")
+    _chk(mean, torch.float64, "mean")
+    xp, d = _pad4(x)
+    if tuple(mean.shape) != (d,):
+        raise ValueError("mean must have shape (%d,)" % d)
+    if out is None:
+        out = torch.zeros((d, d), dtype=torch.float64, device=x.device)
+    _chk(out, torch.float64, "out")
+    if tuple(out.shape) != (d, d):
+        raise ValueError("out must have shape (%d, %d)" % (d, d))
+    dp = xp.shape[1]
+    if dp != d:
+        mean = torch.nn.functional.pad(mean, (0, dp - d)).contiguous()
+        buf = torch.nn.functional.pad(out, (0, dp - d, 0, dp - d)).contiguous()
+    else:
+        buf = out
+    lib.call("dirb200_gram_f64", _ptr(xp), xp.shape[0], dp, _ptr(mean), _ptr(buf), _stream())
+    if buf is not out:
+        out.copy_(buf[:d, :d])
+    return out
+
+
 def topk_merge(scores, idx, k):
     """scores/idx: (G,Q,k) fp64 / int64 per-shard lists with global indices -> merged (Q,k)."""
     _chk(scores, torch.float64, "scores")

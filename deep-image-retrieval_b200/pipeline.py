@@ -650,6 +650,69 @@ def test_dir_main(argv=None):
     return res
 
 
+def merge_pca(checkpoint, name, pca):
+    """A shallow copy of the checkpoint dict whose 'pca' dict (a new one; other entries kept) maps name -> pca.
+    -> (new checkpoint, True if an entry of that name was replaced)."""
+    pcas = dict(checkpoint.get("pca") or {})
+    replaced = name in pcas
+    pcas[name] = pca
+    out = dict(checkpoint)
+    out["pca"] = pcas
+    return out, replaced
+
+
+def learn_whiten_main(argv=None):
+    """python -m dirtorch.learn_whiten (extension; the reference has no such command): fit PCA(whiten=True) on the GPU
+    (whitening.fit_pca) and write a copy of the checkpoint with pca[--name] set, for test_dir / extract_features
+    --whiten NAME.  The descriptors come from exactly one of: --dataset (extracted, pooled and normalised as
+    extract_features does, without whitening; database images only), --load-feats (an .npy of such descriptors) or
+    --store (a descriptor store of extract_to_store)."""
+    import argparse
+    from .whitening import fit_pca
+    parser = argparse.ArgumentParser(description="Learn a PCA whitening on the GPU and store it in a checkpoint")
+    parser.add_argument("--checkpoint", type=str, required=True, help="path to weights")
+    parser.add_argument("--name", type=str, required=True, help="name of the whitening in checkpoint['pca']")
+    parser.add_argument("--output", type=str, required=True, help="path of the checkpoint to write")
+    parser.add_argument("--dataset", "-d", type=str, default="", help="command to load the dataset to fit on")
+    parser.add_argument("--load-feats", type=str, default="", help=".npy of descriptors to fit on")
+    parser.add_argument("--store", type=str, default="", help="descriptor store to fit on")
+    parser.add_argument("--trfs", type=str, required=False, default="", nargs="+", help="test transforms (can be several)")
+    parser.add_argument("--pooling", type=str, default="gem", help="pooling scheme if several trf chains")
+    parser.add_argument("--gemp", type=int, default=3, help="GeM pooling power")
+    parser.add_argument("--threads", type=int, default=8, help="number of thread workers")
+    parser.add_argument("--n-components", type=int, default=None, help="number of components kept (default: all)")
+    parser.add_argument("--gpu", type=int, default=0, help="GPU id")
+    args = parser.parse_args(argv)
+    if sum(bool(s) for s in (args.dataset, args.load_feats, args.store)) != 1:
+        parser.error("exactly one of --dataset, --load-feats and --store is required")
+    if os.path.abspath(args.output) == os.path.abspath(args.checkpoint):
+        parser.error("--output must differ from --checkpoint")
+    common.torch_set_gpu([args.gpu])
+    if args.dataset:
+        dataset = datasets.create(args.dataset)
+        print("Dataset:", dataset)
+        net = load_model(args.checkpoint, True)
+        descs = []
+        for trf in [args.trfs] if isinstance(args.trfs, str) else args.trfs:
+            kw = dict(iscuda=net.iscuda, threads=args.threads, batch_size=16, same_size="Pad" in trf or "Crop" in trf)
+            descs.append(extract_image_features(dataset, trf, net, desc="DB", **kw))
+        X = _pool_and_normalize(descs, args.pooling, args.gemp)
+        del net
+    elif args.load_feats:
+        X = np.load(args.load_feats, mmap_mode="r")
+    else:
+        X = DescriptorStore(args.store)
+    pca = fit_pca(X, n_components=args.n_components)
+    print(">> PCA fit on %d x %d descriptors: %d components, %.4g of the variance kept" % (
+        pca.n_samples_, pca.n_features_in_, pca.n_components_, float(np.sum(pca.explained_variance_ratio_))))
+    checkpoint = torch.load(args.checkpoint, map_location="cpu", weights_only=False)
+    checkpoint, replaced = merge_pca(checkpoint, args.name, pca)
+    if replaced:
+        print("replacing the existing whitening '%s'" % args.name)
+    common.save_checkpoint(checkpoint, False, args.output)
+    return pca
+
+
 def extract_features_main(argv=None):
     """python -m dirtorch.extract_features (extract_features.py:82-124)."""
     import argparse

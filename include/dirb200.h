@@ -371,6 +371,18 @@ int dirb200_aqe_expand(const float* q_dev, int Q, int D, const float* db32_dev, 
                        const double* nn_scores_dev, int k, double alpha, int partial, int64_t row_offset, int64_t n_rows,
                        float* out_dev, void* stream);
 
+/* The statistics of a PCA fit, in fp64 (replaces the host work of sklearn's PCA.fit, _pca.py _fit_full).  x_dev
+ * [N][D] fp32 row-major, any N >= 0.  Both ADD into the caller's buffers, so rows may be fed in chunks; both run in a
+ * fixed summation order that depends on (N, D) only (no atomics): the same call gives bit-identical results on every
+ * run and every device.  Scratch comes from the library's per-device cache.
+ * dirb200_col_sums_f64: sum_dev[j] += sum_i x[i][j].
+ * dirb200_gram_f64: gram_dev[i][j] += sum_r (x[r][i] - mean[i]) (x[r][j] - mean[j]), the full symmetric [D][D]
+ * matrix, centred in fp64 (the covariance_eigh branch forms X^T X - n m m^T instead, which cancels when |mean| is
+ * large against the spread).  D % 4 == 0 (else DIRB200_EINVAL) and D <= 8064 (else DIRB200_ENOTSUP: the split-K
+ * partial tiles are bounded to 256 MiB). */
+int dirb200_col_sums_f64(const float* x_dev, int64_t N, int D, double* sum_dev, void* stream);
+int dirb200_gram_f64(const float* x_dev, int64_t N, int D, const double* mean_dev, double* gram_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
