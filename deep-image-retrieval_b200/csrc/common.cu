@@ -152,6 +152,16 @@ int encode_tmap_nhwc_halo(CUtensorMap* m, const void* base, int B, int H, int W,
   return 0;
 }
 
+int require_sm90() {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) {
+    cudaGetLastError();
+    set_error("no CUDA device");
+    return DIRB200_ENODEVICE;
+  }
+  return dirb200_device_check(dev);
+}
+
 }  // namespace dirb
 
 extern "C" {

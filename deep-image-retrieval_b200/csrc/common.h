@@ -86,6 +86,9 @@ inline bool first_launch_on_device(std::atomic<uint64_t>& mask) {
   return true;
 }
 
+// dirb200_device_check of the current device: DIRB200_ENODEVICE when there is none or it is not sm_90.
+int require_sm90();
+
 // Launch counter (the "gpu_launches" the benchmark reports): every kernel launch of this library bumps it.
 void count_launch(int n = 1);
 int64_t launches_total();

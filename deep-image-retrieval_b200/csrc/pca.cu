@@ -214,16 +214,6 @@ __global__ void col_sum_reduce_kernel(const double* __restrict__ part, int P, in
   sum[j] += v;
 }
 
-int require_sm90() {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("no CUDA device");
-    return DIRB200_ENODEVICE;
-  }
-  return dirb200_device_check(dev);
-}
-
 }  // namespace
 }  // namespace dirb
 

@@ -105,6 +105,9 @@ SIGNATURES = {
     # replaces the covariance_eigh branch's X^T X - n m m^T
     "dirb200_col_sums_f64": (i32, [p, i64, i32, p, p]),
     "dirb200_gram_f64": (i32, [p, i64, i32, p, p, p]),
+    # the AP / TAP losses of loss.py: histogram + fp64 finalisation, and the elementwise backward
+    "dirb200_aploss_forward": (i32, [p, p, i64, i64, i32, p, i32, p, p, p, p]),
+    "dirb200_aploss_backward": (i32, [p, p, i64, i64, i32, p, p, p, p, p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -394,6 +394,46 @@ def gram_f64(x, mean, out=None):
     return out
 
 
+APLOSS_MODES = {"ap": 0, "tap": 1, "taps": 2}
+
+
+def _aploss_args(x, label, nq, table):
+    _chk(x, torch.float32, "x")
+    _chk(label, torch.uint8, "label")
+    _chk(table, torch.float32, "table")
+    if x.dim() != 2 or tuple(label.shape) != tuple(x.shape):
+        raise ValueError("x and label must be (N, M) tensors of the same shape")
+    if table.numel() != 4 * nq:
+        raise ValueError("table must hold 4 nq = %d values" % (4 * nq))
+    return x.shape
+
+
+def aploss_forward(x, label, nq, table, mode):
+    """Per-row AP of the quantised scores (dirb200_aploss_forward).  x (N,M) fp32, label (N,M) uint8, table the 2nq
+    weights then 2nq biases of the quantiser, mode 'ap' / 'tap' / 'taps'.  Returns (hist (N,2nq+1) int64 in units of
+    2^-32, G (N,2nq) fp64 = [dAP/dc | dAP/dcp], ap (N,) fp32)."""
+    n, m = _aploss_args(x, label, nq, table)
+    hist = torch.empty((n, 2 * nq + 1), dtype=torch.int64, device=x.device)
+    G = torch.empty((n, 2 * nq), dtype=torch.float64, device=x.device)
+    ap = torch.empty(n, dtype=torch.float32, device=x.device)
+    lib.call("dirb200_aploss_forward", _ptr(x), _ptr(label), n, m, int(nq), _ptr(table), APLOSS_MODES[mode],
+             _ptr(hist), _ptr(G), _ptr(ap), _stream())
+    return hist, G, ap
+
+
+def aploss_backward(x, label, nq, table, G, grad_ap):
+    """dx (N,M) fp32 = grad_ap[n] * sum_j (G_c + l G_cp)[n][j] dq_j/dx (dirb200_aploss_backward)."""
+    n, m = _aploss_args(x, label, nq, table)
+    _chk(G, torch.float64, "G")
+    _chk(grad_ap, torch.float32, "grad_ap")
+    if tuple(G.shape) != (n, 2 * nq) or tuple(grad_ap.shape) != (n,):
+        raise ValueError("G must be (N, 2nq) and grad_ap (N,)")
+    dx = torch.empty((n, m), dtype=torch.float32, device=x.device)
+    lib.call("dirb200_aploss_backward", _ptr(x), _ptr(label), n, m, int(nq), _ptr(table), _ptr(G), _ptr(grad_ap),
+             _ptr(dx), _stream())
+    return dx
+
+
 def topk_merge(scores, idx, k):
     """scores/idx: (G,Q,k) fp64 / int64 per-shard lists with global indices -> merged (Q,k)."""
     _chk(scores, torch.float64, "scores")

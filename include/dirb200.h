@@ -383,6 +383,25 @@ int dirb200_aqe_expand(const float* q_dev, int Q, int D, const float* db32_dev, 
 int dirb200_col_sums_f64(const float* x_dev, int64_t N, int D, double* sum_dev, void* stream);
 int dirb200_gram_f64(const float* x_dev, int64_t N, int D, const double* mean_dev, double* gram_dev, void* stream);
 
+/* The listwise AP loss of "Learning with Average Precision" (reference dirtorch/loss.py), without the N x 2nq x M
+ * quantised tensor.  x_dev [N][M] fp32 scores, label_dev [N][M] uint8 (0 = negative, anything else = positive), any
+ * N >= 1 and 1 <= M < 2^31 (else DIRB200_ENOTSUP), 2 <= nq <= 100.  table_dev: 4 nq fp32 on the device, the 2nq
+ * quantiser weights then the 2nq biases, built as loss.py:29-41 builds the Conv1d (the kernels rely on that shape:
+ * bin j peaks at fmaf(w_1, x, b_1) = j).  Bin j of a score is max(0, min(v_j, v_{j+nq})), v_i = fl32(fmaf(w_i, x, b_i)).
+ * dirb200_aploss_forward: mode 0 = APLoss.forward (loss.py:43-55, eps 1e-16), 1 = TAPLoss (loss.py:90-119, eps 1e-8),
+ * 2 = TAPLoss(simplified=True).  Writes hist_dev [N][2nq+1] int64 (c, cp and the positive count, each in units of
+ * 2^-32; exact, independent of the launch shape), G_dev [N][2nq] fp64 (dAP/dc, dAP/dcp) and ap_dev [N] fp32 (the
+ * per-row AP, computed in fp64 and rounded once; NaN for a row without positives, as the reference).
+ * dirb200_aploss_backward: dx_dev [N][M] = grad_ap[n] * sum_j (G_c[n][j] + l G_cp[n][j]) dq_j/dx, with torch's
+ * subgradients: clamp(min=0) passes where the min is >= 0, torch.min splits a tie 1/2 : 1/2.  Both run on `stream`
+ * with no host synchronisation and no float atomics: the results are bit-identical on every run. */
+int dirb200_aploss_forward(const float* x_dev, const uint8_t* label_dev, int64_t N, int64_t M, int nq,
+                           const float* table_dev, int mode, int64_t* hist_dev, double* G_dev, float* ap_dev,
+                           void* stream);
+int dirb200_aploss_backward(const float* x_dev, const uint8_t* label_dev, int64_t N, int64_t M, int nq,
+                            const float* table_dev, const double* G_dev, const float* grad_ap_dev, float* dx_dev,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif
