@@ -89,6 +89,14 @@ inline bool first_launch_on_device(std::atomic<uint64_t>& mask) {
 // dirb200_device_check of the current device: DIRB200_ENODEVICE when there is none or it is not sm_90.
 int require_sm90();
 
+// Sorted top-k of Q candidate lists (search.cu, the deep search's finish): list q holds min(cnt[q], cap2) pairs
+// (rows[q * cap2 + i], sc[q * cap2 + i]), cap2 a multiple of SORT_RUN.  Runs of SORT_RUN are sorted in shared memory
+// by (score desc, row asc) into sc / run_ix (the same layout), then merged by rank into out_score / out_idx [Q][k]
+// ((-inf, -1) past the end of a short list).  Q <= 65535.
+constexpr int SORT_RUN = 2048;
+int sort_runs_merge(const int* rows, const int* cnt, int cap2, double* sc, int64_t* run_ix, int Q, int k,
+                    unsigned long long* status, double* out_score, int64_t* out_idx, cudaStream_t stream);
+
 // Launch counter (the "gpu_launches" the benchmark reports): every kernel launch of this library bumps it.
 void count_launch(int n = 1);
 int64_t launches_total();

@@ -886,6 +886,22 @@ __global__ void merge_runs_kernel(const double* __restrict__ in_score, const int
 }
 
 }  // namespace
+
+static_assert(DEEP_RUN == SORT_RUN, "sort_runs_merge's run length is the deep finish's");
+
+int sort_runs_merge(const int* rows, const int* cnt, int cap2, double* sc, int64_t* run_ix, int Q, int k,
+                    unsigned long long* status, double* out_score, int64_t* out_idx, cudaStream_t stream) {
+  const int runs = cap2 / DEEP_RUN;
+  deep_run_sort_kernel<<<dim3(runs, Q), FIN_THREADS, 0, stream>>>(rows, cnt, cap2, 0, sc, run_ix, status);
+  const int64_t n = static_cast<int64_t>(Q) * k;
+  fill_empty_result_kernel<<<static_cast<unsigned>(ceil_div(n, 256)), 256, 0, stream>>>(out_score, out_idx, n);
+  const int64_t elems = static_cast<int64_t>(runs) * std::min(DEEP_RUN, k);
+  merge_runs_kernel<<<dim3(static_cast<unsigned>(ceil_div(elems, 256)), Q), 256, 0, stream>>>(
+      sc, run_ix, runs, DEEP_RUN, DEEP_RUN, cap2, cnt, cap2, Q, k, out_score, out_idx);
+  count_launch(3);
+  DIRB_CUDA(cudaGetLastError());
+  return 0;
+}
 }  // namespace dirb
 
 using namespace dirb;

@@ -108,6 +108,16 @@ SIGNATURES = {
     # the AP / TAP losses of loss.py: histogram + fp64 finalisation, and the elementwise backward
     "dirb200_aploss_forward": (i32, [p, p, i64, i64, i32, p, i32, p, p, p, p]),
     "dirb200_aploss_backward": (i32, [p, p, i64, i64, i32, p, p, p, p, p]),
+    # diffusion re-ranking (Zhou et al. 2003, Iscen et al. 2017): mutual-kNN graph, seeds, batched CG, rank counts
+    "dirb200_diffusion_graph_workspace_bytes": (C.c_size_t, [i64, i32]),
+    "dirb200_diffusion_graph": (i32, [p, p, i64, i32, i32, f64, p, p, p, p, p]),
+    "dirb200_diffusion_seeds": (i32, [p, p, i32, i32, f64, i64, p, p]),
+    "dirb200_diffusion_solve_workspace_bytes": (C.c_size_t, [i64, i32]),
+    "dirb200_diffusion_solve": (i32, [p, p, p, i64, p, i32, f64, i32, f64, p, p, p, p, p]),
+    "dirb200_diffusion_rank_count_workspace_bytes": (C.c_size_t, [i32, i32]),
+    "dirb200_diffusion_rank_count": (i32, [p, i64, i32, p, p, p, p, i32, p, p, p, p]),
+    "dirb200_diffusion_topk_workspace_bytes": (C.c_size_t, [i32, i32]),
+    "dirb200_diffusion_topk": (i32, [p, i64, i32, i32, p, p, p, p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

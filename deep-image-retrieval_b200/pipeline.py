@@ -387,9 +387,47 @@ def _aps_from_label_counts(db, qdescs, bdescs, max_thresholds=1 << 26, q_block=4
     return aps, tops
 
 
+def _aps_from_diffusion(db, qdescs, bdescs, params):
+    """Per-query AP after diffusion re-ranking (extension): the graph of the database rows, the CG solve of every
+    query, and for every positive the number of rows ranking before it by f (dirb200_diffusion_rank_count), graded by
+    datasets.eval_query_AP_from_counts with f in place of the scores."""
+    from .diffusion import Diffusion
+    build = {k: params[k] for k in ("k", "gamma") if k in params}
+    solve = {k: params[k] for k in ("kq", "alpha", "iters", "tol") if k in params}
+    offs, rows, flags = [0], [], []
+    for q in range(qdescs.shape[0]):
+        r, fl = db.rank_targets(q)
+        rows.append(r)
+        flags.append(fl)
+        offs.append(offs[-1] + len(r))
+    rows = np.concatenate(rows) if rows else np.zeros(0, np.int64)
+    flags = np.concatenate(flags) if flags else np.zeros(0, np.uint8)
+    sc, above = Diffusion(bdescs, **build).rank_counts(qdescs, np.array(offs, np.int64), rows, flags, **solve)
+    sc, above = sc.cpu().numpy(), above.cpu().numpy()
+    return [db.eval_query_AP_from_counts(q, rows[offs[q]:offs[q + 1]], sc[offs[q]:offs[q + 1]], above[offs[q]:offs[q + 1]])
+            for q in range(qdescs.shape[0])]
+
+
+def diffusion_params(values):
+    """--diffusion K KQ [GAMMA [ALPHA]] -> the eval_model `diffusion` dict (the paper's defaults for what is not given)."""
+    from .diffusion import DEFAULTS, check_params
+    if not 2 <= len(values) <= 4:
+        raise ValueError("--diffusion takes K KQ [GAMMA [ALPHA]] (got %d values)" % len(values))
+    out = dict(DEFAULTS)
+    for key, v in zip(("k", "kq", "gamma", "alpha"), values):
+        if key in ("k", "kq") and float(v) != int(v):
+            raise ValueError("--diffusion: %s must be an integer (got %r)" % (key.upper(), v))
+        out[key] = int(v) if key in ("k", "kq") else float(v)
+    check_params(**out)
+    return out
+
+
 def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=None, aqe=None, adba=None, threads=8,
-               batch_size=16, save_feats=None, load_feats=None, dbg=(), rank_topk=0, dense_scores=False):
+               batch_size=16, save_feats=None, load_feats=None, dbg=(), rank_topk=0, dense_scores=False, diffusion=None):
     """Evaluate a network on a retrieval dataset (test_dir.py:97-180).  aqe / adba: dict(k=..., alpha=...).
+    diffusion (extension): dict of dirb200.diffusion parameters (k, kq, gamma, alpha, iters, tol); the rows are then
+    ranked by diffusion over the database's mutual-kNN graph, after whitening and alpha-DBA / alpha-QE.  Only datasets
+    with relevance lists are graded that way (NotImplementedError otherwise).
     Ranking: datasets with relevance lists (Oxford/Paris style) are graded from GPU rank counts and label datasets
     from GPU threshold counts + the exact top-100 - no Q x N score matrix, no host argsort; dense_scores=True
     (extension) forces the literal matmul + per-query sort of the reference; rank_topk > 0 (extension) grades
@@ -433,7 +471,13 @@ def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=Non
     tops = None
     qn, bn = _dev_f32(qdescs), _dev_f32(bdescs)
     unit = bool(float((qn.norm(dim=1) - 1).abs().max()) < 1e-3 and float((bn.norm(dim=1) - 1).abs().max()) < 1e-3)
-    if rank_topk and hasattr(db, "eval_query_AP_from_ranking"):
+    if diffusion is not None:
+        if not hasattr(db, "eval_query_AP_from_counts"):
+            raise NotImplementedError("diffusion re-ranking grades datasets with relevance lists (Oxford / Paris "
+                                      "style) only; %s has none" % type(db).__name__)
+        aps = _aps_from_diffusion(db, qn, bn, diffusion)
+        scores = None
+    elif rank_topk and hasattr(db, "eval_query_AP_from_ranking"):
         # Large databases: rank with the exact top-k engine instead of materialising the Q x N score matrix; a
         # query whose positives are not all inside the top-k falls back to its exact dense score row.
         aps = _aps_from_topk(db, qn, bn, int(rank_topk))
@@ -624,7 +668,14 @@ def test_dir_main(argv=None):
                              "back to their dense score row) instead of the dense score matrix")
     parser.add_argument("--dense-scores", action="store_true",
                         help="(extension) force the reference's literal matmul + per-query sort instead of GPU rank counts")
+    parser.add_argument("--diffusion", type=float, nargs="+", metavar="K KQ [GAMMA [ALPHA]]",
+                        help="(extension) rank by diffusion over the mutual K-NN graph of the database, seeded by each "
+                             "query's KQ nearest rows (defaults: gamma 3, alpha 0.99, 20 CG iterations)")
     args = parser.parse_args(argv)
+    try:
+        diffusion = diffusion_params(args.diffusion) if args.diffusion is not None else None
+    except ValueError as e:
+        parser.error(str(e))
     args.iscuda = common.torch_set_gpu(args.gpu)
     aqe = {"k": int(args.aqe[0]), "alpha": args.aqe[1]} if args.aqe is not None else None
     adba = {"k": int(args.adba[0]), "alpha": args.adba[1]} if args.adba is not None else None
@@ -635,7 +686,7 @@ def test_dir_main(argv=None):
     res = eval_model(dataset, net, args.trfs, pooling=args.pooling, gemp=args.gemp, detailed=args.detailed,
                      threads=args.threads, dbg=args.dbg, whiten=whiten, aqe=aqe, adba=adba,
                      save_feats=args.save_feats, load_feats=args.load_feats, rank_topk=args.rank_topk,
-                     dense_scores=args.dense_scores)
+                     dense_scores=args.dense_scores, diffusion=diffusion)
     # (the reference's '%s = %g' line raises on the list-valued entries that --detailed adds; print scalars only)
     print(" * " + "\n * ".join(["%s = %g" % p for p in res.items() if isinstance(p[1], (int, float))]))
     if args.out_json:

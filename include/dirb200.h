@@ -402,6 +402,50 @@ int dirb200_aploss_backward(const float* x_dev, const uint8_t* label_dev, int64_
                             const float* table_dev, const double* G_dev, const float* grad_ap_dev, float* dx_dev,
                             void* stream);
 
+/* Diffusion re-ranking: manifold ranking (Zhou et al., "Ranking on Data Manifolds", NIPS 2003) over the mutual-kNN
+ * graph of the database, solved by conjugate gradient (Iscen et al., "Efficient Diffusion on Region Manifolds", CVPR
+ * 2017).  The rules are restated in DESIGN.md section 4.7; all arithmetic is fp64 and no value is accumulated with
+ * atomics, so a given input gives bit-identical output on every run.  Workspaces are caller-owned device buffers of
+ * the *_workspace_bytes size.
+ * dirb200_diffusion_graph: nn_idx_dev / nn_score_dev [N][width] are the exact top-width lists of the database against
+ * itself (dirb200_index_search with width = k + 1, or fewer columns when N <= k; -1 entries are skipped).
+ * nn(i) = the first k entries other than i itself (by index).  Writes the CSR of
+ * S = D^-1/2 A D^-1/2 (step 2 of Zhou et al.'s algorithm, on the sparse mutual-kNN affinity of Iscen et al.): A_ij = max(s_ij, 0)^gamma for mutual neighbours (j in nn(i) and i in nn(j)), d_i = sum_j A_ij in
+ * ascending j, S_ij = A_ij * (u_i * u_j) with u_i = 1/sqrt(d_i) (0 for d_i = 0): exactly symmetric.  row_ptr_dev
+ * [N+1] int64, col_dev / val_dev capacity N * k (nnz = row_ptr[N] <= N k), columns ascending within a row.  1 <= k <=
+ * 2047 (else DIRB200_ENOTSUP), width <= k + 1, gamma > 0.
+ * dirb200_diffusion_seeds: y_dev [N][Q] (zeroed by the call) gets y[j][q] = max(s, 0)^gamma for each (j, s) of query
+ * q's top-kq list idx_dev / score_dev [Q][kq] (the query vector y of Iscen et al.; entries -1 are skipped).
+ * dirb200_diffusion_solve: (I - alpha S) f = y for the Q columns of y_dev [N][Q] (the closed form
+ * f* = (I - alpha S)^-1 y of Zhou et al.'s iteration, up to its (1 - alpha) scale) by conjugate gradient from f = 0: at most `iters` iterations, query q stops
+ * (f, r, p frozen) at the first iteration whose recurrence residual has ||r|| <= tol ||y_q||; y_q = 0 gives f = 0.
+ * Writes f_dev [N][Q], iters_dev [Q] (iterations done) and resid_dev [Q] (final recurrence ||r||).  A query's f is
+ * bit-identical whatever Q and whatever its column.  0 <= alpha < 1, iters >= 1, tol >= 0.
+ * dirb200_diffusion_rank_count: for the flagged targets t of each query (CSR offsets t_off [Q+1] on host and device,
+ * t_rows int64 in [0, N), t_flags uint8), above_dev[t] = the number of rows ranking before t_rows[t] when the column
+ * q of f_dev [N][Q] is ranked by f descending, ties -> lower index, -0 == +0 (0 for unflagged targets), and
+ * t_score_dev[t] = f[t_rows[t]][q] for every target.  At most 12000 targets per query and 65535 queries (else
+ * DIRB200_ENOTSUP).
+ * dirb200_diffusion_topk: the exact top-k rows of each column q of f_dev [N][Q] under the same order (Zhou et al.'s
+ * step 4, "rank each point according to its score f*"): scores_dev [Q][k] fp64 = f, idx_dev [Q][k] int64.  1 <= k <=
+ * N, Q <= 65535 (else DIRB200_ENOTSUP). */
+size_t dirb200_diffusion_graph_workspace_bytes(int64_t N, int k);
+int dirb200_diffusion_graph(const int64_t* nn_idx_dev, const double* nn_score_dev, int64_t N, int width, int k,
+                            double gamma, void* ws_dev, int64_t* row_ptr_dev, int* col_dev, double* val_dev, void* stream);
+int dirb200_diffusion_seeds(const int64_t* idx_dev, const double* score_dev, int Q, int kq, double gamma, int64_t N,
+                            double* y_dev, void* stream);
+size_t dirb200_diffusion_solve_workspace_bytes(int64_t N, int Q);
+int dirb200_diffusion_solve(const int64_t* row_ptr_dev, const int* col_dev, const double* val_dev, int64_t N,
+                            const double* y_dev, int Q, double alpha, int iters, double tol, void* ws_dev, double* f_dev,
+                            int* iters_dev, double* resid_dev, void* stream);
+size_t dirb200_diffusion_rank_count_workspace_bytes(int Q, int T);
+int dirb200_diffusion_rank_count(const double* f_dev, int64_t N, int Q, const int* t_off_host, const int* t_off_dev,
+                                 const int64_t* t_rows_dev, const uint8_t* t_flags_dev, int T, void* ws_dev,
+                                 double* t_score_dev, int64_t* above_dev, void* stream);
+size_t dirb200_diffusion_topk_workspace_bytes(int Q, int k);
+int dirb200_diffusion_topk(const double* f_dev, int64_t N, int Q, int k, void* ws_dev, double* scores_dev,
+                           int64_t* idx_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
