@@ -40,6 +40,16 @@ int dirb200_conv_c23(const void* t1_dev, int B, int H, int W, int Cm, const void
                   CH16(res_dev), H16(out_dev), ST(stream));
 }
 
+int dirb200_conv_c31(const void* t2_dev, int B, int H, int W, int Cm, const void* w3_dev, const float* scale3_dev,
+                     const float* shift3_dev, const void* x_dev, void* y_dev, const void* w1_dev, const float* scale1_dev,
+                     const float* shift1_dev, void* t1_dev, void* stream) {
+  DIRB_REQUIRE(t2_dev && w3_dev && scale3_dev && shift3_dev && x_dev && y_dev && w1_dev && scale1_dev && shift1_dev && t1_dev,
+               DIRB200_EINVAL, "null argument");
+  DIRB_REQUIRE(B > 0 && H > 0 && W > 0, DIRB200_EINVAL, "bad shape");
+  return conv_c31(B, H, W, Cm, CH16(t2_dev), CH16(w3_dev), scale3_dev, shift3_dev, CH16(x_dev), H16(y_dev), CH16(w1_dev),
+                  scale1_dev, shift1_dev, H16(t1_dev), ST(stream));
+}
+
 size_t dirb200_stem_workspace_bytes(int B, int H, int W) { return stem_workspace_bytes(B, H, W); }
 
 int dirb200_stem_pack_weight(const float* w_oihw_host, void* w2_host) {

@@ -10,6 +10,7 @@
 #include <algorithm>
 
 #include "conv_c23.cuh"
+#include "conv_c31.cuh"
 #include "conv_pers.cuh"
 #include "conv_stem.cuh"
 
@@ -286,6 +287,45 @@ int conv_c23(int B, int H, int W, int Cm, const __half* t1, const __half* w2, co
   if (Cm == 256) return launch_c23<256>(tmA, tmB2, tmB3, tmR, tmO, p, total, scale2, shift2, stream);
   if (Cm == 64) return launch_c23<64>(tmA, tmB2, tmB3, tmR, tmO, p, total, scale2, shift2, stream);
   return launch_c23<128>(tmA, tmB2, tmB3, tmR, tmO, p, total, scale2, shift2, stream);
+}
+
+// conv3 (1x1, Cm -> 4 Cm) + BN + residual + ReLU of identity Bottleneck b and conv1 (1x1, 4 Cm -> Cm) + BN + ReLU of
+// identity Bottleneck b+1 in one kernel (conv_c31.cuh).  t2: (B,H,W,Cm); w3: [4*Cm][Cm]; x / y: (B,H,W,4*Cm) block b's
+// input and output; w1: [Cm][4*Cm]; t1: (B,H,W,Cm) block b+1's conv1 output.
+bool conv_c31_supported(int Cm) { return Cm == 64 || Cm == 128 || Cm == 256; }
+// Each fused tile walks all 4*Cm channels of X: with fewer tiles than SMs some SMs would idle while the unfused
+// launches spread narrower tiles over all of them.
+bool conv_c31_profitable(int B, int H, int W, int Cm) {
+  return conv_c31_supported(Cm) && ceil_div(static_cast<int64_t>(B) * H * W, 128) >= num_sms();
+}
+
+int conv_c31(int B, int H, int W, int Cm, const __half* t2, const __half* w3, const float* scale3, const float* shift3,
+             const __half* x, __half* y, const __half* w1, const float* scale1, const float* shift1, __half* t1,
+             cudaStream_t stream, const ConvExt* ext) {
+  DIRB_REQUIRE(conv_c31_supported(Cm), DIRB200_ENOTSUP, "fused conv3+conv1 needs Cm in {64, 128, 256} (got %d)", Cm);
+  DIRB_REQUIRE(t2 && w3 && scale3 && shift3 && x && y && w1 && scale1 && shift1 && t1, DIRB200_EINVAL, "null argument");
+  const int64_t M = static_cast<int64_t>(B) * H * W;
+  ConvPersParams p{};
+  p.a_spatial = 0;
+  p.scale = scale3;
+  p.shift = shift3;
+  set_ext(p, ext, H, W);
+  DIRB_TRY(set_total_tiles(p, ceil_div(M, 128)));
+  CUtensorMap tmT2, tmW3, tmX, tmY, tmW1, tmT1;   // activations in 64-row boxes: each consumer warpgroup moves its own rows
+  DIRB_TRY(encode_tmap_2d(&tmT2, t2, Cm, M, (uint64_t)Cm * 2, 64, 64));
+  DIRB_TRY(encode_tmap_2d(&tmW3, w3, Cm, 4 * Cm, (uint64_t)Cm * 2, 64, C31Smem<64>::N3));
+  DIRB_TRY(encode_tmap_2d(&tmX, x, 4 * Cm, M, (uint64_t)Cm * 8, 64, 64));
+  DIRB_TRY(encode_tmap_2d(&tmY, y, 4 * Cm, M, (uint64_t)Cm * 8, 64, 64));
+  DIRB_TRY(encode_tmap_2d(&tmW1, w1, 4 * Cm, Cm, (uint64_t)Cm * 8, 64, Cm < 128 ? Cm : 128));
+  DIRB_TRY(encode_tmap_2d(&tmT1, t1, Cm, M, (uint64_t)Cm * 2, 64, 64));
+#define DIRB_C31(CM)                                                                                                   \
+  return p.ext != nullptr                                                                                              \
+             ? conv_c31_launch<CM, true>(tmT2, tmW3, tmX, tmY, tmW1, tmT1, p, scale1, shift1, num_sms(), stream)       \
+             : conv_c31_launch<CM, false>(tmT2, tmW3, tmX, tmY, tmW1, tmT1, p, scale1, shift1, num_sms(), stream)
+  if (Cm == 256) DIRB_C31(256);
+  if (Cm == 128) DIRB_C31(128);
+  DIRB_C31(64);
+#undef DIRB_C31
 }
 
 // ------------------------------------------------------------------------------------------------ stem

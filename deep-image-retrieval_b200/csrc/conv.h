@@ -35,6 +35,13 @@ bool conv_c23_profitable(int B, int H, int W, int Cm);
 int conv_c23(int B, int H, int W, int Cm, const __half* t1, const __half* w2, const float* scale2, const float* shift2,
              const __half* w3, const float* scale3, const float* shift3, const __half* res, __half* out,
              cudaStream_t stream, const ConvExt* ext = nullptr);
+// conv3 (1x1, x4) + BN + residual + ReLU of an identity Bottleneck and conv1 (1x1) + BN + ReLU of the identity
+// Bottleneck after it in one kernel (conv_c31.cuh): y = block output, t1 = the next block's conv1 output.
+bool conv_c31_supported(int Cm);
+bool conv_c31_profitable(int B, int H, int W, int Cm);
+int conv_c31(int B, int H, int W, int Cm, const __half* t2, const __half* w3, const float* scale3, const float* shift3,
+             const __half* x, __half* y, const __half* w1, const float* scale1, const float* shift1, __half* t1,
+             cudaStream_t stream, const ConvExt* ext = nullptr);
 // The same wgmma kernel with one tile per CTA (no persistence), kept as an A/B baseline (impl 2).
 int conv_tc_np(const ConvShape& s, const __half* in, const __half* w, const float* scale, const float* shift,
                const __half* res, int relu, __half* out, cudaStream_t stream, const ConvExt* ext = nullptr);

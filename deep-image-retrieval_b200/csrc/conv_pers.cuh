@@ -87,6 +87,52 @@ __device__ __forceinline__ bool row_in_extent(const ConvPersParams& p, int m_til
   return y < __ldg(p.ext + static_cast<int64_t>(n) * p.ext_ld) && x < __ldg(p.ext + static_cast<int64_t>(n) * p.ext_ld + 1);
 }
 
+// Convolution epilogue of one thread's accumulators (layout of wgmma.cuh): BN scale / shift (+ the residual already in
+// the staging buffer) (+ ReLU), ragged rows zeroed (keep bit 2 * hf + h = row r0 + 64 * hf + 8 * h lies inside its
+// image), fp16 into the staging buffer at stg_base: 128 rows x 64 channels per 128-byte-swizzled chunk, one chunk per 64
+// of the BN columns.  scale / shift point at the first column.
+template <int BN, int NH, bool RAGGED>
+__device__ __forceinline__ void conv_epilogue_to_staging(const float (&acc)[NH][BN / 2], uint32_t stg_base, int r0, int t4,
+                                                         const float* scale, const float* shift, bool has_res, bool relu,
+                                                         uint32_t keep) {
+  constexpr int STG_CHUNK = 128 * 128;
+  // this thread's rows r0 + 64 * hf + 8 * h all share r0 & 7, so their 128-byte swizzle (16-byte unit j ^ (r & 7)) is
+  // the same and the rows differ by immediate offsets
+  const uint32_t stg_addr = stg_base + r0 * 128 + t4 * 4;
+  const int rsw = r0 & 7;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = j * 8 + 2 * t4;
+    const float2 sc = __ldg(reinterpret_cast<const float2*>(scale + col));
+    const float2 sh = __ldg(reinterpret_cast<const float2*>(shift + col));
+#pragma unroll
+    for (int hf = 0; hf < NH; ++hf) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t sp = stg_addr + (j >> 3) * STG_CHUNK + (64 * hf + 8 * h) * 128 + (((j & 7) ^ rsw) << 4);
+        float v0 = fmaf(acc[hf][4 * j + 2 * h], sc.x, sh.x);
+        float v1 = fmaf(acc[hf][4 * j + 2 * h + 1], sc.y, sh.y);
+        if (has_res) {
+          uint32_t rv;
+          asm volatile("ld.shared.u32 %0, [%1];" : "=r"(rv) : "r"(sp));
+          const float2 f = unpack_h2(rv);
+          v0 += f.x;
+          v1 += f.y;
+        }
+        if (relu) {
+          v0 = fmaxf(v0, 0.f);
+          v1 = fmaxf(v1, 0.f);
+        }
+        if (RAGGED && !((keep >> (2 * hf + h)) & 1)) {                     // ragged batch: outside the image = zero padding of the next layer
+          v0 = 0.f;
+          v1 = 0.f;
+        }
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(sp), "r"(pack_h2(v0, v1)) : "memory");
+      }
+    }
+  }
+}
+
 // HALO (3x3 / stride 1 / pad 1, 8 x 16 output tiles): the ring holds weight tiles only; per 64-channel block ONE TMA box
 // brings the 10 x 18 input patch into a separate ring of NP patch slots, and the nine taps read it as shifted views.
 // PP (ping-pong consumers, convolution epilogue only): each consumer warpgroup has its own staging buffers, residual
@@ -443,41 +489,8 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (leader) bulk_wait_read<0>();            // the previous tile's stores have left the staging buffers
         named_bar_sync(epi_bar, epi_threads);
       }
-      // this thread's rows r0 + 64 * hf + 8 * h all share r0 & 7, so their 128-byte swizzle (16-byte unit j ^ (r & 7)) is
-      // the same and the rows differ by immediate offsets
-      const uint32_t stg_addr = smem_u32(stg_w) + r0 * 128 + t4 * 4;
-      const int rsw = r0 & 7;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = j * 8 + 2 * t4;
-        const float2 sc = __ldg(reinterpret_cast<const float2*>(p.scale + c.n_tile * BN + col));
-        const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + c.n_tile * BN + col));
-#pragma unroll
-        for (int hf = 0; hf < NH; ++hf) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t sp = stg_addr + (j >> 3) * L::STG_CHUNK + (64 * hf + 8 * h) * 128 + (((j & 7) ^ rsw) << 4);
-            float v0 = fmaf(acc[hf][4 * j + 2 * h], sc.x, sh.x);
-            float v1 = fmaf(acc[hf][4 * j + 2 * h + 1], sc.y, sh.y);
-            if (p.has_res) {
-              uint32_t rv;
-              asm volatile("ld.shared.u32 %0, [%1];" : "=r"(rv) : "r"(sp));
-              const float2 f = unpack_h2(rv);
-              v0 += f.x;
-              v1 += f.y;
-            }
-            if (p.relu) {
-              v0 = fmaxf(v0, 0.f);
-              v1 = fmaxf(v1, 0.f);
-            }
-            if (RAGGED && !((keep >> (2 * hf + h)) & 1)) {                     // ragged batch: outside the image = zero padding of the next layer
-              v0 = 0.f;
-              v1 = 0.f;
-            }
-            asm volatile("st.shared.u32 [%0], %1;" ::"r"(sp), "r"(pack_h2(v0, v1)) : "memory");
-          }
-        }
-      }
+      conv_epilogue_to_staging<BN, NH, RAGGED>(acc, smem_u32(stg_w), r0, t4, p.scale + c.n_tile * BN,
+                                               p.shift + c.n_tile * BN, p.has_res, p.relu, keep);
       fence_proxy_async_smem();                     // generic-proxy smem writes -> visible to the TMA engine
       named_bar_sync(epi_bar, epi_threads);
       if (leader) {

@@ -543,6 +543,14 @@ static bool c23_taken(const dirb200_net* n, int B, int h, int w, int Cm) {
          (n->fuse_c23 == 2 ? conv_c23_supported(h, w, Cm) : conv_c23_profitable(B, h, w, Cm));
 }
 
+// Whether identity Bottleneck b's conv3 and the conv1 of the block after it (next; null at the end of a stage) run as
+// the fused conv_c31 kernel for B images at h x w: both blocks stride-1 identity Bottlenecks, at most 256 mid channels
+// and a tile for every SM.  Layer4's 512 mid channels would need 256 accumulator registers per thread for conv1 alone.
+static bool c31_taken(const dirb200_net* n, const Block& b, const Block* next, int B, int h, int w) {
+  return !n->basic && n->conv_impl == 0 && next != nullptr && !b.has_down && b.c2.stride == 1 && !next->has_down &&
+         next->c2.stride == 1 && conv_c31_profitable(B, h, w, b.c3.Cin);
+}
+
 static void ragged_table(const dirb200_net* n, const int* hw, int B, std::vector<int>* t) {
   t->assign(static_cast<size_t>(B) * RG_LD, 0);
   for (int i = 0; i < B; ++i) {
@@ -654,6 +662,7 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
   // ---------------------------------------------------------------- stages 1..4: layer1..layer4
   const __half* x = w.stage_out[0];
   int first = 0;
+  bool t1_ready = false;   // the block's conv1 output was written together with the previous block's output (conv_c31)
   for (int s = 1; s < 5; ++s) {
     const int last = n->layer_end[s - 1];       // blocks [first, last)
     int lvl = 1 + s;                            // level of x
@@ -689,8 +698,11 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
         continue;
       }
       const int st = blk.c2.stride;
-      DIRB_TRY(run_conv(n, blk.c1, x, cb, h, wd, nullptr, 1, t1, stream, 0, ext(e0, lvl_in, wd)));
-      DIRB_TRY(record_tap(n, tp + ".conv1", t1, cb, h, wd, cm, stream));
+      if (!t1_ready) {
+        DIRB_TRY(run_conv(n, blk.c1, x, cb, h, wd, nullptr, 1, t1, stream, 0, ext(e0, lvl_in, wd)));
+        DIRB_TRY(record_tap(n, tp + ".conv1", t1, cb, h, wd, cm, stream));
+      }
+      t1_ready = false;
       const bool c23 = !blk.has_down && st == 1 && c23_taken(n, cb, h, wd, blk.c2.Cin);
       // ragged: a stride-1 conv2 in the K order of the slot's kernel choice (the fused kernel has the HALO order)
       const ConvExt* e2 = st == 1 ? ext3(e1, lvl, wd, blk.has_down ? 2 : 3, c23 || halo_order_plain(n, h, wd))
@@ -724,6 +736,25 @@ static int run_chunk(dirb200_net* n, const Workspace& w, const float* imgs, cons
         DIRB_TRY(conv_fused_ds(cb, h2, w2, blk.c3.Cin, t2, h, wd, blk.down.Cin, st, x, blk.wcat, blk.c3.Cout, blk.ones,
                                blk.cat_shift, y, stream, ext(e0, lvl, w2)));
         DIRB_TRY(record_tap(n, tp, y, cb, h2, w2, cout, stream));
+        x = y;
+        continue;
+      }
+      if (c31_taken(n, blk, bi + 1 < last ? &n->blocks[bi + 1] : nullptr, cb, h, wd)) {
+        // identity block followed by an identity block: conv3 (+ x) and the next block's conv1 in one kernel, the
+        // block output feeds conv1 from shared memory; the next block starts at conv2
+        const int Cm = blk.c3.Cin;
+        const double flops = 2.0 * cb * h * wd * (8.0 * Cm * Cm);
+        const double bytes = 2.0 * (static_cast<double>(cb) * h * wd * (2.0 * Cm + 8.0 * Cm) + 8.0 * Cm * Cm);   // t2 + t1, x + y, weights
+        n->last_flops += flops;
+        char tg[96];
+        snprintf(tg, sizeof(tg), "1x1 %d->%d +res + 1x1 ->%d fused @%dx%d", Cm, 4 * Cm, Cm, h, wd);
+        ProfScope ps(n, stream, 0, flops, bytes, tg);
+        const Block& nx = n->blocks[bi + 1];
+        DIRB_TRY(conv_c31(cb, h, wd, Cm, t2, blk.c3.w, blk.c3.scale, blk.c3.shift, x, y, nx.c1.w, nx.c1.scale, nx.c1.shift,
+                          t1, stream, ext(e0, lvl, w2)));
+        DIRB_TRY(record_tap(n, tp, y, cb, h, wd, cout, stream));
+        DIRB_TRY(record_tap(n, "layer" + std::to_string(s) + "." + std::to_string(j + 1) + ".conv1", t1, cb, h, wd, Cm, stream));
+        t1_ready = true;
         x = y;
         continue;
       }

@@ -64,6 +64,7 @@ SIGNATURES = {
     "dirb200_nchw_to_nhwc8": (i32, [p, i32, i32, i32, p, p]),
     "dirb200_conv_bn_act": (i32, [p, i32, i32, i32, i32, p, i32, i32, i32, i32, i32, p, p, p, i32, i32, p, p]),
     "dirb200_conv_c23": (i32, [p, i32, i32, i32, i32, p, p, p, p, p, p, p, p, i32, p]),
+    "dirb200_conv_c31": (i32, [p, i32, i32, i32, i32, p, p, p, p, p, p, p, p, p, p]),
     "dirb200_stem_workspace_bytes": (C.c_size_t, [i32, i32, i32]),
     "dirb200_stem_pack_weight": (i32, [p, p]),
     "dirb200_stem_conv": (i32, [p, i32, i32, i32, p, p, p, p, p, p]),

@@ -95,6 +95,22 @@ def conv_c23(t1, w2_packed, scale2, shift2, w3_packed, scale3, shift3, res, vari
     return out
 
 
+def conv_c31(t2, w3_packed, scale3, shift3, x, w1_packed, scale1, shift1):
+    """Identity Bottleneck b's conv3 and block b+1's conv1 in one kernel: y = relu(bn3(conv1x1(t2)) + x),
+    t1 = relu(bn1(conv1x1(y))).  t2 NHWC fp16 (B,H,W,Cm), x (B,H,W,4Cm) -> (y, t1)."""
+    _chk(t2, torch.float16, "t2")
+    _chk(x, torch.float16, "x")
+    b, h, w, cm = t2.shape
+    assert tuple(x.shape) == (b, h, w, 4 * cm)
+    y = torch.empty_like(x)
+    t1 = torch.empty_like(t2)
+    lib.call("dirb200_conv_c31", _ptr(t2), b, h, w, cm, _ptr(_chk(w3_packed, torch.float16, "w3")),
+             _ptr(_chk(scale3, torch.float32, "scale3")), _ptr(_chk(shift3, torch.float32, "shift3")), _ptr(x), _ptr(y),
+             _ptr(_chk(w1_packed, torch.float16, "w1")), _ptr(_chk(scale1, torch.float32, "scale1")),
+             _ptr(_chk(shift1, torch.float32, "shift1")), _ptr(t1), _stream())
+    return y, t1
+
+
 def stem_conv(x_nchw, w_oihw, scale, shift):
     """Conv 7x7/s2/p3 (3->64) + BN + ReLU on tensor cores: NCHW fp32 (B,3,H,W) -> NHWC fp16 (B,Ho,Wo,64)."""
     _chk(x_nchw, torch.float32, "x_nchw")

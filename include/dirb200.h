@@ -184,6 +184,13 @@ int dirb200_conv_bn_act(const void* in_dev, int B, int H, int W, int Cin, const 
 int dirb200_conv_c23(const void* t1_dev, int B, int H, int W, int Cm, const void* w2_dev, const float* scale2_dev,
                      const float* shift2_dev, const void* w3_dev, const float* scale3_dev, const float* shift3_dev,
                      const void* res_dev, void* out_dev, int variant, void* stream);
+/* conv3 of an identity Bottleneck and conv1 of the identity Bottleneck after it in one kernel (resnet.py:75-85):
+ * y = relu(bn3(conv1x1(t2)) + x), t1 = relu(bn1(conv1x1(y))).  t2 NHWC fp16 (B,H,W,Cm), w3 [4*Cm][Cm] fp16, x / y NHWC
+ * fp16 (B,H,W,4*Cm), w1 [Cm][4*Cm] fp16 (the layouts of dirb200_conv_bn_act), t1 NHWC fp16 (B,H,W,Cm).  Cm in
+ * {64, 128, 256}.  conv1 reads y from shared memory; y and t1 equal the two dirb200_conv_bn_act launches bit for bit. */
+int dirb200_conv_c31(const void* t2_dev, int B, int H, int W, int Cm, const void* w3_dev, const float* scale3_dev,
+                     const float* shift3_dev, const void* x_dev, void* y_dev, const void* w1_dev, const float* scale1_dev,
+                     const float* shift1_dev, void* t1_dev, void* stream);
 /* The stem on tensor cores: Conv2d(3, 64, 7, stride 2, pad 3, bias=False) + folded BN + ReLU, resnet.py:115-118.
  * imgs_dev NCHW fp32 (B,3,H,W); w2_dev = the [64][256] fp16 weight layout produced (on the host) by
  * dirb200_stem_pack_weight from the OIHW fp32 [64][3][7][7] tensor; ws_dev scratch of
