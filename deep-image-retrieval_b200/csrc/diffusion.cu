@@ -633,21 +633,11 @@ int topk_cap(int k) { return static_cast<int>(ceil_div(k, SORT_RUN) * SORT_RUN);
 
 constexpr int RC_MAX_FLAGGED = 12000;       // the per-block histogram (nf + 1 counters) stays within 48 KB
 
-}  // namespace
-}  // namespace dirb
-
-using namespace dirb;
-
-extern "C" {
-
-size_t dirb200_diffusion_graph_workspace_bytes(int64_t N, int k) {
-  if (N < 1 || k < 1) return 0;
-  return graph_ws(nullptr, N, k).total;
-}
-
-int dirb200_diffusion_graph(const int64_t* nn_idx_dev, const double* nn_score_dev, int64_t N, int width, int k,
-                            double gamma, void* ws_dev, int64_t* row_ptr_dev, int* col_dev, double* val_dev,
-                            void* stream_) {
+// the graph launches of dirb200_diffusion_graph; a_dev / u_dev (both or neither) also receive A (val before
+// normalize_kernel, N * k capacity) and u
+int diffusion_graph(const int64_t* nn_idx_dev, const double* nn_score_dev, int64_t N, int width, int k, double gamma,
+                    void* ws_dev, int64_t* row_ptr_dev, int* col_dev, double* val_dev, double* a_dev, double* u_dev,
+                    void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DIRB_REQUIRE(N >= 1 && N < INT_MAX && k >= 1 && width >= 1 && width <= k + 1, DIRB200_EINVAL,
                "diffusion_graph: bad sizes N %lld, width %d, k %d", (long long)N, width, k);
@@ -667,10 +657,41 @@ int dirb200_diffusion_graph(const int64_t* nn_idx_dev, const double* nn_score_de
   scan_top_kernel<<<1, 1, 0, stream>>>(g.tiles, nt);
   scan_out_kernel<<<nt, SCAN_THREADS, 0, stream>>>(g.mcnt, N, g.tiles, row_ptr_dev);
   fill_kernel<<<wblocks, 256, 0, stream>>>(g.nbr, g.w, g.cnt, g.mutual, N, k, row_ptr_dev, col_dev, val_dev, g.u);
+  if (a_dev) {
+    DIRB_CUDA(cudaMemcpyAsync(a_dev, val_dev, size_t(N) * k * 8, cudaMemcpyDeviceToDevice, stream));
+    DIRB_CUDA(cudaMemcpyAsync(u_dev, g.u, size_t(N) * 8, cudaMemcpyDeviceToDevice, stream));
+  }
   normalize_kernel<<<wblocks, 256, 0, stream>>>(row_ptr_dev, col_dev, N, g.u, val_dev);
   count_launch(7);
   DIRB_CUDA(cudaGetLastError());
   return 0;
+}
+
+}  // namespace
+}  // namespace dirb
+
+using namespace dirb;
+
+extern "C" {
+
+size_t dirb200_diffusion_graph_workspace_bytes(int64_t N, int k) {
+  if (N < 1 || k < 1) return 0;
+  return graph_ws(nullptr, N, k).total;
+}
+
+int dirb200_diffusion_graph(const int64_t* nn_idx_dev, const double* nn_score_dev, int64_t N, int width, int k,
+                            double gamma, void* ws_dev, int64_t* row_ptr_dev, int* col_dev, double* val_dev,
+                            void* stream) {
+  return diffusion_graph(nn_idx_dev, nn_score_dev, N, width, k, gamma, ws_dev, row_ptr_dev, col_dev, val_dev, nullptr,
+                         nullptr, stream);
+}
+
+int dirb200_diffusion_graph_weights(const int64_t* nn_idx_dev, const double* nn_score_dev, int64_t N, int width, int k,
+                                    double gamma, void* ws_dev, int64_t* row_ptr_dev, int* col_dev, double* val_dev,
+                                    double* a_dev, double* u_dev, void* stream) {
+  DIRB_REQUIRE(a_dev && u_dev, DIRB200_EINVAL, "diffusion_graph_weights: null argument");
+  return diffusion_graph(nn_idx_dev, nn_score_dev, N, width, k, gamma, ws_dev, row_ptr_dev, col_dev, val_dev, a_dev,
+                         u_dev, stream);
 }
 
 int dirb200_diffusion_seeds(const int64_t* idx_dev, const double* score_dev, int Q, int kq, double gamma, int64_t N,

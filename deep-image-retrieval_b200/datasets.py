@@ -344,7 +344,7 @@ class ImageListRelevants(Dataset):
         flags = np.array([1 if int(r) in pos else 0 for r in rows], dtype=np.uint8)
         return rows, flags
 
-    def _ap_from_counts(self, q, rows, scores, above, mode):
+    def _ap_from_counts(self, q, rows, scores, above, mode, inside=None):
         rel = set(int(i) for i in self.get_relevants(q, mode))
         junk = set(int(i) for i in self.get_junk(q, mode))
         rel -= junk                                  # a label set to 0 (junk) after 1 wins, as in get_query_groundtruth
@@ -356,9 +356,22 @@ class ImageListRelevants(Dataset):
         ranks = []
         for p in rel:
             sp = scores[at[p]]
-            before = int(((js > sp) | ((js == sp) & (jidx < p))).sum()) if len(jidx) else 0   # junk rows ranked before p
+            if inside is None:
+                before = int(((js > sp) | ((js == sp) & (jidx < p))).sum()) if len(jidx) else 0   # junk rows ranked before p
+            else:                                                 # (inside R_q, value, index) order of truncation
+                ip = bool(inside[at[p]])
+                ji = np.array([bool(inside[at[int(j)]]) for j in jidx], dtype=bool)
+                before = int(((ji & (not ip)) | ((ji == ip) & ((js > sp) | ((js == sp) & (jidx < p))))).sum()) \
+                    if len(jidx) else 0
             ranks.append(int(above[at[p]]) - before)
         return compute_average_precision(np.sort(np.array(ranks, dtype=np.int64)))
+
+    def eval_query_AP_from_truncated_counts(self, query_idx, rows, inside, values, above):
+        """eval_query_AP_from_counts for truncated diffusion: the rows of R_q (inside) rank before all others, so a
+        junk row ranks before a positive by (inside, value, index) - f' inside R_q, the exact score outside."""
+        if self.relevants:
+            return self._ap_from_counts(query_idx, rows, values, above, "classic", inside)
+        return {m: self._ap_from_counts(query_idx, rows, values, above, m, inside) for m in ("easy", "medium", "hard")}
 
     def eval_query_AP_from_counts(self, query_idx, rows, scores, above):
         """AP of `eval_query_AP` from the exact scores of the labelled rows and, for each positive, the number of

@@ -119,6 +119,15 @@ SIGNATURES = {
     "dirb200_diffusion_rank_count": (i32, [p, i64, i32, p, p, p, p, i32, p, p, p, p]),
     "dirb200_diffusion_topk_workspace_bytes": (C.c_size_t, [i32, i32]),
     "dirb200_diffusion_topk": (i32, [p, i64, i32, i32, p, p, p, p]),
+    # truncated diffusion: each query on the subgraph of its own top-m rows, all CG iterations in one launch
+    "dirb200_diffusion_graph_weights": (i32, [p, p, i64, i32, i32, f64, p, p, p, p, p, p, p]),
+    "dirb200_diffusion_trunc_build_workspace_bytes": (C.c_size_t, [i32, i32]),
+    "dirb200_diffusion_trunc_build": (i32, [p, p, p, i64, i32, p, p, i32, i32, i32, f64, p, p, p, p, p, p, p, p, p]),
+    "dirb200_diffusion_trunc_solve_workspace_bytes": (C.c_size_t, [i32, i32]),
+    "dirb200_diffusion_trunc_solve": (i32, [p, p, p, i32, p, i32, i32, f64, i32, f64, p, p, p, p, p]),
+    "dirb200_diffusion_trunc_topk_workspace_bytes": (C.c_size_t, [i32, i32, i32]),
+    "dirb200_diffusion_trunc_topk": (i32, [p, p, i32, i32, p, p, i32, i32, p, p, p, p]),
+    "dirb200_diffusion_trunc_rank_count": (i32, [p, p, i32, i32, p, p, p, i32, p, p, p, p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

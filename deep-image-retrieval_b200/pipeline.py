@@ -402,6 +402,15 @@ def _aps_from_diffusion(db, qdescs, bdescs, params):
         offs.append(offs[-1] + len(r))
     rows = np.concatenate(rows) if rows else np.zeros(0, np.int64)
     flags = np.concatenate(flags) if flags else np.zeros(0, np.uint8)
+    if params.get("truncate") is not None:
+        # truncated diffusion: a junk row and a positive are ordered by (inside R_q, value, index), rule T6
+        d = Diffusion(bdescs, truncation=True, **build)
+        inside, sc, above = d.rank_counts_truncated(qdescs, np.array(offs, np.int64), rows, flags, params["truncate"],
+                                                    **solve)
+        inside, sc, above = inside.cpu().numpy(), sc.cpu().numpy(), above.cpu().numpy()
+        return [db.eval_query_AP_from_truncated_counts(q, rows[offs[q]:offs[q + 1]], inside[offs[q]:offs[q + 1]],
+                                                       sc[offs[q]:offs[q + 1]], above[offs[q]:offs[q + 1]])
+                for q in range(qdescs.shape[0])]
     sc, above = Diffusion(bdescs, **build).rank_counts(qdescs, np.array(offs, np.int64), rows, flags, **solve)
     sc, above = sc.cpu().numpy(), above.cpu().numpy()
     return [db.eval_query_AP_from_counts(q, rows[offs[q]:offs[q + 1]], sc[offs[q]:offs[q + 1]], above[offs[q]:offs[q + 1]])
@@ -422,10 +431,21 @@ def diffusion_params(values):
     return out
 
 
+def diffusion_truncate(value):
+    """--diffusion-truncate M -> the `truncate` entry of eval_model's `diffusion` dict (an integer >= 1; M >= KQ is
+    checked once the number of rows N is known, as min(M, N) >= KQ)."""
+    from .diffusion import check_truncate
+    try:
+        return check_truncate(value)
+    except (ValueError, OverflowError):
+        raise ValueError("--diffusion-truncate: M must be an integer >= 1 (got %r)" % (value,))
+
+
 def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=None, aqe=None, adba=None, threads=8,
                batch_size=16, save_feats=None, load_feats=None, dbg=(), rank_topk=0, dense_scores=False, diffusion=None):
     """Evaluate a network on a retrieval dataset (test_dir.py:97-180).  aqe / adba: dict(k=..., alpha=...).
-    diffusion (extension): dict of dirb200.diffusion parameters (k, kq, gamma, alpha, iters, tol); the rows are then
+    diffusion (extension): dict of dirb200.diffusion parameters (k, kq, gamma, alpha, iters, tol, and optionally
+    truncate = m: each query solved on the subgraph of its own m nearest rows); the rows are then
     ranked by diffusion over the database's mutual-kNN graph, after whitening and alpha-DBA / alpha-QE.  Only datasets
     with relevance lists are graded that way (NotImplementedError otherwise).
     Ranking: datasets with relevance lists (Oxford/Paris style) are graded from GPU rank counts and label datasets
@@ -671,9 +691,16 @@ def test_dir_main(argv=None):
     parser.add_argument("--diffusion", type=float, nargs="+", metavar="K KQ [GAMMA [ALPHA]]",
                         help="(extension) rank by diffusion over the mutual K-NN graph of the database, seeded by each "
                              "query's KQ nearest rows (defaults: gamma 3, alpha 0.99, 20 CG iterations)")
+    parser.add_argument("--diffusion-truncate", type=float, default=None, metavar="M",
+                        help="(extension, with --diffusion) truncated diffusion: solve each query on the subgraph of "
+                             "its own M nearest rows and rank the other rows after them in exact-score order")
     args = parser.parse_args(argv)
     try:
         diffusion = diffusion_params(args.diffusion) if args.diffusion is not None else None
+        if args.diffusion_truncate is not None:
+            if diffusion is None:
+                raise ValueError("--diffusion-truncate needs --diffusion")
+            diffusion["truncate"] = diffusion_truncate(args.diffusion_truncate)
     except ValueError as e:
         parser.error(str(e))
     args.iscuda = common.torch_set_gpu(args.gpu)

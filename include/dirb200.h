@@ -453,6 +453,49 @@ size_t dirb200_diffusion_topk_workspace_bytes(int Q, int k);
 int dirb200_diffusion_topk(const double* f_dev, int64_t N, int Q, int k, void* ws_dev, double* scores_dev,
                            int64_t* idx_dev, void* stream);
 
+/* Truncated diffusion (Iscen et al. 2017): each query solved on the subgraph of its own top-m rows R_q (DESIGN.md
+ * section 4.7, rules T1-T6).  Every query of a call has the same m (= min(m, N) rows); local row l of query q is the
+ * l-th row of R_q in ascending global index.  Per-query local matrices are stored ELL, column-major per query: entry e
+ * of local row l at [q][e][l], kw entries per row (kw >= the longest row of the global graph).
+ * dirb200_diffusion_graph_weights: dirb200_diffusion_graph (the same workspace, the same row_ptr / col / val bits),
+ * and also a_dev (capacity N * k) = A_ij, the values before normalisation, and u_dev [N] = u_i.
+ * dirb200_diffusion_trunc_build: from the exact lists list_idx_dev / list_score_dev [Q][m] (Index.search at depth m)
+ * and the global CSR of A: rows_dev [Q][m] int64 (R_q ascending), lcnt_dev [Q][m] (entries per local row),
+ * lcol_dev [Q][kw][m] int32 (local columns, ascending) and lval_dev [Q][kw][m] fp64 = S'_ij = A_ij * (u'_i * u'_j),
+ * d_dev / u_dev [Q][m] = d'_i (the row of A within R_q summed in ascending j) and u'_i = 1/sqrt(d'_i) (0 if d'_i = 0),
+ * y_dev [Q][m] = max(s, 0)^gamma at the first kq list entries, 0 elsewhere.  1 <= kq <= m <= N, gamma > 0.
+ * dirb200_diffusion_trunc_solve: (I - alpha S') f' = y' per query by conjugate gradient, all iterations in one launch,
+ * with the arithmetic and the reduction order of dirb200_diffusion_solve (with m = N it returns that call's f, iteration
+ * count and residual bit for bit).  Writes f_dev [Q][m], iters_dev [Q], resid_dev [Q]; the same arguments as
+ * dirb200_diffusion_solve otherwise.
+ * dirb200_diffusion_trunc_topk: the first k rows under rule T6: the m local rows by f' descending, ties -> lower row,
+ * -0 == +0, then (k > m) entries m .. k-1 of the exact lists list_idx_dev / list_score_dev [Q][list_width] (list_width
+ * >= k; unused when k <= m).  scores_dev [Q][k] = f' for the local rows, the exact score after them; idx_dev [Q][k].
+ * Q <= 65535 (else DIRB200_ENOTSUP).
+ * dirb200_diffusion_trunc_rank_count: for each target (device CSR offsets t_off_dev [Q+1], t_rows_dev, t_flags_dev):
+ * inside_dev = 1 when the row lies in R_q, value_dev = its f' (0 outside), above_dev = the rows of R_q ranking before
+ * it under rule T6 (flagged targets inside R_q; 0 otherwise).  A target outside R_q ranks after all of R_q, in exact
+ * score order: its rank count is dirb200_index_rank_count's. */
+int dirb200_diffusion_graph_weights(const int64_t* nn_idx_dev, const double* nn_score_dev, int64_t N, int width, int k,
+                                    double gamma, void* ws_dev, int64_t* row_ptr_dev, int* col_dev, double* val_dev,
+                                    double* a_dev, double* u_dev, void* stream);
+size_t dirb200_diffusion_trunc_build_workspace_bytes(int Q, int m);
+int dirb200_diffusion_trunc_build(const int64_t* row_ptr_dev, const int* col_dev, const double* a_dev, int64_t N,
+                                  int kw, const int64_t* list_idx_dev, const double* list_score_dev, int Q, int m,
+                                  int kq, double gamma, void* ws_dev, int64_t* rows_dev, int* lcnt_dev, int* lcol_dev,
+                                  double* lval_dev, double* d_dev, double* u_dev, double* y_dev, void* stream);
+size_t dirb200_diffusion_trunc_solve_workspace_bytes(int Q, int m);
+int dirb200_diffusion_trunc_solve(const int* lcnt_dev, const int* lcol_dev, const double* lval_dev, int kw,
+                                  const double* y_dev, int Q, int m, double alpha, int iters, double tol, void* ws_dev,
+                                  double* f_dev, int* iters_dev, double* resid_dev, void* stream);
+size_t dirb200_diffusion_trunc_topk_workspace_bytes(int Q, int m, int k);
+int dirb200_diffusion_trunc_topk(const int64_t* rows_dev, const double* f_dev, int Q, int m,
+                                 const int64_t* list_idx_dev, const double* list_score_dev, int list_width, int k,
+                                 void* ws_dev, double* scores_dev, int64_t* idx_dev, void* stream);
+int dirb200_diffusion_trunc_rank_count(const int64_t* rows_dev, const double* f_dev, int Q, int m,
+                                       const int* t_off_dev, const int64_t* t_rows_dev, const uint8_t* t_flags_dev,
+                                       int T, uint8_t* inside_dev, double* value_dev, int64_t* above_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
