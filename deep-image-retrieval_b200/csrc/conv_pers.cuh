@@ -29,7 +29,8 @@
 
 namespace dirb {
 
-enum { PERS_EPI_CONV = 0, PERS_EPI_SIM_DENSE = 1, PERS_EPI_SIM_FILTER = 2, PERS_EPI_SIM_GMAX = 3, PERS_EPI_F32 = 4 };
+enum { PERS_EPI_CONV = 0, PERS_EPI_SIM_DENSE = 1, PERS_EPI_SIM_FILTER = 2, PERS_EPI_SIM_GMAX = 3, PERS_EPI_F32 = 4,
+       PERS_EPI_SIM_JOIN = 5 };
 
 struct ConvPersParams {
   int a_spatial, taps, kw_taps, cin_blocks, stride, pad;
@@ -52,7 +53,7 @@ struct ConvPersParams {
   int M, N;                    // valid queries / database rows of this launch
   float* dense;                // [M][dense_ld] fp32 scores                     (PERS_EPI_SIM_DENSE)
   int64_t dense_ld;
-  const float* thr;            // [M] per-query threshold                       (PERS_EPI_SIM_FILTER)
+  const float* thr;            // [M] per-query threshold                       (PERS_EPI_SIM_FILTER / _JOIN)
   unsigned long long* cand;    // [M][cand_cap] packed (score bits << 32 | row)
   int* cand_cnt;               // [M]
   int cand_cap;
@@ -185,6 +186,35 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvPersParams& p, int t)
   return c;
 }
 
+// PERS_EPI_SIM_JOIN (self-join of a row block against itself and the rows after it): A rows and B rows start at the
+// same database row, a multiple of 128, so tile (m, n) with n < m lies wholly below the diagonal and is never launched.
+// The m_tiles x n_tiles grid (n_tiles >= m_tiles) keeps the tiles with n >= m, m fastest: column n < m_tiles holds
+// n + 1 tiles, every later column m_tiles, so the launch has T_m (T_m + 1) / 2 + (T_n - T_m) T_m tiles.
+__device__ __forceinline__ TileCoord decode_tile_tri(const ConvPersParams& p, int t) {
+  TileCoord c;
+  const int64_t mt = p.m_tiles;
+  const int64_t tri = mt * (mt + 1) / 2;
+  if (t < tri) {
+    int64_t n = static_cast<int64_t>((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+    while (n * (n + 1) / 2 > t) --n;
+    while ((n + 1) * (n + 2) / 2 <= t) ++n;
+    c.n_tile = static_cast<int>(n);
+    c.m_tile = static_cast<int>(t - n * (n + 1) / 2);
+  } else {
+    const int64_t u = t - tri;
+    c.n_tile = static_cast<int>(mt + u / mt);
+    c.m_tile = static_cast<int>(u % mt);
+  }
+  c.wo0 = c.ho0 = c.n0 = 0;
+  return c;
+}
+
+template <int EPI>
+__device__ __forceinline__ TileCoord decode_any_tile(const ConvPersParams& p, int t) {
+  if constexpr (EPI == PERS_EPI_SIM_JOIN) return decode_tile_tri(p, t);
+  else return decode_tile(p, t);
+}
+
 // Writes one accumulator pair (two adjacent columns of one row) of the similarity / whitening epilogues.
 __device__ __forceinline__ void store_dense_pair(const ConvPersParams& p, int64_t qi, int col, float v0, float v1) {
   float* dp = p.dense + qi * p.dense_ld + col;
@@ -284,7 +314,7 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       uint32_t g = 0;  // ring slot counter, runs across tiles
       uint32_t gp = 0;  // patch slot counter (HALO)
       for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
-        const TileCoord c = decode_tile(p, t);
+        const TileCoord c = decode_any_tile<EPI>(p, t);
         const bool kcm = RAGGED && !HALO && p.kc_major != nullptr &&
                          __ldg(p.kc_major + static_cast<int64_t>(c.n0) * p.ext_ld) != 0;
         if constexpr (HALO) {
@@ -364,7 +394,7 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint32_t g = 0, i = PP ? wg : 0, gp = 0;
   for (int t = blockIdx.x + (PP ? wg * static_cast<int>(gridDim.x) : 0); t < p.total_tiles;
        t += (PP ? 2 : 1) * gridDim.x, i += PP ? 2 : 1) {
-    const TileCoord c = decode_tile(p, t);
+    const TileCoord c = decode_any_tile<EPI>(p, t);
     const uint32_t jw = PP ? i >> 1 : i;             // tiles this warpgroup has finished: the residual barrier's phase
     // ragged batches: bit 2 * hf + h = this thread's row r0 + 64 * hf + 8 * h lies inside its image (decided before the
     // main loop, where the previous tile's accumulators are dead)
@@ -507,16 +537,18 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       for (int h = 0; h < 2; ++h) {
         const int64_t qi = static_cast<int64_t>(c.m_tile) * 128 + r0 + 8 * h;
         const bool valid = qi < p.M;
-        if (EPI == PERS_EPI_SIM_FILTER) {
+        if (EPI == PERS_EPI_SIM_FILTER || EPI == PERS_EPI_SIM_JOIN) {
           // every match of the row (score >= the query's threshold) is appended to its candidate list: the four threads
-          // holding a row reserve their slots with ONE atomicAdd and split them by a prefix sum over the quad
+          // holding a row reserve their slots with ONE atomicAdd and split them by a prefix sum over the quad.  The
+          // self-join keeps only the columns after the row (col > row: the pair (i, j) once, i < j, never (i, i)).
+          constexpr bool JOIN = EPI == PERS_EPI_SIM_JOIN;
           const float t_q = valid ? __ldg(p.thr + qi) : INFINITY;
           int cnt = 0;
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             const int col = c.n_tile * BN + j * 8 + 2 * t4;
-            cnt += (acc[0][4 * j + 2 * h] >= t_q && col < p.N) ? 1 : 0;
-            cnt += (acc[0][4 * j + 2 * h + 1] >= t_q && col + 1 < p.N) ? 1 : 0;
+            cnt += (acc[0][4 * j + 2 * h] >= t_q && col < p.N && (!JOIN || col > qi)) ? 1 : 0;
+            cnt += (acc[0][4 * j + 2 * h + 1] >= t_q && col + 1 < p.N && (!JOIN || col + 1 > qi)) ? 1 : 0;
           }
           int incl = cnt;
 #pragma unroll
@@ -537,7 +569,7 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               for (int e = 0; e < 2; ++e) {
                 const float v = acc[0][4 * j + 2 * h + e];
                 const int col = c.n_tile * BN + j * 8 + 2 * t4 + e;
-                if (v >= t_q && col < p.N) {
+                if (v >= t_q && col < p.N && (!JOIN || col > qi)) {
                   if (pos < p.cand_cap)
                     dst[pos] = (static_cast<unsigned long long>(__float_as_uint(v)) << 32) | static_cast<unsigned int>(col);
                   ++pos;

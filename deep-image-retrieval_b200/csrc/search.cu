@@ -31,6 +31,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -885,6 +886,53 @@ __global__ void merge_runs_kernel(const double* __restrict__ in_score, const int
   }
 }
 
+// ------------------------------------------------------------------------------------------------ range search / join
+// Candidates of rows q0 .. q0 + nq of a block, one warp per candidate: the exact score (exact_dot_warp, row of the block
+// first) and the database row, into the [nq][cap2] layout of sort_runs_merge.  Lists hold cnt[q] <= cap entries here.
+__global__ void join_rescore_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cnt, int cap,
+                                    int q0, const float* __restrict__ a32, const float* __restrict__ db32, int D,
+                                    int64_t col0, int cap2, int* __restrict__ rows, double* __restrict__ sc) {
+  const int q = blockIdx.y;
+  const int n = cnt[q0 + q];
+  const int wpb = blockDim.x >> 5, lane = threadIdx.x & 31;
+  const unsigned long long* c = cand + static_cast<int64_t>(q0 + q) * cap;
+  const float* a = a32 + static_cast<int64_t>(q0 + q) * D;
+  for (int w = blockIdx.x * wpb + (threadIdx.x >> 5); w < n; w += gridDim.x * wpb) {
+    const int64_t row = col0 + static_cast<int64_t>(c[w] & 0xffffffffu);
+    const double e = exact_dot_warp(a, db32 + row * D, D, lane);
+    if (lane == 0) {
+      rows[static_cast<int64_t>(q) * cap2 + w] = static_cast<int>(row);
+      sc[static_cast<int64_t>(q) * cap2 + w] = e;
+    }
+  }
+}
+
+// Per row of the sub-block: the ordered list (score desc) keeps its prefix with e >= tau.
+__global__ void join_kept_kernel(const double* __restrict__ out_sc, int K, const int* __restrict__ cnt, int q0, int nq,
+                                 double tau, int* __restrict__ kept) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= nq) return;
+  const double* s = out_sc + static_cast<int64_t>(q) * K;
+  int lo = 0, hi = cnt[q0 + q];
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (s[mid] >= tau) lo = mid + 1; else hi = mid;
+  }
+  kept[q] = lo;
+}
+
+// The kept prefixes -> the result CSR at off[q] (offsets of this sub-block, relative to res_*).
+__global__ void join_emit_kernel(const double* __restrict__ out_sc, const int64_t* __restrict__ out_ix, int K,
+                                 const int* __restrict__ kept, const int64_t* __restrict__ off, int64_t index_offset,
+                                 double* __restrict__ res_sc, int64_t* __restrict__ res_ix) {
+  const int q = blockIdx.y;
+  const int n = kept[q];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    res_sc[off[q] + i] = out_sc[static_cast<int64_t>(q) * K + i];
+    res_ix[off[q] + i] = out_ix[static_cast<int64_t>(q) * K + i] + index_offset;
+  }
+}
+
 }  // namespace
 
 static_assert(DEEP_RUN == SORT_RUN, "sort_runs_merge's run length is the deep finish's");
@@ -973,6 +1021,19 @@ struct dirb200_index {
     double* surv_sc = nullptr;
     int64_t* run_ix = nullptr;
   } pend;
+  // range search / self-join: workspace, options and the last result (CSR, kept until the next call)
+  int join_cap = 0;                // candidate capacity per row of the first filter pass (0 = min(columns, 4096))
+  void* jws = nullptr;             // filter pass: fp16 queries, thresholds, counts, candidate lists
+  size_t jws_bytes = 0;
+  void* jws2 = nullptr;            // re-scoring and sort buffers of a sub-block
+  size_t jws2_bytes = 0;
+  double* res_sc = nullptr;
+  int64_t* res_ix = nullptr;
+  size_t res_cap = 0;              // entries
+  std::vector<int64_t> res_off;    // host CSR offsets of the last result
+  int64_t join_stats[5] = {0, 0, 0, 0, 0};   // candidates, pairs, filter re-runs, filter launches, tiles
+  double join_ms[3] = {0, 0, 0};   // option profile: filter passes, exact re-scoring, sort + compaction
+  cudaEvent_t jev[4] = {};
   TmapCache tmaps;
   int profile = 0;                 // option "profile": time the phases of a search with CUDA events
   cudaEvent_t ev[10] = {};
@@ -1007,7 +1068,10 @@ static int sim_gemm(dirb200_index* h, int epi, const __half* q16, int Q, const _
     p.n_tiles = static_cast<int>(ceil_div(rows, BN));
     p.m_tiles = static_cast<int>(ceil_div(Q, 128));
     p.m_fastest = 1;
-    const int64_t total = static_cast<int64_t>(p.m_tiles) * p.n_tiles;
+    // the self-join launches the tiles on or above the diagonal only (decode_tile_tri)
+    const int64_t total = epi == PERS_EPI_SIM_JOIN
+                              ? static_cast<int64_t>(p.m_tiles) * p.n_tiles - static_cast<int64_t>(p.m_tiles) * (p.m_tiles - 1) / 2
+                              : static_cast<int64_t>(p.m_tiles) * p.n_tiles;
     DIRB_REQUIRE(total < (int64_t(1) << 31), DIRB200_ENOTSUP, "too many tiles");
     p.total_tiles = static_cast<int>(total);
     p.dense = a.dense; p.dense_ld = a.dense_ld;
@@ -1017,6 +1081,8 @@ static int sim_gemm(dirb200_index* h, int epi, const __half* q16, int Q, const _
       return conv_pers_launch<BN, 6, PERS_EPI_SIM_DENSE>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
     if (epi == PERS_EPI_SIM_GMAX)
       return conv_pers_launch<BN, 6, PERS_EPI_SIM_GMAX>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
+    if (epi == PERS_EPI_SIM_JOIN)
+      return conv_pers_launch<BN, 6, PERS_EPI_SIM_JOIN>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
     return conv_pers_launch<BN, 6, PERS_EPI_SIM_FILTER>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
   }
 }
@@ -1066,6 +1132,7 @@ int dirb200_index_set_option(dirb200_index* h, const char* key, double value) {
   else if (k == "retries") h->retries = std::max(0, std::min(4, static_cast<int>(value)));
   else if (k == "deferred_check") h->deferred = value != 0;
   else if (k == "ws_budget") h->ws_budget = std::max(0.0, value);
+  else if (k == "join_cap") h->join_cap = std::max(0, static_cast<int>(value));
   else DIRB_REQUIRE(false, DIRB200_EKEY, "unknown index option '%s'", key);
   return 0;
 }
@@ -1124,6 +1191,11 @@ int dirb200_index_destroy(dirb200_index* h) {
   for (auto e : h->ev) if (e) cudaEventDestroy(e);
   if (h->status_ev) cudaEventDestroy(h->status_ev);
   if (h->ws) cudaFree(h->ws);
+  for (auto e : h->jev) if (e) cudaEventDestroy(e);
+  if (h->jws) cudaFree(h->jws);
+  if (h->jws2) cudaFree(h->jws2);
+  if (h->res_sc) cudaFree(h->res_sc);
+  if (h->res_ix) cudaFree(h->res_ix);
   if (h->sel_own) cudaFree(h->sel_own);
   if (h->h_status) cudaFreeHost(h->h_status);
   delete h;
@@ -1625,6 +1697,307 @@ int dirb200_index_count_ge(dirb200_index* h, const float* q32, int Q, const int*
   h->stats[1] = st.band;
   h->stats[3] = st.fallback;
   h->stats[4] = launches_total() - launches0;
+  return 0;
+}
+
+// ---- range search and self-join (DESIGN.md section 4.8, rules J1-J6)
+// One block of rows (queries, or database rows i0 .. i0 + M of a self-join) against the database rows col0 .. N:
+//   1. filter pass: the fp16 tensor-core GEMM keeps every column with fp16-path score >= thr (PERS_EPI_SIM_FILTER, or
+//      PERS_EPI_SIM_JOIN over the tiles on or above the diagonal with col > row); its atomicAdd counts every match
+//      exactly, also past the list capacity.  The counts come back to the host (the one synchronisation of a block); a
+//      list that overflowed re-runs the block with capacity = its count, or the block is halved when that does not fit
+//      option ws_budget.
+//   2. exact re-scoring of the candidates (exact_dot_warp) and their order (score desc, row asc, sort_runs_merge), in
+//      sub-blocks of rows whose sort buffers fit the budget; the rows with e >= tau are a prefix of each ordered list.
+//   3. the prefixes are appended to the result CSR (second synchronisation, for their lengths).
+// thr = tau - eps16 rounded down to fp32: every row with e >= tau has fp16-path score >= thr (rule J5).
+namespace {
+
+float join_threshold(double tau, double eps16) {
+  const double x = tau - eps16;
+  float f = static_cast<float>(x);
+  if (static_cast<double>(f) > x) f = nextafterf(f, -INFINITY);
+  return f;
+}
+
+struct JoinRun {
+  dirb200_index* h;
+  const float* a32;        // rows of the block side (queries, or the database itself)
+  bool tri;                // self-join: the block's rows are database rows, columns start at the block's first row
+  double tau;
+  float thr;
+  cudaStream_t stream;
+};
+
+size_t join_filter_bytes(int M, int D, int cap, bool tri) {
+  const size_t m = static_cast<size_t>(M);
+  auto r = [](size_t b) { return (b + 255) / 256 * 256; };
+  return (tri ? 0 : r(m * D * 2)) + r(m * 4) + r(m * 4) + r(m * static_cast<size_t>(cap) * 8) + r(ST_WORDS * 8);
+}
+size_t join_sort_bytes(int nq, int K) {
+  const size_t m = static_cast<size_t>(nq);
+  const size_t cap2 = static_cast<size_t>(ceil_div(std::max(K, 1), DEEP_RUN) * DEEP_RUN);
+  auto r = [](size_t b) { return (b + 255) / 256 * 256; };
+  return r(m * cap2 * 4) + 2 * r(m * cap2 * 8) + 2 * r(m * static_cast<size_t>(std::max(K, 1)) * 8) + r(m * 4) + r(m * 8);
+}
+
+void join_mark(dirb200_index* h, int i, cudaStream_t stream) {
+  if (!h->profile) return;
+  if (!h->jev[i]) cudaEventCreate(&h->jev[i]);
+  cudaEventRecord(h->jev[i], stream);
+}
+void join_accumulate(dirb200_index* h, int i0, int i1, int slot) {
+  if (!h->profile) return;
+  float ms = 0;
+  if (cudaEventElapsedTime(&ms, h->jev[i0], h->jev[i1]) == cudaSuccess) h->join_ms[slot] += ms;
+}
+
+// Appends n more result entries, keeping the ones already there.
+int join_reserve(dirb200_index* h, int64_t used, int64_t add, cudaStream_t stream) {
+  const size_t need = static_cast<size_t>(used + add);
+  if (need <= h->res_cap) return 0;
+  const size_t cap = std::max(need, h->res_cap + h->res_cap / 2);
+  double* sc = nullptr;
+  int64_t* ix = nullptr;
+  DIRB_CUDA(cudaMalloc(reinterpret_cast<void**>(&sc), cap * 8));
+  DIRB_CUDA(cudaMalloc(reinterpret_cast<void**>(&ix), cap * 8));
+  if (used > 0) {
+    DIRB_CUDA(cudaMemcpyAsync(sc, h->res_sc, used * 8, cudaMemcpyDeviceToDevice, stream));
+    DIRB_CUDA(cudaMemcpyAsync(ix, h->res_ix, used * 8, cudaMemcpyDeviceToDevice, stream));
+    DIRB_CUDA(cudaStreamSynchronize(stream));
+  }
+  if (h->res_sc) DIRB_CUDA(cudaFree(h->res_sc));
+  if (h->res_ix) DIRB_CUDA(cudaFree(h->res_ix));
+  h->res_sc = sc;
+  h->res_ix = ix;
+  h->res_cap = cap;
+  return 0;
+}
+
+// Rows r0 .. r0 + M of the block side against columns col0 .. N; appends their lists to the result.
+int join_rows(const JoinRun& R, int64_t r0, int M, int64_t col0, int cap) {
+  dirb200_index* h = R.h;
+  const int D = h->dim;
+  const int64_t ncols = h->N - col0;
+  cudaStream_t stream = R.stream;
+  const float* a32 = R.a32 + r0 * D;
+  const auto budget = static_cast<size_t>(h->ws_budget);
+  // ---- 1. filter pass (+ one re-run at the exact capacity when a list overflowed)
+  std::vector<int> cnt_h(M);
+  int* cnt = nullptr;
+  unsigned long long* cand = nullptr;
+  unsigned long long* status = nullptr;
+  size_t used = 0;
+  for (int pass = 0;; ++pass) {
+    used = join_filter_bytes(M, D, cap, R.tri);
+    DIRB_TRY(grow_device(&h->jws, &h->jws_bytes, used));
+    uint8_t* w = static_cast<uint8_t*>(h->jws);
+    size_t off = 0;
+    auto carve = [&](size_t bytes) { uint8_t* p = w + off; off += (bytes + 255) / 256 * 256; return p; };
+    __half* a16 = R.tri ? const_cast<__half*>(h->db16) + r0 * D : reinterpret_cast<__half*>(carve(static_cast<size_t>(M) * D * 2));
+    float* thr = reinterpret_cast<float*>(carve(static_cast<size_t>(M) * 4));
+    cnt = reinterpret_cast<int*>(carve(static_cast<size_t>(M) * 4));
+    cand = reinterpret_cast<unsigned long long*>(carve(static_cast<size_t>(M) * cap * 8));
+    status = reinterpret_cast<unsigned long long*>(carve(ST_WORDS * 8));
+    join_mark(h, 0, stream);
+    if (R.tri) {
+      DIRB_CUDA(cudaMemsetAsync(cnt, 0, static_cast<size_t>(M) * 4, stream));
+    } else {
+      const int64_t n = static_cast<int64_t>(M) * D;
+      const int64_t threads = std::max<int64_t>(ceil_div(n, 4), std::max<int64_t>(M, 8));
+      search_prep_kernel<<<static_cast<unsigned>(ceil_div(threads, 256)), 256, 0, stream>>>(a32, a16, n, cnt, M, nullptr, 0, status);
+      count_launch();
+    }
+    fill_f32_kernel<<<static_cast<unsigned>(ceil_div(M, 256)), 256, 0, stream>>>(thr, M, R.thr);
+    count_launch();
+    SimArgs a;
+    a.thr = thr;
+    a.cand = cand;
+    a.cand_cnt = cnt;
+    a.cand_cap = cap;
+    DIRB_TRY(sim_gemm(h, R.tri ? PERS_EPI_SIM_JOIN : PERS_EPI_SIM_FILTER, a16, M, h->db16 + col0 * D, ncols, D, a, stream));
+    const int64_t mt = ceil_div(M, 128), nt = ceil_div(ncols, 128);
+    h->join_stats[3] += 1;
+    h->join_stats[4] += R.tri ? mt * nt - mt * (mt - 1) / 2 : mt * nt;
+    join_mark(h, 1, stream);
+    DIRB_CUDA(cudaMemcpyAsync(cnt_h.data(), cnt, static_cast<size_t>(M) * 4, cudaMemcpyDeviceToHost, stream));
+    DIRB_CUDA(cudaStreamSynchronize(stream));
+    join_accumulate(h, 0, 1, 0);
+    const int cmax = *std::max_element(cnt_h.begin(), cnt_h.end());
+    if (cmax <= cap) break;
+    // overflow: the counts are exact, so one re-run at capacity cmax captures every candidate (rule J6)
+    DIRB_REQUIRE(pass == 0, DIRB200_EOVERFLOW, "candidate count changed between two filter passes");
+    const int cap_new = static_cast<int>(std::min<int64_t>(ceil_div(cmax, 256) * 256, ncols));
+    if (join_filter_bytes(M, D, cap_new, R.tri) + join_sort_bytes(1, cmax) <= budget) {
+      cap = cap_new;
+      h->join_stats[2] += 1;
+      continue;
+    }
+    const int step = R.tri ? 128 : 1;           // a self-join block starts at a tile boundary
+    DIRB_REQUIRE(M > step, DIRB200_EOVERFLOW,
+                 "row %lld has %d candidates within eps16 of tau: %zu bytes of workspace needed, option ws_budget is %.0f",
+                 static_cast<long long>(r0), cmax, join_filter_bytes(1, D, cap_new, R.tri) + join_sort_bytes(1, cmax),
+                 h->ws_budget);
+    const int half = static_cast<int>(ceil_div(ceil_div(M, step), 2) * step);
+    h->join_stats[2] += 1;
+    DIRB_TRY(join_rows(R, r0, half, col0, cap));
+    return join_rows(R, r0 + half, M - half, R.tri ? col0 + half : col0, cap);
+  }
+  for (int q = 0; q < M; ++q) h->join_stats[0] += cnt_h[q];
+  // ---- 2./3. exact re-scoring, order, kept prefixes -> result, in sub-blocks of rows that fit the budget
+  const size_t sort_budget = budget > used ? budget - used : 0;
+  for (int q0 = 0; q0 < M;) {
+    int nq = 0, K = 0;
+    while (q0 + nq < M && nq < 65535) {
+      const int K2 = std::max(K, cnt_h[q0 + nq]);
+      if (nq > 0 && join_sort_bytes(nq + 1, K2) > sort_budget) break;
+      K = K2;
+      ++nq;
+    }
+    DIRB_REQUIRE(join_sort_bytes(nq, K) <= sort_budget || nq > 1, DIRB200_EOVERFLOW,
+                 "row %lld has %d candidates within eps16 of tau: %zu bytes of workspace needed, option ws_budget is %.0f",
+                 static_cast<long long>(r0 + q0), K, used + join_sort_bytes(1, K), h->ws_budget);
+    const int64_t base = h->res_off.back();
+    if (K == 0) {
+      for (int q = 0; q < nq; ++q) h->res_off.push_back(base);
+      q0 += nq;
+      continue;
+    }
+    const int cap2 = static_cast<int>(ceil_div(K, DEEP_RUN) * DEEP_RUN);
+    DIRB_TRY(grow_device(&h->jws2, &h->jws2_bytes, join_sort_bytes(nq, K)));
+    uint8_t* w = static_cast<uint8_t*>(h->jws2);
+    size_t off = 0;
+    auto carve = [&](size_t bytes) { uint8_t* p = w + off; off += (bytes + 255) / 256 * 256; return p; };
+    int* rows = reinterpret_cast<int*>(carve(static_cast<size_t>(nq) * cap2 * 4));
+    double* sc = reinterpret_cast<double*>(carve(static_cast<size_t>(nq) * cap2 * 8));
+    int64_t* run_ix = reinterpret_cast<int64_t*>(carve(static_cast<size_t>(nq) * cap2 * 8));
+    double* out_sc = reinterpret_cast<double*>(carve(static_cast<size_t>(nq) * K * 8));
+    int64_t* out_ix = reinterpret_cast<int64_t*>(carve(static_cast<size_t>(nq) * K * 8));
+    int* kept = reinterpret_cast<int*>(carve(static_cast<size_t>(nq) * 4));
+    int64_t* off_d = reinterpret_cast<int64_t*>(carve(static_cast<size_t>(nq) * 8));
+    join_mark(h, 1, stream);
+    const int64_t sms = num_sms();
+    const unsigned gr = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(32 * sms, nq), ceil_div(K, 8))));
+    join_rescore_kernel<<<dim3(gr, nq), 256, 0, stream>>>(cand, cnt, cap, q0, a32, h->db32, D, col0, cap2, rows, sc);
+    count_launch();
+    join_mark(h, 2, stream);
+    DIRB_TRY(sort_runs_merge(rows, cnt + q0, cap2, sc, run_ix, nq, K, status, out_sc, out_ix, stream));
+    join_kept_kernel<<<static_cast<unsigned>(ceil_div(nq, 256)), 256, 0, stream>>>(out_sc, K, cnt, q0, nq, R.tau, kept);
+    count_launch();
+    std::vector<int> kept_h(nq);
+    DIRB_CUDA(cudaMemcpyAsync(kept_h.data(), kept, static_cast<size_t>(nq) * 4, cudaMemcpyDeviceToHost, stream));
+    DIRB_CUDA(cudaStreamSynchronize(stream));
+    std::vector<int64_t> off_h(nq);
+    int64_t t = base;
+    int kmax = 0;
+    for (int q = 0; q < nq; ++q) {
+      off_h[q] = t - base;
+      t += kept_h[q];
+      kmax = std::max(kmax, kept_h[q]);
+      h->res_off.push_back(t);
+    }
+    if (t > base) {
+      DIRB_TRY(join_reserve(h, base, t - base, stream));
+      DIRB_CUDA(cudaMemcpyAsync(off_d, off_h.data(), static_cast<size_t>(nq) * 8, cudaMemcpyHostToDevice, stream));
+      const unsigned ge = static_cast<unsigned>(std::min<int64_t>(ceil_div(kmax, 256), 64));
+      join_emit_kernel<<<dim3(ge, nq), 256, 0, stream>>>(out_sc, out_ix, K, kept, off_d, h->offset, h->res_sc + base,
+                                                          h->res_ix + base);
+      count_launch();
+    }
+    join_mark(h, 3, stream);
+    DIRB_CUDA(cudaStreamSynchronize(stream));    // off_h / kept_h leave scope; the timing events are complete
+    join_accumulate(h, 1, 2, 1);
+    join_accumulate(h, 2, 3, 2);
+    DIRB_CUDA(cudaGetLastError());
+    q0 += nq;
+  }
+  return 0;
+}
+
+int join_begin(dirb200_index* h, double tau) {
+  DIRB_REQUIRE(h->has_db, DIRB200_ESTATE, "index has no database attached");
+  DIRB_REQUIRE(std::isfinite(tau), DIRB200_EINVAL, "tau must be finite");
+  DIRB_CUDA(cudaSetDevice(h->device));
+  DIRB_TRY(dirb200_index_check(h));
+  h->res_off.assign(1, 0);
+  for (auto& v : h->join_stats) v = 0;
+  for (auto& v : h->join_ms) v = 0;
+  return 0;
+}
+
+// Largest block of rows whose first filter pass fits half of option ws_budget (the rest is for the sort buffers), and
+// whose fp16 rows stay resident in L2 (16 MiB): in the m-fastest tile order every column tile meets all of the block's
+// row tiles, so a larger block re-reads its rows from HBM for each column tile and the GEMM becomes bandwidth-bound.
+int join_block_rows(const dirb200_index* h, int cap, bool tri) {
+  const int step = tri ? 128 : 1;
+  const int l2_rows = std::max(step, (16 << 20) / (2 * h->dim) / 128 * 128);
+  int lo = step, hi = std::min(65535 / step * step, l2_rows);
+  while (lo < hi) {
+    const int mid = (lo + hi + step) / 2 / step * step;
+    if (static_cast<double>(join_filter_bytes(mid, h->dim, cap, tri)) <= 0.5 * h->ws_budget) lo = mid; else hi = mid - step;
+  }
+  return lo;
+}
+
+int join_first_cap(const dirb200_index* h, int64_t ncols) {
+  if (h->join_cap > 0) return h->join_cap;
+  return static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(ncols, 4096)));
+}
+
+}  // namespace
+
+int dirb200_index_range_search(dirb200_index* h, const float* q32, int Q, double tau, int64_t* total_out, void* stream_) {
+  DIRB_REQUIRE(h && q32 && total_out && Q > 0, DIRB200_EINVAL, "bad arguments");
+  DIRB_TRY(join_begin(h, tau));
+  const JoinRun R{h, q32, false, tau, join_threshold(tau, h->eps16), static_cast<cudaStream_t>(stream_)};
+  if (h->N > 0) {
+    const int cap = join_first_cap(h, h->N);
+    const int qb = join_block_rows(h, cap, false);
+    for (int q0 = 0; q0 < Q; q0 += qb) DIRB_TRY(join_rows(R, q0, std::min(qb, Q - q0), 0, cap));
+  } else {
+    h->res_off.assign(static_cast<size_t>(Q) + 1, 0);
+  }
+  h->join_stats[1] = h->res_off.back();
+  *total_out = h->res_off.back();
+  return 0;
+}
+
+int dirb200_index_self_join(dirb200_index* h, int64_t row0, int64_t row1, double tau, int64_t* total_out, void* stream_) {
+  DIRB_REQUIRE(h && total_out, DIRB200_EINVAL, "bad arguments");
+  DIRB_TRY(join_begin(h, tau));
+  DIRB_REQUIRE(row0 >= 0 && row0 <= row1 && row1 <= h->N && row0 % 128 == 0, DIRB200_EINVAL,
+               "need 0 <= row0 <= row1 <= N with row0 a multiple of 128 (got %lld, %lld, N = %lld)",
+               static_cast<long long>(row0), static_cast<long long>(row1), static_cast<long long>(h->N));
+  const JoinRun R{h, h->db32, true, tau, join_threshold(tau, h->eps16), static_cast<cudaStream_t>(stream_)};
+  const int cap = join_first_cap(h, h->N - row0);
+  const int rb = join_block_rows(h, cap, true);
+  for (int64_t i0 = row0; i0 < row1; i0 += rb)
+    DIRB_TRY(join_rows(R, i0, static_cast<int>(std::min<int64_t>(rb, row1 - i0)), i0, cap));
+  h->join_stats[1] = h->res_off.back();
+  *total_out = h->res_off.back();
+  return 0;
+}
+
+int dirb200_index_join_fetch(dirb200_index* h, int64_t* off_dev, int64_t* idx_dev, double* scores_dev, void* stream_) {
+  DIRB_REQUIRE(h && off_dev, DIRB200_EINVAL, "null argument");
+  DIRB_REQUIRE(!h->res_off.empty(), DIRB200_ESTATE, "no range search or self-join result to fetch");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DIRB_CUDA(cudaSetDevice(h->device));
+  const int64_t total = h->res_off.back();
+  DIRB_CUDA(cudaMemcpyAsync(off_dev, h->res_off.data(), h->res_off.size() * 8, cudaMemcpyHostToDevice, stream));
+  if (total > 0) {
+    DIRB_REQUIRE(idx_dev && scores_dev, DIRB200_EINVAL, "null argument");
+    DIRB_CUDA(cudaMemcpyAsync(idx_dev, h->res_ix, total * 8, cudaMemcpyDeviceToDevice, stream));
+    DIRB_CUDA(cudaMemcpyAsync(scores_dev, h->res_sc, total * 8, cudaMemcpyDeviceToDevice, stream));
+  }
+  DIRB_CUDA(cudaStreamSynchronize(stream));    // the host offsets are the source of a copy
+  return 0;
+}
+
+int dirb200_index_join_stats(dirb200_index* h, int64_t stats[5], double ms[3]) {
+  DIRB_REQUIRE(h && stats && ms, DIRB200_EINVAL, "null argument");
+  for (int i = 0; i < 5; ++i) stats[i] = h->join_stats[i];
+  for (int i = 0; i < 3; ++i) ms[i] = h->join_ms[i];
   return 0;
 }
 

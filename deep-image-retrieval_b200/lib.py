@@ -128,6 +128,15 @@ SIGNATURES = {
     "dirb200_diffusion_trunc_topk_workspace_bytes": (C.c_size_t, [i32, i32, i32]),
     "dirb200_diffusion_trunc_topk": (i32, [p, p, i32, i32, p, p, i32, i32, p, p, p, p]),
     "dirb200_diffusion_trunc_rank_count": (i32, [p, p, i32, i32, p, p, p, i32, p, p, p, p]),
+    # range search, triangular self-join and the connected components of its pair graph
+    "dirb200_index_range_search": (i32, [p, p, i32, f64, C.POINTER(i64), p]),
+    "dirb200_index_self_join": (i32, [p, i64, i64, f64, C.POINTER(i64), p]),
+    "dirb200_index_join_fetch": (i32, [p, p, p, p, p]),
+    "dirb200_index_join_stats": (i32, [p, C.POINTER(i64), C.POINTER(f64)]),
+    "dirb200_join_components_workspace_bytes": (C.c_size_t, [i64]),
+    "dirb200_join_components": (i32, [p, p, i64, i64, p, p, p]),
+    "dirb200_join_groups_workspace_bytes": (C.c_size_t, [i64]),
+    "dirb200_join_groups": (i32, [p, i64, p, p, p, C.POINTER(i64), p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

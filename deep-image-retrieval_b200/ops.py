@@ -688,6 +688,53 @@ class Index:
                  _ptr(skip_row), _ptr(count), _stream())
         return count
 
+    def _join_result(self, rows, total):
+        off = torch.empty(rows + 1, dtype=torch.int64, device=self.db32.device)
+        idx = torch.empty(total, dtype=torch.int64, device=self.db32.device)
+        sc = torch.empty(total, dtype=torch.float64, device=self.db32.device)
+        lib.call("dirb200_index_join_fetch", self._h, _ptr(off), _ptr(idx), _ptr(sc), _stream())
+        return off, idx, sc
+
+    def range_search(self, q32: torch.Tensor, tau: float):
+        """Every row with exact score >= tau for each query (DESIGN.md section 4.8, rule J2) -> CSR (offsets int64 (Q+1,),
+        rows int64, scores fp64), each list ordered by (score desc, row asc); the same rows and score bits as the prefix
+        of search(q32, N) down to its last score >= tau.  Exact for any tau, however many rows match."""
+        _chk(q32, torch.float32, "q32")
+        total = C.c_int64()
+        lib.call("dirb200_index_range_search", self._h, _ptr(q32), q32.shape[0], float(tau), C.byref(total), _stream())
+        return self._join_result(q32.shape[0], total.value)
+
+    def self_join(self, tau: float, row_block: int = None):
+        """Every pair (i, j), i < j, of the index's rows with exact score >= tau (rule J3) -> CSR by i (offsets int64
+        (N+1,), partners j int64, scores fp64), partners ordered by (score desc, j asc): range_search(db, tau) without
+        the entries j <= i.  Only the tiles on or above the diagonal of X X^T run on the tensor cores.  row_block (a
+        multiple of 128): rows joined per call, whose results are concatenated (the result does not depend on it)."""
+        n = self.n
+        if row_block is not None and (int(row_block) <= 0 or int(row_block) % 128):
+            raise ValueError("row_block must be a positive multiple of 128 (got %r)" % (row_block,))
+        step = int(row_block) if row_block is not None else max(n, 1)
+        offs, idxs, scs = [], [], []
+        base = 0
+        for r0 in range(0, max(n, 1), step):
+            r1 = min(n, r0 + step)
+            total = C.c_int64()
+            lib.call("dirb200_index_self_join", self._h, r0, r1, float(tau), C.byref(total), _stream())
+            off, idx, sc = self._join_result(r1 - r0, total.value)
+            offs.append(off[:-1] + base if r1 < n else off + base)
+            idxs.append(idx)
+            scs.append(sc)
+            base += total.value
+        return torch.cat(offs), torch.cat(idxs), torch.cat(scs)
+
+    def join_stats(self):
+        """Counters (and, with option 'profile', CUDA-event milliseconds per stage) of the last range_search / self_join."""
+        st = (C.c_int64 * 5)()
+        ms = (C.c_double * 3)()
+        lib.call("dirb200_index_join_stats", self._h, st, ms)
+        out = dict(zip(["candidates", "pairs", "reruns", "filter_launches", "tiles"], [int(v) for v in st]))
+        out.update(zip(["filter_ms", "rescore_ms", "sort_ms"], [float(v) for v in ms]))
+        return out
+
     def check(self):
         """Collect the status of the last search (option deferred_check): raises DirbError on an unresolved overflow."""
         lib.call("dirb200_index_check", self._h)
@@ -716,3 +763,33 @@ class Index:
             self.close()
         except Exception:
             pass
+
+
+def join_components(off, cols, n):
+    """Connected components of the undirected graph of n rows given as a CSR (off int64 (n+1,), cols int64; CUDA
+    tensors) -> labels int64 (n,): the smallest row of each row's component (DESIGN.md section 4.8, rule J4)."""
+    n = int(n)
+    if n < 1:
+        return torch.empty(0, dtype=torch.int64, device=off.device)
+    _chk(off, torch.int64, "off")
+    _chk(cols, torch.int64, "cols")
+    if off.shape[0] != n + 1:
+        raise ValueError("off must have n + 1 entries")
+    labels = torch.empty(n, dtype=torch.int64, device=off.device)
+    ws = torch.empty(int(lib.raw("dirb200_join_components_workspace_bytes")(n)), dtype=torch.uint8, device=off.device)
+    lib.call("dirb200_join_components", _ptr(off), _ptr(cols), n, cols.shape[0], _ptr(ws), _ptr(labels), _stream())
+    return labels
+
+
+def join_groups(labels):
+    """Components of >= 2 rows by ascending label, members ascending -> (group offsets int64 (G+1,), members int64)."""
+    _chk(labels, torch.int64, "labels")
+    n = labels.shape[0]
+    if n < 1:
+        return torch.zeros(1, dtype=torch.int64, device=labels.device), labels.new_empty(0)
+    off = torch.empty(n // 2 + 1, dtype=torch.int64, device=labels.device)
+    members = torch.empty(n, dtype=torch.int64, device=labels.device)
+    ws = torch.empty(int(lib.raw("dirb200_join_groups_workspace_bytes")(n)), dtype=torch.uint8, device=labels.device)
+    counts = (C.c_int64 * 2)()
+    lib.call("dirb200_join_groups", _ptr(labels), n, _ptr(ws), _ptr(off), _ptr(members), counts, _stream())
+    return off[:counts[0] + 1].clone(), members[:counts[1]].clone()

@@ -496,6 +496,44 @@ int dirb200_diffusion_trunc_rank_count(const int64_t* rows_dev, const double* f_
                                        const int* t_off_dev, const int64_t* t_rows_dev, const uint8_t* t_flags_dev,
                                        int T, uint8_t* inside_dev, double* value_dev, int64_t* above_dev, void* stream);
 
+/* Range search and self-join (DESIGN.md section 4.8, rules J1-J6).  e(a, b) is the exact score of the search
+ * (fp64 accumulation of the fp32 products, the same bits as dirb200_index_search; e(a, b) == e(b, a)).  A row is a
+ * candidate when its fp16-path score reaches tau - eps16 (option "eps16", computed in fp64 and rounded down to fp32);
+ * candidates are re-scored exactly and kept when e >= tau.  The result (a CSR: offsets int64, rows int64 + the index
+ * offset, scores fp64, each list ordered by (e desc, row asc)) stays in the handle until the next call; its size goes to
+ * *total_out and dirb200_index_join_fetch copies it out.  A candidate list that overflows its capacity is detected from
+ * the exact match counts and re-run with enough capacity, or its block of rows is halved to fit option "ws_budget";
+ * the result does not depend on either.  What cannot fit the budget fails with DIRB200_EOVERFLOW, naming the count.
+ * Both calls synchronise the stream once per block of rows for the candidate counts and once per sort sub-block.
+ * Option "join_cap": candidate capacity per row of the first pass (0 = min(columns, 4096)).
+ * dirb200_index_range_search: for each query q32_dev[q] (Q >= 1) the rows with e(q, r) >= tau, no self-exclusion.
+ * dirb200_index_self_join: for the rows i of [row0, row1) (row0 a multiple of 128, row1 <= N) the rows j > i with
+ * e(x_i, x_j) >= tau; CSR by i - row0.  Only the 128 x 128 tiles on or above the diagonal run on the tensor cores.
+ * tau must be finite (DIRB200_EINVAL). */
+int dirb200_index_range_search(dirb200_index* idx, const float* q32_dev, int Q, double tau, int64_t* total_out,
+                               void* stream);
+int dirb200_index_self_join(dirb200_index* idx, int64_t row0, int64_t row1, double tau, int64_t* total_out,
+                            void* stream);
+/* Copies the last result: off_dev [rows + 1], idx_dev / scores_dev [total] (may be null when total is 0).
+ * Synchronises the stream. */
+int dirb200_index_join_fetch(dirb200_index* idx, int64_t* off_dev, int64_t* idx_dev, double* scores_dev, void* stream);
+/* Counters of the last range search / self-join: stats = {candidates, pairs, filter re-runs, filter launches, tensor-core
+ * tiles}; with option "profile" = 1, ms = CUDA-event milliseconds of {filter passes, exact re-scoring, sort +
+ * compaction}. */
+int dirb200_index_join_stats(dirb200_index* idx, int64_t stats[5], double ms[3]);
+/* Connected components of the undirected graph of n rows given as a CSR (row_ptr_dev [n+1], col_dev [nnz], both int64;
+ * each pair may appear once or in both directions): labels_dev [n] = the smallest row of each row's component (rule
+ * J4), the same on every run.  Synchronises the stream once per hooking round. */
+size_t dirb200_join_components_workspace_bytes(int64_t n);
+int dirb200_join_components(const int64_t* row_ptr_dev, const int64_t* col_dev, int64_t n, int64_t nnz, void* ws_dev,
+                            int64_t* labels_dev, void* stream);
+/* Groups = components of >= 2 rows, by ascending label, members ascending: group g holds
+ * members_dev[group_off_dev[g] .. group_off_dev[g+1]).  Capacities: group_off_dev n / 2 + 1, members_dev n.
+ * counts_out = {groups, members} (host).  Synchronises the stream. */
+size_t dirb200_join_groups_workspace_bytes(int64_t n);
+int dirb200_join_groups(const int64_t* labels_dev, int64_t n, void* ws_dev, int64_t* group_off_dev, int64_t* members_dev,
+                        int64_t counts_out[2], void* stream);
+
 #ifdef __cplusplus
 }
 #endif
