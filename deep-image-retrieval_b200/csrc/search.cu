@@ -1033,6 +1033,8 @@ struct dirb200_index {
   std::vector<int64_t> res_off;    // host CSR offsets of the last result
   int64_t join_stats[5] = {0, 0, 0, 0, 0};   // candidates, pairs, filter re-runs, filter launches, tiles
   double join_ms[3] = {0, 0, 0};   // option profile: filter passes, exact re-scoring, sort + compaction
+  int nearest_cap = 16;             // dirb200_index_nearest: most candidate groups before a row is re-scored in full
+  int64_t nearest_stats[3] = {0, 0, 0};   // rows with > 1 candidate group, rows re-scored in full, centres re-scored
   cudaEvent_t jev[4] = {};
   TmapCache tmaps;
   int profile = 0;                 // option "profile": time the phases of a search with CUDA events
@@ -1087,6 +1089,90 @@ static int sim_gemm(dirb200_index* h, int epi, const __half* q16, int Q, const _
   }
 }
 
+namespace dirb {
+namespace {
+// ------------------------------------------------------------------------------------------------ nearest row
+// dirb200_index_nearest (DESIGN.md section 4.9, rules K2 / K3), per block of queries:
+//   1. queries to fp16 (nearest_prep_kernel);
+//   2. one PERS_EPI_SIM_GMAX pass: G[q][g] = fp16-path maximum of the 32 rows 32g .. 32g + 31;
+//   3. nearest_kernel, one block per query: M = max_g G, t = M - 2 eps16 rounded down to fp32; the groups with G >= t
+//      hold every row whose exact score can be the best (its group reaches e* - eps16 >= M - 2 eps16), and are
+//      re-scored exactly (exact_dot_warp); more than nearest_cap such groups -> every row is re-scored.  The best
+//      (score desc, row asc) is the search's top-1.
+constexpr int NEAREST_THREADS = 256;
+constexpr int NEAREST_MAX_CAP = 256;
+
+__global__ void nearest_prep_kernel(const float* __restrict__ q32, __half* __restrict__ q16, int64_t n) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x)
+    q16[i] = __float2half_rn(q32[i]);
+}
+
+__device__ __forceinline__ bool nearest_better(double s, int64_t c, double bs, int64_t bc) {
+  return s > bs || (s == bs && c < bc);
+}
+
+__global__ void __launch_bounds__(NEAREST_THREADS) nearest_kernel(const float* __restrict__ G, int ng, const float* __restrict__ q32,
+                                                                  const float* __restrict__ db32, int64_t K, int D,
+                                                                  double eps16, int cap, int64_t offset,
+                                                                  int64_t* __restrict__ labels, double* __restrict__ scores,
+                                                                  unsigned long long* __restrict__ stats) {
+  __shared__ float red[NEAREST_THREADS / 32];
+  __shared__ int groups[NEAREST_MAX_CAP];
+  __shared__ int n_groups;
+  __shared__ double best_s[NEAREST_THREADS / 32];
+  __shared__ int64_t best_c[NEAREST_THREADS / 32];
+  const int q = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* g = G + static_cast<int64_t>(q) * ng;
+  float m = -INFINITY;
+  for (int j = threadIdx.x; j < ng; j += NEAREST_THREADS) m = fmaxf(m, g[j]);
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (lane == 0) red[warp] = m;
+  if (threadIdx.x == 0) n_groups = 0;
+  __syncthreads();
+  m = red[0];
+  for (int w = 1; w < NEAREST_THREADS / 32; ++w) m = fmaxf(m, red[w]);
+  const double x = static_cast<double>(m) - 2.0 * eps16;
+  float t = static_cast<float>(x);
+  if (static_cast<double>(t) > x) t = nextafterf(t, -INFINITY);
+  for (int j = threadIdx.x; j < ng; j += NEAREST_THREADS)
+    if (g[j] >= t) {
+      const int pos = atomicAdd(&n_groups, 1);
+      if (pos < cap) groups[pos] = j;
+    }
+  __syncthreads();
+  const int nc = n_groups;
+  const bool full = nc > cap;
+  const int64_t n_rows = full ? K : static_cast<int64_t>(nc) * 32;
+  const float* a = q32 + static_cast<int64_t>(q) * D;
+  double bs = -INFINITY;
+  int64_t bc = INT64_MAX;
+  unsigned long long scored = 0;
+  for (int64_t j = warp; j < n_rows; j += NEAREST_THREADS / 32) {
+    const int64_t c = full ? j : static_cast<int64_t>(groups[j >> 5]) * 32 + (j & 31);
+    if (c >= K) continue;                                      // uniform over the warp
+    const double e = exact_dot_warp(a, db32 + c * D, D, lane);
+    if (nearest_better(e, c, bs, bc)) { bs = e; bc = c; }
+    ++scored;
+  }
+  if (lane == 0) {
+    best_s[warp] = bs;
+    best_c[warp] = bc;
+    atomicAdd(stats + 2, scored);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < NEAREST_THREADS / 32; ++w)
+      if (nearest_better(best_s[w], best_c[w], bs, bc)) { bs = best_s[w]; bc = best_c[w]; }
+    labels[q] = offset + bc;
+    scores[q] = bs;
+    if (nc > 1) atomicAdd(stats, 1ull);
+    if (full) atomicAdd(stats + 1, 1ull);
+  }
+}
+
+}  // namespace
+}  // namespace dirb
+
 // Grow the search workspace to `need` bytes.  Cached query maps point into it, so they are dropped when it moves.
 static int grow_ws(dirb200_index* h, size_t need) {
   if (need > h->ws_bytes) h->tmaps.es.clear();
@@ -1133,6 +1219,7 @@ int dirb200_index_set_option(dirb200_index* h, const char* key, double value) {
   else if (k == "deferred_check") h->deferred = value != 0;
   else if (k == "ws_budget") h->ws_budget = std::max(0.0, value);
   else if (k == "join_cap") h->join_cap = std::max(0, static_cast<int>(value));
+  else if (k == "nearest_cap") h->nearest_cap = std::max(0, std::min(NEAREST_MAX_CAP, static_cast<int>(value)));
   else DIRB_REQUIRE(false, DIRB200_EKEY, "unknown index option '%s'", key);
   return 0;
 }
@@ -1998,6 +2085,57 @@ int dirb200_index_join_stats(dirb200_index* h, int64_t stats[5], double ms[3]) {
   DIRB_REQUIRE(h && stats && ms, DIRB200_EINVAL, "null argument");
   for (int i = 0; i < 5; ++i) stats[i] = h->join_stats[i];
   for (int i = 0; i < 3; ++i) ms[i] = h->join_ms[i];
+  return 0;
+}
+
+int dirb200_index_nearest(dirb200_index* h, const float* q32_dev, int Q, int64_t* labels_dev, double* scores_dev,
+                          void* stream_) {
+  DIRB_REQUIRE(h && h->has_db, DIRB200_EINVAL, "index has no database");
+  DIRB_REQUIRE(Q >= 0 && (Q == 0 || (q32_dev && labels_dev && scores_dev)), DIRB200_EINVAL, "bad arguments");
+  DIRB_REQUIRE(h->N >= 1, DIRB200_EINVAL, "the index is empty");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  for (int i = 0; i < 3; ++i) h->nearest_stats[i] = 0;
+  if (Q == 0) return 0;
+  const int D = h->dim;
+  const int64_t K = h->N;
+  const int ng = static_cast<int>(ceil_div(K, 32));
+  // per query: its fp16 row and its group maxima; the largest block within option ws_budget (at least 128 queries)
+  const size_t per_q = static_cast<size_t>(D) * 2 + static_cast<size_t>(ng) * 4;
+  const int64_t fit = static_cast<int64_t>(std::max(0.0, h->ws_budget - 4096.0) / static_cast<double>(per_q));
+  const int qb = static_cast<int>(std::min<int64_t>(Q, std::max<int64_t>(128, fit / 128 * 128)));
+  const size_t o_g = (static_cast<size_t>(qb) * D * 2 + 255) & ~size_t(255);
+  const size_t o_st = (o_g + static_cast<size_t>(qb) * ng * 4 + 255) & ~size_t(255);
+  DIRB_TRY(grow_ws(h, o_st + 64));
+  uint8_t* w = static_cast<uint8_t*>(h->ws);
+  __half* q16 = reinterpret_cast<__half*>(w);
+  float* G = reinterpret_cast<float*>(w + o_g);
+  unsigned long long* st = reinterpret_cast<unsigned long long*>(w + o_st);
+  DIRB_CUDA(cudaMemsetAsync(st, 0, 24, stream));
+  for (int q0 = 0; q0 < Q; q0 += qb) {
+    const int nq = std::min(qb, Q - q0);
+    const float* a = q32_dev + static_cast<int64_t>(q0) * D;
+    const int64_t n = static_cast<int64_t>(nq) * D;
+    nearest_prep_kernel<<<static_cast<unsigned>(std::min<int64_t>(ceil_div(n, 256), 65536)), 256, 0, stream>>>(a, q16, n);
+    count_launch();
+    SimArgs sa;
+    sa.dense = G;
+    sa.dense_ld = ng;
+    DIRB_TRY(sim_gemm(h, PERS_EPI_SIM_GMAX, q16, nq, h->db16, K, D, sa, stream));
+    nearest_kernel<<<nq, NEAREST_THREADS, 0, stream>>>(G, ng, a, h->db32, K, D, h->eps16, h->nearest_cap, h->offset,
+                                                       labels_dev + q0, scores_dev + q0, st);
+    count_launch();
+  }
+  unsigned long long hs[3];
+  DIRB_CUDA(cudaMemcpyAsync(hs, st, 24, cudaMemcpyDeviceToHost, stream));
+  DIRB_CUDA(cudaStreamSynchronize(stream));
+  DIRB_CUDA(cudaGetLastError());
+  for (int i = 0; i < 3; ++i) h->nearest_stats[i] = static_cast<int64_t>(hs[i]);
+  return 0;
+}
+
+int dirb200_index_nearest_stats(dirb200_index* h, int64_t stats[3]) {
+  DIRB_REQUIRE(h && stats, DIRB200_EINVAL, "null argument");
+  for (int i = 0; i < 3; ++i) stats[i] = h->nearest_stats[i];
   return 0;
 }
 

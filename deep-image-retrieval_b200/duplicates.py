@@ -145,11 +145,9 @@ def _load_set(path):
     raise ValueError("%s is neither a descriptor store nor an .npy file" % path)
 
 
-def parse_args(argv=None):
-    import argparse
-    p = argparse.ArgumentParser(description="Find near-duplicate descriptors (every pair with exact score >= T) and "
-                                            "their groups, or the overlap of two sets")
-    p.add_argument("--threshold", type=float, required=True, help="score threshold T (inclusive)")
+def add_input_args(p):
+    """The descriptor-set inputs shared by the command lines that read one set: an .npy, a store, or a dataset to extract
+    with a checkpoint and the usual extraction and whitening flags."""
     p.add_argument("--load-feats", type=str, default="", help=".npy of descriptors")
     p.add_argument("--store", type=str, default="", help="descriptor store")
     p.add_argument("--dataset", "-d", type=str, default="", help="command to load the dataset to extract")
@@ -162,6 +160,30 @@ def parse_args(argv=None):
     p.add_argument("--whitenv", type=int, default=None, help="number of components, default is None (all)")
     p.add_argument("--whitenm", type=float, default=1.0, help="whitening multiplier")
     p.add_argument("--threads", type=int, default=8, help="number of thread workers")
+
+
+def check_input_args(p, args):
+    if sum(bool(s) for s in (args.dataset, args.load_feats, args.store)) != 1:
+        p.error("exactly one of --dataset, --load-feats and --store is required")
+    if args.dataset and not args.checkpoint:
+        p.error("--dataset needs --checkpoint")
+
+
+def load_input(args):
+    """(dataset or None, descriptors) of the inputs add_input_args declares."""
+    if args.dataset:
+        return _extract(args)
+    if args.load_feats:
+        return None, _load_set(args.load_feats)
+    return None, DescriptorStore(args.store)
+
+
+def parse_args(argv=None):
+    import argparse
+    p = argparse.ArgumentParser(description="Find near-duplicate descriptors (every pair with exact score >= T) and "
+                                            "their groups, or the overlap of two sets")
+    p.add_argument("--threshold", type=float, required=True, help="score threshold T (inclusive)")
+    add_input_args(p)
     p.add_argument("--against", type=str, default="", help=".npy or store: report, for each row of the first set, "
                                                            "the rows of this set with score >= T")
     p.add_argument("--eps16", type=float, default=None, help="score error bound for rows that are not unit-norm")
@@ -169,10 +191,7 @@ def parse_args(argv=None):
     p.add_argument("--out-json", type=str, default="", help="json receiving the groups (image keys with --dataset)")
     p.add_argument("--gpu", type=int, default=0, help="GPU id")
     args = p.parse_args(argv)
-    if sum(bool(s) for s in (args.dataset, args.load_feats, args.store)) != 1:
-        p.error("exactly one of --dataset, --load-feats and --store is required")
-    if args.dataset and not args.checkpoint:
-        p.error("--dataset needs --checkpoint")
+    check_input_args(p, args)
     if not math.isfinite(args.threshold):
         p.error("--threshold must be finite")
     if args.eps16 is not None and not (math.isfinite(args.eps16) and args.eps16 > 0):
@@ -204,13 +223,7 @@ def find_duplicates_main(argv=None):
     groups (connected components), or with --against the rows of a second set that each row reaches."""
     args = parse_args(argv)
     torch.cuda.set_device(args.gpu)
-    dataset = None
-    if args.dataset:
-        dataset, X = _extract(args)
-    elif args.load_feats:
-        X = _load_set(args.load_feats)
-    else:
-        X = DescriptorStore(args.store)
+    dataset, X = load_input(args)
     if args.against:
         off, rows, scores = overlap(X, _load_set(args.against), args.threshold, eps16=args.eps16)
         pairs = pairs_from_csr(off, rows)

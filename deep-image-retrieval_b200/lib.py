@@ -137,6 +137,18 @@ SIGNATURES = {
     "dirb200_join_components": (i32, [p, p, i64, i64, p, p, p]),
     "dirb200_join_groups_workspace_bytes": (C.c_size_t, [i64]),
     "dirb200_join_groups": (i32, [p, i64, p, p, p, C.POINTER(i64), p]),
+    "dirb200_index_nearest": (i32, [p, p, i32, p, p, p]),
+    "dirb200_index_nearest_stats": (i32, [p, C.POINTER(i64)]),
+    # spherical k-means around the exact top-1 assignment: sizes + objective, empty-cluster relocation, centre update,
+    # k-means++ draws
+    "dirb200_kmeans_stats_workspace_bytes": (C.c_size_t, [i64, i32]),
+    "dirb200_kmeans_stats": (i32, [p, p, p, i64, i32, p, p, C.POINTER(i64), p]),
+    "dirb200_kmeans_relocate_workspace_bytes": (C.c_size_t, [i64]),
+    "dirb200_kmeans_relocate": (i32, [p, p, i64, i32, p, p, C.POINTER(i64), p]),
+    "dirb200_kmeans_update_workspace_bytes": (C.c_size_t, [i64, i32, i32]),
+    "dirb200_kmeans_update": (i32, [p, i64, i32, p, p, i32, p, p, C.POINTER(i64), p]),
+    "dirb200_kmeans_pp_workspace_bytes": (C.c_size_t, [i64, i32]),
+    "dirb200_kmeans_pp": (i32, [p, i64, i32, i64, p, i32, p, p, p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

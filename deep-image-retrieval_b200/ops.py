@@ -726,6 +726,26 @@ class Index:
             base += total.value
         return torch.cat(offs), torch.cat(idxs), torch.cat(scs)
 
+    def nearest(self, q32: torch.Tensor):
+        """Exact nearest row of each query (DESIGN.md section 4.9, rules K2 / K3) -> (labels int64 (Q,), scores fp64
+        (Q,)): the top-1 of search(q32, 1) bit for bit, from group maxima of the fp16 tensor-core pass and exact
+        re-scoring of the groups within 2 eps16 of the best (all rows past option 'nearest_cap' groups)."""
+        _chk(q32, torch.float32, "q32")
+        if q32.dim() != 2 or q32.shape[1] != self.dim:
+            raise ValueError("queries must be (Q, %d)" % self.dim)
+        nq = q32.shape[0]
+        labels = torch.empty(nq, dtype=torch.int64, device=q32.device)
+        scores = torch.empty(nq, dtype=torch.float64, device=q32.device)
+        lib.call("dirb200_index_nearest", self._h, _ptr(q32), nq, _ptr(labels), _ptr(scores), _stream())
+        return labels, scores
+
+    def nearest_stats(self):
+        """Counters of the last nearest(): band_rows (queries with more than one candidate group), full_rescores
+        (queries re-scored over all rows), rescored (rows re-scored in all)."""
+        st = (C.c_int64 * 3)()
+        lib.call("dirb200_index_nearest_stats", self._h, st)
+        return dict(zip(["band_rows", "full_rescores", "rescored"], [int(v) for v in st]))
+
     def join_stats(self):
         """Counters (and, with option 'profile', CUDA-event milliseconds per stage) of the last range_search / self_join."""
         st = (C.c_int64 * 5)()

@@ -534,6 +534,46 @@ size_t dirb200_join_groups_workspace_bytes(int64_t n);
 int dirb200_join_groups(const int64_t* labels_dev, int64_t n, void* ws_dev, int64_t* group_off_dev, int64_t* members_dev,
                         int64_t counts_out[2], void* stream);
 
+/* Exact nearest row for many queries (extension; DESIGN.md section 4.9, rules K2 / K3): for each query q32_dev[q]
+ * (Q >= 0) labels_dev[q] = the smallest row (+ the index offset) maximising the exact score, scores_dev[q] that score:
+ * the top-1 of dirb200_index_search bit for bit.  One PERS_EPI_SIM_GMAX pass gives the fp16-path maximum of each group
+ * of 32 rows; the groups within 2 eps16 (rounded down to fp32) of the largest are re-scored exactly, or every row when
+ * more than option "nearest_cap" (default 16, at most 256) groups qualify.  Query blocks fit option "ws_budget".
+ * Synchronises the stream.  dirb200_index_nearest_stats: {queries with more than one candidate group, queries
+ * re-scored over all rows, rows re-scored} of the last call. */
+int dirb200_index_nearest(dirb200_index* idx, const float* q32_dev, int Q, int64_t* labels_dev, double* scores_dev,
+                          void* stream);
+int dirb200_index_nearest_stats(dirb200_index* idx, int64_t stats[3]);
+/* Spherical k-means (extension; DESIGN.md section 4.9, rules K4-K7) on unit fp32 rows x32_dev [n][d] (d a multiple of
+ * 64, n < 2^29).  The assignment (rule K2) is dirb200_index_nearest of the rows against the centres.
+ * dirb200_kmeans_stats: counts_dev [k] = cluster sizes of labels_dev [n]; out = {labels that differ from prev_dev (n
+ * when prev_dev is null), sum of rint(scores_dev[i] * 2^32) (the objective in units of 2^-32, exact in any order),
+ * empty clusters}.  Synchronises the stream. */
+size_t dirb200_kmeans_stats_workspace_bytes(int64_t n, int k);
+int dirb200_kmeans_stats(const int64_t* labels_dev, const double* scores_dev, const int64_t* prev_dev, int64_t n, int k,
+                         void* ws_dev, int* counts_dev, int64_t out[3], void* stream);
+/* Rule K4, in place on labels_dev / counts_dev (the sizes dirb200_kmeans_stats returned): each empty cluster, in
+ * ascending order, takes the row of lowest (score, row) among the rows whose cluster still has >= 2 rows.  k <= n.
+ * *moves_out = rows moved.  Synchronises the stream. */
+size_t dirb200_kmeans_relocate_workspace_bytes(int64_t n);
+int dirb200_kmeans_relocate(int64_t* labels_dev, const double* scores_dev, int64_t n, int k, int* counts_dev,
+                            void* ws_dev, int64_t* moves_out, void* stream);
+/* Rule K5: centres_dev [k][d] = fl32(s_c / sqrt(||s_c||^2)), s_c the fp64 sum of cluster c's rows in ascending row
+ * order (counts_dev [k]: the cluster sizes of labels_dev, as dirb200_kmeans_stats / _relocate leave them), in chunks of 256 rows (each chunk summed sequentially, the chunk sums added in chunk order); ||s_c||^2 as
+ * DESIGN.md section 4.9 states.  A cluster with s_c = 0 (or no rows) keeps its centre; *zero_sums_out counts them.
+ * Synchronises the stream. */
+size_t dirb200_kmeans_update_workspace_bytes(int64_t n, int k, int d);
+int dirb200_kmeans_update(const float* x32_dev, int64_t n, int d, const int64_t* labels_dev, const int* counts_dev, int k,
+                          float* centres_dev, void* ws_dev, int64_t* zero_sums_out, void* stream);
+/* Rule K7, k-means++ by D^2 sampling: chosen_dev [k] = the rows drawn, chosen_dev[0] = first; draw j >= 1 uses
+ * u_host[j - 1] in [0, 1) (host, k - 1 values).  Weights w_i = max(0, 2 - 2 e(x_i, nearest chosen row)) in int64 units
+ * of 2^-32, 0 for chosen rows; with T their total, the drawn row is the first whose inclusive prefix exceeds
+ * min(floor(u * double(T)), T - 1).  When T = 0 (fewer than k distinct rows) that draw and all later ones are -1.
+ * Synchronises the stream once, at the end. */
+size_t dirb200_kmeans_pp_workspace_bytes(int64_t n, int k);
+int dirb200_kmeans_pp(const float* x32_dev, int64_t n, int d, int64_t first, const double* u_host, int k, void* ws_dev,
+                      int64_t* chosen_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
