@@ -30,7 +30,7 @@
 namespace dirb {
 
 enum { PERS_EPI_CONV = 0, PERS_EPI_SIM_DENSE = 1, PERS_EPI_SIM_FILTER = 2, PERS_EPI_SIM_GMAX = 3, PERS_EPI_F32 = 4,
-       PERS_EPI_SIM_JOIN = 5 };
+       PERS_EPI_SIM_JOIN = 5, PERS_EPI_SIM_LGMAX = 6, PERS_EPI_SIM_LFILTER = 7 };
 
 struct ConvPersParams {
   int a_spatial, taps, kw_taps, cin_blocks, stride, pad;
@@ -68,6 +68,14 @@ struct ConvPersParams {
   const int* ext;
   const int* kc_major;
   int ext_ld, ext_n, out_h, out_w;
+  // list epilogues (PERS_EPI_SIM_LGMAX / _LFILTER, the inverted-file search): tile t is entry t of a device-built table
+  // {A row, B row, column tile of the list, valid rows | valid columns << 16}.  A row s of the packed queries belongs to
+  // query slot_q[s]; B row b of the list-ordered database is database row perm[b].  LGMAX writes the maximum of group g
+  // of A row s's list to dense[gbase[s] + g]; LFILTER appends (score, perm[b]) to query slot_q[s]'s candidate list.
+  const int4* tiles;
+  const int* slot_q;
+  const int64_t* perm;
+  const int64_t* gbase;
 };
 
 // Whether accumulator row r of tile c lies inside its image's extent (ragged batches; true without an extent table).
@@ -164,6 +172,7 @@ constexpr int PERS_CONSUMER_THREADS = 256;
 
 struct TileCoord {
   int m_tile, n_tile, wo0, ho0, n0;
+  int a_row, b_row, m_valid, n_valid;   // list tiles only (decode_tile_list)
 };
 __device__ __forceinline__ TileCoord decode_tile(const ConvPersParams& p, int t) {
   TileCoord c;
@@ -209,9 +218,28 @@ __device__ __forceinline__ TileCoord decode_tile_tri(const ConvPersParams& p, in
   return c;
 }
 
+// PERS_EPI_SIM_LGMAX / _LFILTER: one table entry per tile; a tile never spans two lists (n_tile = its column tile within
+// the list), rows past m_valid are the zero padding of the list's query segment, columns past n_valid belong to the next
+// list or lie past the last row.
+template <int EPI>
+constexpr bool pers_list_epi() { return EPI == PERS_EPI_SIM_LGMAX || EPI == PERS_EPI_SIM_LFILTER; }
+__device__ __forceinline__ TileCoord decode_tile_list(const ConvPersParams& p, int t) {
+  TileCoord c;
+  const int4 e = __ldg(p.tiles + t);
+  c.a_row = e.x;
+  c.b_row = e.y;
+  c.m_tile = 0;
+  c.n_tile = e.z;
+  c.m_valid = e.w & 0xffff;
+  c.n_valid = e.w >> 16;
+  c.wo0 = c.ho0 = c.n0 = 0;
+  return c;
+}
+
 template <int EPI>
 __device__ __forceinline__ TileCoord decode_any_tile(const ConvPersParams& p, int t) {
   if constexpr (EPI == PERS_EPI_SIM_JOIN) return decode_tile_tri(p, t);
+  else if constexpr (pers_list_epi<EPI>()) return decode_tile_list(p, t);
   else return decode_tile(p, t);
 }
 
@@ -362,9 +390,9 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             tma_load_4d(sa, &tmA, &full_bar[s], kc * 64, c.wo0 * p.stride + kw - p.pad,
                         c.ho0 * p.stride + kh - p.pad, c.n0);
           } else {
-            tma_load_2d(sa, &tmA, &full_bar[s], it * 64, c.m_tile * 128);
+            tma_load_2d(sa, &tmA, &full_bar[s], it * 64, pers_list_epi<EPI>() ? c.a_row : c.m_tile * 128);
           }
-          tma_load_2d(sa + L::A_BYTES, &tmB, &full_bar[s], kb * 64, c.n_tile * BN);
+          tma_load_2d(sa + L::A_BYTES, &tmB, &full_bar[s], kb * 64, pers_list_epi<EPI>() ? c.b_row : c.n_tile * BN);
         }
       }
     }
@@ -593,6 +621,66 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
             m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
             if (t4 == 0 && valid && nb0 < p.N) p.dense[qi * p.dense_ld + (nb0 >> 5)] = m;
+          }
+        } else if (EPI == PERS_EPI_SIM_LFILTER) {
+          // the filter over a list tile: the same quad-level reservation, the query through slot_q, the row through perm
+          const int r = r0 + 8 * h;
+          const bool ok = r < c.m_valid;
+          const int q = ok ? __ldg(p.slot_q + c.a_row + r) : 0;
+          const float t_q = ok ? __ldg(p.thr + q) : INFINITY;
+          int cnt = 0;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = j * 8 + 2 * t4;
+            cnt += (acc[0][4 * j + 2 * h] >= t_q && col < c.n_valid) ? 1 : 0;
+            cnt += (acc[0][4 * j + 2 * h + 1] >= t_q && col + 1 < c.n_valid) ? 1 : 0;
+          }
+          int incl = cnt;
+#pragma unroll
+          for (int d = 1; d < 4; d <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, d, 4);
+            if (t4 >= d) incl += y;
+          }
+          const int total = __shfl_sync(0xffffffffu, incl, 3, 4);
+          int base = 0;
+          if (t4 == 0 && total > 0) base = atomicAdd(p.cand_cnt + q, total);
+          base = __shfl_sync(0xffffffffu, base, 0, 4);
+          if (cnt > 0) {
+            int pos = base + incl - cnt;
+            unsigned long long* dst = p.cand + static_cast<int64_t>(q) * p.cand_cap;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float v = acc[0][4 * j + 2 * h + e];
+                const int col = j * 8 + 2 * t4 + e;
+                if (v >= t_q && col < c.n_valid) {
+                  if (pos < p.cand_cap) {
+                    const unsigned int row = static_cast<unsigned int>(__ldg(p.perm + c.b_row + col));
+                    dst[pos] = (static_cast<unsigned long long>(__float_as_uint(v)) << 32) | row;
+                  }
+                  ++pos;
+                }
+              }
+            }
+          }
+        } else if (EPI == PERS_EPI_SIM_LGMAX) {
+          // group maxima of a list tile: groups of 32 list positions, numbered from the list's first row
+          const int r = r0 + 8 * h;
+          const bool ok = r < c.m_valid;
+          const int64_t gb = ok ? __ldg(p.gbase + c.a_row + r) + static_cast<int64_t>(c.n_tile) * (BN / 32) : 0;
+#pragma unroll
+          for (int gi = 0; gi < BN / 32; ++gi) {
+            float m = -INFINITY;
+#pragma unroll
+            for (int j = 4 * gi; j < 4 * gi + 4; ++j) {
+              const int col = j * 8 + 2 * t4;
+              m = (col < c.n_valid) ? fmaxf(m, acc[0][4 * j + 2 * h]) : m;
+              m = (col + 1 < c.n_valid) ? fmaxf(m, acc[0][4 * j + 2 * h + 1]) : m;
+            }
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+            if (t4 == 0 && ok && gi * 32 < c.n_valid) p.dense[gb + gi] = m;
           }
         } else if (valid) {                           // PERS_EPI_SIM_DENSE / PERS_EPI_F32
 #pragma unroll

@@ -1036,6 +1036,16 @@ struct dirb200_index {
   int nearest_cap = 16;             // dirb200_index_nearest: most candidate groups before a row is re-scored in full
   int64_t nearest_stats[3] = {0, 0, 0};   // rows with > 1 candidate group, rows re-scored in full, centres re-scored
   cudaEvent_t jev[4] = {};
+  // inverted lists (dirb200_index_set_lists): caller-owned fp16 rows in list order, list position -> row, K + 1 offsets
+  const __half* l16 = nullptr;
+  const int64_t* lperm = nullptr;
+  const int64_t* lcell_off = nullptr;
+  int lists_k = 0;
+  void* lws[2] = {nullptr, nullptr};   // list search: [0] pair counts and offsets, [1] tile table, packed queries, lists
+  size_t lws_bytes[2] = {0, 0};
+  int64_t lists_stats[6] = {0, 0, 0, 0, 0, 0};   // pairs, query rows issued, tiles, probed rows, candidates, re-runs
+  double lists_ms[4] = {0, 0, 0, 0};             // option profile: table build, GMAX pass + seed, FILTER pass, finish
+  cudaEvent_t lev[5] = {};
   TmapCache tmaps;
   int profile = 0;                 // option "profile": time the phases of a search with CUDA events
   cudaEvent_t ev[10] = {};
@@ -1202,6 +1212,10 @@ int dirb200_index_set_db(dirb200_index* h, const float* db32_dev, const void* db
   h->offset = index_offset;
   h->has_db = true;
   h->tmaps.es.clear();
+  h->l16 = nullptr;            // lists belong to the rows they were built from: a new database detaches them
+  h->lperm = nullptr;
+  h->lcell_off = nullptr;
+  h->lists_k = 0;
   return 0;
 }
 
@@ -1281,6 +1295,8 @@ int dirb200_index_destroy(dirb200_index* h) {
   for (auto e : h->jev) if (e) cudaEventDestroy(e);
   if (h->jws) cudaFree(h->jws);
   if (h->jws2) cudaFree(h->jws2);
+  for (auto e : h->lev) if (e) cudaEventDestroy(e);
+  for (void* b : h->lws) if (b) cudaFree(b);
   if (h->res_sc) cudaFree(h->res_sc);
   if (h->res_ix) cudaFree(h->res_ix);
   if (h->sel_own) cudaFree(h->sel_own);
@@ -2374,6 +2390,497 @@ int dirb200_aqe_expand(const float* q_dev, int Q, int D, const float* db32_dev, 
                                        n_rows, out_dev);
   count_launch();
   DIRB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ inverted lists
+// dirb200_index_search_lists (DESIGN.md section 4.10, rules I1-I6): the exact top-k of the union R(q) of the lists each
+// query probes, per block of queries:
+//   1. pairs (query, probed list) in (list asc, query asc) order without atomics: M[c][q] = probe rank + 1 of list c
+//      for query q, one block per list counts its pairs, one block scans the lists (query segments zero-padded to a
+//      multiple of 128 rows, tile offsets) and the queries (offsets of their group maxima); the totals come back to the
+//      host (one synchronisation per block: the grid of the persistent passes and the workspace need them);
+//   2. one block per list writes its slots (segment row -> query, first group maximum) and its tiles, m fastest
+//      (CTAs running together share the list tile), and the queries are packed into their segments in fp16;
+//   3. PERS_EPI_SIM_LGMAX over the tile table: the maximum of every group of 32 list rows of every pair; thr_q = k-th
+//      largest of q's group maxima (distinct rows) - 2 eps16, -inf with fewer than k groups;
+//   4. PERS_EPI_SIM_LFILTER over the same table into per-query candidate lists of (score, row); the counts come back to
+//      the host, and a block whose lists overflowed runs again at the exact count (or in halves, rule I6);
+//   5. the search's candidate selection and finish (search_finish_kernel / the deep finish) re-score against the fp32
+//      rows in row order, so the key is the exact search's.
+namespace dirb {
+namespace {
+constexpr int IVF_THREADS = 256;
+constexpr int IVF_SCAN = 1024;
+enum { LT_PAIRS = 0, LT_SLOTS = 1, LT_TILES = 2, LT_GROUPS = 3, LT_ROWS = 4, LT_ERR = 5, LT_MAXCNT = 6, LT_CAND = 7, LT_WORDS = 8 };
+
+__device__ __forceinline__ int64_t list_size(const int64_t* cell_off, int c) { return cell_off[c + 1] - cell_off[c]; }
+
+// Inclusive scan of one value per thread over a block of `nthreads` threads (a multiple of 32); *total = block sum.
+__device__ long long ivf_block_scan(long long v, long long* warp_sums, long long* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  long long incl = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const long long y = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += y;
+  }
+  if (lane == 31) warp_sums[warp] = incl;
+  __syncthreads();
+  long long before = 0, tot = 0;
+  for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) {
+    if (w < warp) before += warp_sums[w];
+    tot += warp_sums[w];
+  }
+  __syncthreads();
+  *total = tot;
+  return incl + before;
+}
+
+// M[c][q] = j + 1 for probe j of query q (M cleared before); a probe outside [0, K) or a list probed twice is an error.
+__global__ void ivf_mark_kernel(const int64_t* __restrict__ probes, int nq, int np, int K, int* __restrict__ M,
+                                long long* __restrict__ tot) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= static_cast<int64_t>(nq) * np) return;
+  const int q = static_cast<int>(i / np), j = static_cast<int>(i % np);
+  const int64_t c = probes[i];
+  if (c < 0 || c >= K) {
+    atomicOr(reinterpret_cast<unsigned long long*>(tot + LT_ERR), 1ull);
+    return;
+  }
+  if (atomicExch(M + c * nq + q, j + 1) != 0) atomicOr(reinterpret_cast<unsigned long long*>(tot + LT_ERR), 2ull);
+}
+
+// Per query: the offset of each probe's group maxima among the query's (probe order), their number, the probed rows.
+__global__ void ivf_query_groups_kernel(const int64_t* __restrict__ probes, int nq, int np, int K,
+                                        const int64_t* __restrict__ cell_off, int* __restrict__ loc,
+                                        long long* __restrict__ qgroups, long long* __restrict__ tot) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= nq) return;
+  long long g = 0, rows = 0;
+  for (int j = 0; j < np; ++j) {
+    const int64_t c = probes[static_cast<int64_t>(q) * np + j];
+    loc[static_cast<int64_t>(q) * np + j] = static_cast<int>(g);
+    if (c < 0 || c >= K) continue;
+    const int64_t n = list_size(cell_off, static_cast<int>(c));
+    g += (n + 31) / 32;
+    rows += n;
+  }
+  qgroups[q] = g;
+  atomicAdd(reinterpret_cast<unsigned long long*>(tot + LT_ROWS), static_cast<unsigned long long>(rows));
+}
+
+// One block per list: its number of probing queries.
+__global__ void __launch_bounds__(IVF_THREADS) ivf_list_count_kernel(const int* __restrict__ M, int nq, int* __restrict__ pc) {
+  __shared__ int red[IVF_THREADS / 32];
+  const int c = blockIdx.x;
+  int n = 0;
+  for (int q = threadIdx.x; q < nq; q += IVF_THREADS) n += M[static_cast<int64_t>(c) * nq + q] != 0;
+  for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = n;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < IVF_THREADS / 32; ++w) n += red[w];
+    pc[c] = n;
+  }
+}
+
+// One block: segment and tile offsets of the lists (lists without rows get neither), group offsets of the queries.
+__global__ void __launch_bounds__(IVF_SCAN) ivf_scan_kernel(const int* __restrict__ pc, const int64_t* __restrict__ cell_off, int K,
+                                                           const long long* __restrict__ qgroups, int nq,
+                                                           int64_t* __restrict__ seg_off, int64_t* __restrict__ tile_off,
+                                                           int64_t* __restrict__ qgoff, long long* __restrict__ tot) {
+  __shared__ long long ws[IVF_SCAN / 32];
+  long long cs = 0, ct = 0, cp = 0;
+  for (int base = 0; base < K; base += IVF_SCAN) {
+    const int c = base + threadIdx.x;
+    long long slots = 0, tiles = 0, pairs = 0;
+    if (c < K) {
+      const int64_t n = list_size(cell_off, c);
+      pairs = pc[c];
+      if (n > 0) {
+        slots = (pairs + 127) / 128 * 128;
+        tiles = slots / 128 * ((n + 127) / 128);
+      }
+    }
+    long long t1, t2, t3;
+    const long long is = ivf_block_scan(slots, ws, &t1);
+    const long long it = ivf_block_scan(tiles, ws, &t2);
+    ivf_block_scan(pairs, ws, &t3);
+    if (c < K) {
+      seg_off[c] = cs + is - slots;
+      tile_off[c] = ct + it - tiles;
+    }
+    cs += t1;
+    ct += t2;
+    cp += t3;
+  }
+  long long cg = 0;
+  for (int base = 0; base < nq; base += IVF_SCAN) {
+    const int q = base + threadIdx.x;
+    const long long v = q < nq ? qgroups[q] : 0;
+    long long t;
+    const long long incl = ivf_block_scan(v, ws, &t);
+    if (q < nq) qgoff[q] = cg + incl - v;
+    cg += t;
+  }
+  if (threadIdx.x == 0) {
+    seg_off[K] = cs;
+    tile_off[K] = ct;
+    qgoff[nq] = cg;
+    tot[LT_PAIRS] = cp;
+    tot[LT_SLOTS] = cs;
+    tot[LT_TILES] = ct;
+    tot[LT_GROUPS] = cg;
+  }
+}
+
+// One block per list with rows: its slots in ascending query order (a block-wide scan of M[c][*]), the zero padding of
+// its segment, and its tiles {A row, B row, column tile, valid rows | valid columns << 16}, m fastest.
+__global__ void __launch_bounds__(IVF_THREADS) ivf_list_fill_kernel(const int* __restrict__ M, int nq, int np,
+                                                                   const int* __restrict__ pc,
+                                                                   const int64_t* __restrict__ cell_off,
+                                                                   const int64_t* __restrict__ seg_off,
+                                                                   const int64_t* __restrict__ tile_off,
+                                                                   const int64_t* __restrict__ qgoff, const int* __restrict__ loc,
+                                                                   int* __restrict__ slot_q, int64_t* __restrict__ gbase,
+                                                                   int4* __restrict__ tiles) {
+  __shared__ long long ws[IVF_THREADS / 32];
+  const int c = blockIdx.x;
+  const int64_t n = list_size(cell_off, c);
+  const int pairs = pc[c];
+  if (n == 0 || pairs == 0) return;
+  const int64_t s0 = seg_off[c];
+  long long carry = 0;
+  for (int base = 0; base < nq; base += IVF_THREADS) {
+    const int q = base + threadIdx.x;
+    const int j1 = q < nq ? M[static_cast<int64_t>(c) * nq + q] : 0;
+    long long t;
+    const long long incl = ivf_block_scan(j1 != 0, ws, &t);
+    if (j1 != 0) {
+      const int64_t s = s0 + carry + incl - 1;
+      slot_q[s] = q;
+      gbase[s] = qgoff[q] + loc[static_cast<int64_t>(q) * np + j1 - 1];
+    }
+    carry += t;
+  }
+  const int slots = (pairs + 127) / 128 * 128;
+  for (int s = pairs + threadIdx.x; s < slots; s += IVF_THREADS) {
+    slot_q[s0 + s] = -1;
+    gbase[s0 + s] = 0;
+  }
+  const int mt = slots / 128;
+  const int nt = static_cast<int>((n + 127) / 128);
+  const int64_t t0 = tile_off[c];
+  for (int i = threadIdx.x; i < mt * nt; i += IVF_THREADS) {
+    const int m = i % mt, nn = i / mt;
+    const int mv = min(128, pairs - 128 * m);
+    const int64_t left = n - 128 * static_cast<int64_t>(nn);
+    const int nv = left < 128 ? static_cast<int>(left) : 128;
+    tiles[t0 + i] = make_int4(static_cast<int>(s0 + 128 * m), static_cast<int>(cell_off[c] + 128 * static_cast<int64_t>(nn)), nn,
+                              mv | (nv << 16));
+  }
+}
+
+// Packed fp16 queries: slot s holds query slot_q[s], padding slots zeros.  Candidate counters cleared.
+__global__ void ivf_pack_kernel(const float* __restrict__ q32, int D, const int* __restrict__ slot_q, int64_t slots,
+                                __half* __restrict__ q16, int* __restrict__ cnt, int nq) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  const int d4 = D / 4;
+  if (i < nq) cnt[i] = 0;
+  if (i >= slots * d4) return;
+  const int64_t s = i / d4;
+  const int d = static_cast<int>(i % d4) * 4;
+  const int q = slot_q[s];
+  uint2 o = make_uint2(0u, 0u);
+  if (q >= 0) {
+    const float4 v = *reinterpret_cast<const float4*>(q32 + static_cast<int64_t>(q) * D + d);
+    o.x = pack_h2(v.x, v.y);
+    o.y = pack_h2(v.z, v.w);
+  }
+  *reinterpret_cast<uint2*>(q16 + s * D + d) = o;
+}
+
+// thr[q] = (k-th largest of the query's group maxima) - band; fewer than k groups -> -inf.
+__global__ void __launch_bounds__(SEL_THREADS) ivf_seed_kernel(const float* __restrict__ G, const int64_t* __restrict__ qgoff,
+                                                               int k, float band, float* __restrict__ thr) {
+  __shared__ uint32_t hist[256];
+  __shared__ uint32_t bc[2];
+  const int q = blockIdx.x;
+  const int64_t g0 = qgoff[q];
+  const float t = block_kth_largest(DenseAcc{G + g0}, static_cast<int>(qgoff[q + 1] - g0), k, hist, bc);
+  if (threadIdx.x == 0) thr[q] = t - band;
+}
+
+// Largest candidate count (the exact size a re-run needs) and the candidates captured in all.
+__global__ void ivf_count_kernel(const int* __restrict__ cnt, int nq, long long* __restrict__ tot) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= nq) return;
+  atomicMax(tot + LT_MAXCNT, static_cast<long long>(cnt[q]));
+  atomicAdd(reinterpret_cast<unsigned long long*>(tot + LT_CAND), static_cast<unsigned long long>(cnt[q]));
+}
+}  // namespace
+}  // namespace dirb
+
+// One grouped pass of the persistent kernel over a device-built tile table (see above).
+static int list_gemm(dirb200_index* h, int epi, const __half* q16, int64_t slots, const int4* tiles, int64_t n_tiles,
+                     const int* slot_q, const int64_t* gbase, const SimArgs& a, cudaStream_t stream) {
+  constexpr int BN = 128;
+  const int D = h->dim;
+  DIRB_REQUIRE(n_tiles < (int64_t(1) << 31) && slots < (int64_t(1) << 31), DIRB200_ENOTSUP, "too many tiles");
+  const CUtensorMap* tm;
+  DIRB_TRY(h->tmaps.get(q16, D, slots, 128, &tm));
+  const CUtensorMap a_copy = *tm;
+  DIRB_TRY(h->tmaps.get(h->l16, D, h->N, BN, &tm));
+  const CUtensorMap b_copy = *tm;
+  ConvPersParams p{};
+  p.a_spatial = 0;
+  p.taps = 1; p.kw_taps = 1; p.cin_blocks = D / 64; p.stride = 1; p.pad = 0;
+  p.tw = 128; p.th = 1; p.nb = 1; p.tiles_w = 1; p.tiles_h = 1;
+  p.M = static_cast<int>(slots);
+  p.N = static_cast<int>(h->N);
+  p.total_tiles = static_cast<int>(n_tiles);
+  p.dense = a.dense;
+  p.thr = a.thr; p.cand = a.cand; p.cand_cnt = a.cand_cnt; p.cand_cap = a.cand_cap;
+  p.tiles = tiles; p.slot_q = slot_q; p.perm = h->lperm; p.gbase = gbase;
+  if (epi == PERS_EPI_SIM_LGMAX)
+    return conv_pers_launch<BN, 6, PERS_EPI_SIM_LGMAX>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
+  return conv_pers_launch<BN, 6, PERS_EPI_SIM_LFILTER>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
+}
+
+static void list_mark(dirb200_index* h, int i, cudaStream_t stream) {
+  if (!h->profile) return;
+  if (!h->lev[i]) cudaEventCreate(&h->lev[i]);
+  cudaEventRecord(h->lev[i], stream);
+}
+
+static int lists_grow(dirb200_index* h, int i, size_t need) {
+  if (need > h->lws_bytes[i]) h->tmaps.es.clear();   // cached query maps may point into the buffer that moves
+  return grow_device(&h->lws[i], &h->lws_bytes[i], need);
+}
+
+// One block of nq queries.  *split = 1: the block's workspace does not fit option ws_budget (nothing was written).
+static int lists_block(dirb200_index* h, const float* q32, int nq, int k, const int64_t* probes, int np, double* out_sc,
+                       int64_t* out_ix, cudaStream_t stream, int* split) {
+  const int K = h->lists_k, D = h->dim;
+  const int64_t N = h->N;
+  *split = 0;
+  auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
+  // ---- 1. pair counts and offsets
+  const size_t oM = 0, oLoc = oM + al(static_cast<size_t>(K) * nq * 4), oQg = oLoc + al(static_cast<size_t>(nq) * np * 4);
+  const size_t oPc = oQg + al(static_cast<size_t>(nq) * 8), oSeg = oPc + al(static_cast<size_t>(K) * 4);
+  const size_t oTo = oSeg + al(static_cast<size_t>(K + 1) * 8), oQgo = oTo + al(static_cast<size_t>(K + 1) * 8);
+  const size_t oTot = oQgo + al(static_cast<size_t>(nq + 1) * 8), bytesA = oTot + al(LT_WORDS * 8);
+  if (nq > 1 && static_cast<double>(bytesA) > h->ws_budget) { *split = 1; return 0; }
+  DIRB_TRY(lists_grow(h, 0, bytesA));
+  uint8_t* wa = static_cast<uint8_t*>(h->lws[0]);
+  int* M = reinterpret_cast<int*>(wa + oM);
+  int* loc = reinterpret_cast<int*>(wa + oLoc);
+  long long* qgroups = reinterpret_cast<long long*>(wa + oQg);
+  int* pc = reinterpret_cast<int*>(wa + oPc);
+  int64_t* seg_off = reinterpret_cast<int64_t*>(wa + oSeg);
+  int64_t* tile_off = reinterpret_cast<int64_t*>(wa + oTo);
+  int64_t* qgoff = reinterpret_cast<int64_t*>(wa + oQgo);
+  long long* tot = reinterpret_cast<long long*>(wa + oTot);
+  list_mark(h, 0, stream);
+  DIRB_CUDA(cudaMemsetAsync(M, 0, static_cast<size_t>(K) * nq * 4, stream));
+  DIRB_CUDA(cudaMemsetAsync(tot, 0, LT_WORDS * 8, stream));
+  const int64_t npairs = static_cast<int64_t>(nq) * np;
+  ivf_mark_kernel<<<static_cast<unsigned>(ceil_div(npairs, IVF_THREADS)), IVF_THREADS, 0, stream>>>(probes, nq, np, K, M, tot);
+  ivf_query_groups_kernel<<<static_cast<unsigned>(ceil_div(nq, IVF_THREADS)), IVF_THREADS, 0, stream>>>(
+      probes, nq, np, K, h->lcell_off, loc, qgroups, tot);
+  ivf_list_count_kernel<<<K, IVF_THREADS, 0, stream>>>(M, nq, pc);
+  ivf_scan_kernel<<<1, IVF_SCAN, 0, stream>>>(pc, h->lcell_off, K, qgroups, nq, seg_off, tile_off, qgoff, tot);
+  count_launch(4);
+  long long ht[LT_WORDS];
+  DIRB_CUDA(cudaMemcpyAsync(ht, tot, sizeof(ht), cudaMemcpyDeviceToHost, stream));
+  DIRB_CUDA(cudaStreamSynchronize(stream));
+  DIRB_CUDA(cudaGetLastError());
+  DIRB_REQUIRE((ht[LT_ERR] & 1) == 0, DIRB200_EINVAL, "a probe lies outside [0, %d)", K);
+  DIRB_REQUIRE((ht[LT_ERR] & 2) == 0, DIRB200_EINVAL, "a query probes the same list twice");
+  const int64_t slots = ht[LT_SLOTS], n_tiles = ht[LT_TILES], groups = ht[LT_GROUPS];
+  // ---- 2.-5. per candidate capacity: first the default, then (rule I6) the exact largest count
+  const SearchSizes z = search_sizes(h, k);
+  int cap = h->cand_cap > 0 ? h->cand_cap : z.cap;
+  const int cap2 = z.cap2;
+  const float band = static_cast<float>(2.0 * h->eps16);
+  for (int run = 0;; ++run) {
+    const size_t oQ16 = 0, oSq = al(static_cast<size_t>(slots) * D * 2), oGb = oSq + al(static_cast<size_t>(slots) * 4);
+    const size_t oTl = oGb + al(static_cast<size_t>(slots) * 8), oG = oTl + al(static_cast<size_t>(n_tiles) * 16);
+    const size_t oThr = oG + al(static_cast<size_t>(groups) * 4), oCnt = oThr + al(static_cast<size_t>(nq) * 4);
+    const size_t oCand = oCnt + al(static_cast<size_t>(nq) * 4), oKth = oCand + al(static_cast<size_t>(nq) * cap * 8);
+    const size_t oSel = oKth + al(static_cast<size_t>(nq) * 4), oGates = oSel + al(static_cast<size_t>(nq) * 4);
+    const size_t oSt = oGates + al(8 * 4), oSurv = oSt + al(ST_WORDS * 8);
+    size_t bytesB = oSurv;
+    const size_t surv_row = bytesB, surv_cnt = surv_row + al(static_cast<size_t>(nq) * cap2 * 4);
+    const size_t surv_sc = surv_cnt + al(static_cast<size_t>(nq) * 4), run_ix = surv_sc + al(static_cast<size_t>(nq) * cap2 * 8);
+    if (z.deep) bytesB = run_ix + al(static_cast<size_t>(nq) * cap2 * 8);
+    if (static_cast<double>(bytesA + bytesB) > h->ws_budget) {
+      if (nq > 1) { *split = 1; return 0; }
+      DIRB_REQUIRE(false, DIRB200_EOVERFLOW,
+                   "the list search of one query needs %.0f bytes (%d candidates) and option ws_budget is %.0f bytes",
+                   static_cast<double>(bytesA + bytesB), cap, h->ws_budget);
+    }
+    DIRB_TRY(lists_grow(h, 1, bytesB));
+    uint8_t* wb = static_cast<uint8_t*>(h->lws[1]);
+    __half* q16 = reinterpret_cast<__half*>(wb + oQ16);
+    int* slot_q = reinterpret_cast<int*>(wb + oSq);
+    int64_t* gbase = reinterpret_cast<int64_t*>(wb + oGb);
+    int4* tiles = reinterpret_cast<int4*>(wb + oTl);
+    float* G = reinterpret_cast<float*>(wb + oG);
+    float* thr = reinterpret_cast<float*>(wb + oThr);
+    int* cnt = reinterpret_cast<int*>(wb + oCnt);
+    unsigned long long* cand = reinterpret_cast<unsigned long long*>(wb + oCand);
+    float* kth_k = reinterpret_cast<float*>(wb + oKth);
+    float* sel = reinterpret_cast<float*>(wb + oSel);
+    int* gates = reinterpret_cast<int*>(wb + oGates);
+    unsigned long long* status = reinterpret_cast<unsigned long long*>(wb + oSt);
+    if (run > 0) list_mark(h, 0, stream);
+    ivf_list_fill_kernel<<<K, IVF_THREADS, 0, stream>>>(M, nq, np, pc, h->lcell_off, seg_off, tile_off, qgoff, loc, slot_q, gbase,
+                                                         tiles);
+    const int64_t packs = std::max<int64_t>(slots * (D / 4), nq);
+    ivf_pack_kernel<<<static_cast<unsigned>(ceil_div(packs, IVF_THREADS)), IVF_THREADS, 0, stream>>>(q32, D, slot_q, slots, q16, cnt,
+                                                                                                     nq);
+    DIRB_CUDA(cudaMemsetAsync(gates, 0, 8 * 4, stream));
+    DIRB_CUDA(cudaMemsetAsync(status, 0, ST_WORDS * 8, stream));
+    DIRB_CUDA(cudaMemsetAsync(tot + LT_MAXCNT, 0, 16, stream));
+    count_launch(2);
+    list_mark(h, 1, stream);
+    SimArgs a;
+    if (n_tiles > 0) {
+      a.dense = G;
+      DIRB_TRY(list_gemm(h, PERS_EPI_SIM_LGMAX, q16, slots, tiles, n_tiles, slot_q, gbase, a, stream));
+    }
+    ivf_seed_kernel<<<nq, SEL_THREADS, 0, stream>>>(G, qgoff, k, band, thr);
+    count_launch();
+    list_mark(h, 2, stream);
+    if (n_tiles > 0) {
+      a = SimArgs();
+      a.thr = thr;
+      a.cand = cand;
+      a.cand_cnt = cnt;
+      a.cand_cap = cap;
+      DIRB_TRY(list_gemm(h, PERS_EPI_SIM_LFILTER, q16, slots, tiles, n_tiles, slot_q, gbase, a, stream));
+    }
+    ivf_count_kernel<<<static_cast<unsigned>(ceil_div(nq, IVF_THREADS)), IVF_THREADS, 0, stream>>>(cnt, nq, tot);
+    count_launch();
+    DIRB_CUDA(cudaMemcpyAsync(ht + LT_MAXCNT, tot + LT_MAXCNT, 16, cudaMemcpyDeviceToHost, stream));
+    DIRB_CUDA(cudaStreamSynchronize(stream));
+    DIRB_CUDA(cudaGetLastError());
+    if (ht[LT_MAXCNT] > cap) {               // rule I6: run the block again with room for every match
+      DIRB_REQUIRE(ht[LT_MAXCNT] < (int64_t(1) << 30), DIRB200_EOVERFLOW, "%lld candidates for one query",
+                   static_cast<long long>(ht[LT_MAXCNT]));
+      cap = static_cast<int>((ht[LT_MAXCNT] + 255) / 256 * 256);
+      ++h->lists_stats[5];
+      continue;
+    }
+    cand_kth_kernel<<<nq, SEL_THREADS, 0, stream>>>(cand, cnt, cap, k, k, band, kth_k, sel, thr, N, nullptr, gates, 1, status);
+    count_launch();
+    list_mark(h, 3, stream);
+    auto& P = h->pend;
+    P = dirb200_index::Pending();
+    P.active = true;
+    P.Q = nq;
+    P.k = k;
+    P.cap = cap;
+    P.cap2 = cap2;
+    P.band = band;
+    P.cnt = cnt;
+    P.cand = cand;
+    P.status = status;
+    P.kth_k = kth_k;
+    P.sel_dev = sel;
+    P.launches0 = launches_total();
+    if (z.deep) {
+      P.surv_row = reinterpret_cast<int*>(wb + surv_row);
+      P.surv_cnt = reinterpret_cast<int*>(wb + surv_cnt);
+      P.surv_sc = reinterpret_cast<double*>(wb + surv_sc);
+      P.run_ix = reinterpret_cast<int64_t*>(wb + run_ix);
+    }
+    const int deferred = h->deferred;
+    h->deferred = 0;                          // the list search always collects its status
+    const int rc = search_finish_impl(h, q32, sel, out_sc, out_ix, stream, PeerX{}, nullptr);
+    h->deferred = deferred;
+    DIRB_TRY(rc);
+    list_mark(h, 4, stream);
+    h->lists_stats[0] += ht[LT_PAIRS];
+    h->lists_stats[1] += slots;
+    h->lists_stats[2] += n_tiles;
+    h->lists_stats[3] += ht[LT_ROWS];
+    h->lists_stats[4] += ht[LT_CAND];
+    if (h->profile) {
+      DIRB_CUDA(cudaEventSynchronize(h->lev[4]));
+      for (int i = 0; i < 4; ++i) {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, h->lev[i], h->lev[i + 1]);
+        h->lists_ms[i] += ms;
+      }
+    }
+    return 0;
+  }
+}
+
+extern "C" {
+
+int dirb200_index_set_lists(dirb200_index* h, const void* db16_lists_dev, const int64_t* perm_dev, const int64_t* cell_off_dev,
+                            int K, void* stream_) {
+  DIRB_REQUIRE(h && h->has_db, DIRB200_ESTATE, "index has no database attached");
+  DIRB_REQUIRE(K >= 0, DIRB200_EINVAL, "K must be >= 0");
+  h->tmaps.es.clear();
+  h->l16 = nullptr;
+  h->lperm = nullptr;
+  h->lcell_off = nullptr;
+  h->lists_k = 0;
+  if (K == 0) return 0;                       // detaches the lists
+  DIRB_REQUIRE(h->N >= 1 && db16_lists_dev && perm_dev && cell_off_dev, DIRB200_EINVAL, "bad list arguments");
+  DIRB_CUDA(cudaSetDevice(h->device));
+  std::vector<int64_t> off(static_cast<size_t>(K) + 1);
+  DIRB_CUDA(cudaMemcpyAsync(off.data(), cell_off_dev, off.size() * 8, cudaMemcpyDeviceToHost, static_cast<cudaStream_t>(stream_)));
+  DIRB_CUDA(cudaStreamSynchronize(static_cast<cudaStream_t>(stream_)));
+  DIRB_REQUIRE(off[0] == 0 && off[K] == h->N, DIRB200_EINVAL, "cell offsets must run from 0 to N = %lld",
+               static_cast<long long>(h->N));
+  for (int c = 0; c < K; ++c) DIRB_REQUIRE(off[c] <= off[c + 1], DIRB200_EINVAL, "cell offsets must not decrease (list %d)", c);
+  h->l16 = static_cast<const __half*>(db16_lists_dev);
+  h->lperm = perm_dev;
+  h->lcell_off = cell_off_dev;
+  h->lists_k = K;
+  return 0;
+}
+
+int dirb200_index_search_lists(dirb200_index* h, const float* q32_dev, int Q, int k, const int64_t* probes_dev, int nprobe,
+                               double* scores_dev, int64_t* idx_dev, void* stream_) {
+  DIRB_REQUIRE(h && h->lists_k > 0, DIRB200_ESTATE, "index has no lists attached (dirb200_index_set_lists)");
+  DIRB_REQUIRE(Q >= 0 && (Q == 0 || (q32_dev && probes_dev && scores_dev && idx_dev)), DIRB200_EINVAL, "bad arguments");
+  DIRB_REQUIRE(k >= 1 && k <= K_MAX, DIRB200_ENOTSUP, "need 0 < k <= %d (got %d)", K_MAX, k);
+  DIRB_REQUIRE(nprobe >= 1 && nprobe <= h->lists_k, DIRB200_EINVAL, "nprobe must be in [1, %d] (got %d)", h->lists_k, nprobe);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  for (auto& v : h->lists_stats) v = 0;
+  for (auto& v : h->lists_ms) v = 0;
+  if (Q == 0) return 0;
+  DIRB_CUDA(cudaSetDevice(h->device));
+  DIRB_TRY(dirb200_index_check(h));
+  // blocks start at the exact search's size and are halved while their workspace does not fit (rule I6)
+  int qb = std::min(Q, search_max_queries(h, k));
+  for (int q0 = 0; q0 < Q;) {
+    const int nb = std::min(qb, Q - q0);
+    int split = 0;
+    DIRB_TRY(lists_block(h, q32_dev + static_cast<int64_t>(q0) * h->dim, nb, k, probes_dev + static_cast<int64_t>(q0) * nprobe,
+                         nprobe, scores_dev + static_cast<int64_t>(q0) * k, idx_dev + static_cast<int64_t>(q0) * k, stream, &split));
+    if (split) {
+      qb = (nb + 1) / 2;
+      continue;
+    }
+    q0 += nb;
+  }
+  return 0;
+}
+
+int dirb200_index_lists_stats(dirb200_index* h, int64_t stats[6], double ms[4]) {
+  DIRB_REQUIRE(h && stats && ms, DIRB200_EINVAL, "null argument");
+  for (int i = 0; i < 6; ++i) stats[i] = h->lists_stats[i];
+  for (int i = 0; i < 4; ++i) ms[i] = h->lists_ms[i];
   return 0;
 }
 

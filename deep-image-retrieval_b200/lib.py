@@ -139,6 +139,9 @@ SIGNATURES = {
     "dirb200_join_groups": (i32, [p, i64, p, p, p, C.POINTER(i64), p]),
     "dirb200_index_nearest": (i32, [p, p, i32, p, p, p]),
     "dirb200_index_nearest_stats": (i32, [p, C.POINTER(i64)]),
+    "dirb200_index_set_lists": (i32, [p, p, p, p, i32, p]),
+    "dirb200_index_search_lists": (i32, [p, p, i32, i32, p, i32, p, p, p]),
+    "dirb200_index_lists_stats": (i32, [p, C.POINTER(i64), C.POINTER(f64)]),
     # spherical k-means around the exact top-1 assignment: sizes + objective, empty-cluster relocation, centre update,
     # k-means++ draws
     "dirb200_kmeans_stats_workspace_bytes": (C.c_size_t, [i64, i32]),

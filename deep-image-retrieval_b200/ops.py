@@ -746,6 +746,42 @@ class Index:
         lib.call("dirb200_index_nearest_stats", self._h, st)
         return dict(zip(["band_rows", "full_rescores", "rescored"], [int(v) for v in st]))
 
+    def set_lists(self, db16_lists, perm, cell_off):
+        """Attach inverted lists (DESIGN.md section 4.10, rule I2): db16_lists fp16 (N, D) = the rows in list order,
+        perm int64 (N,) = list position -> row, cell_off int64 (K + 1,) = list boundaries (CUDA tensors, kept alive
+        by the index).  Exact search, rank counts and the options keep working on the original-order rows."""
+        _chk(db16_lists, torch.float16, "db16_lists")
+        _chk(perm, torch.int64, "perm")
+        _chk(cell_off, torch.int64, "cell_off")
+        if tuple(db16_lists.shape) != (self.n, self.dim) or perm.shape[0] != self.n or cell_off.dim() != 1:
+            raise ValueError("lists must hold the index's %d rows of dimension %d" % (self.n, self.dim))
+        self._lists = (db16_lists, perm, cell_off)
+        lib.call("dirb200_index_set_lists", self._h, _ptr(db16_lists), _ptr(perm), _ptr(cell_off), cell_off.shape[0] - 1,
+                 _stream())
+
+    def search_lists(self, q32: torch.Tensor, k: int, probes: torch.Tensor):
+        """Exact top-k of the union of the lists each query probes (rules I3-I6) -> (scores fp64 (Q,k), idx int64 (Q,k)),
+        order score desc, row asc, tail (-inf, -1) when the union holds fewer than k rows.  probes int64 (Q, nprobe)."""
+        _chk(q32, torch.float32, "q32")
+        _chk(probes, torch.int64, "probes")
+        nq = q32.shape[0]
+        if probes.dim() != 2 or probes.shape[0] != nq:
+            raise ValueError("probes must be (Q, nprobe)")
+        scores = torch.empty((nq, k), dtype=torch.float64, device=q32.device)
+        idx = torch.empty((nq, k), dtype=torch.int64, device=q32.device)
+        lib.call("dirb200_index_search_lists", self._h, _ptr(q32), nq, int(k), _ptr(probes), probes.shape[1], _ptr(scores),
+                 _ptr(idx), _stream())
+        return scores, idx
+
+    def lists_stats(self):
+        """Counters (and, with option 'profile', CUDA-event milliseconds per stage) of the last search_lists."""
+        st = (C.c_int64 * 6)()
+        ms = (C.c_double * 4)()
+        lib.call("dirb200_index_lists_stats", self._h, st, ms)
+        out = dict(zip(["pairs", "query_rows", "tiles", "probed_rows", "candidates", "reruns"], [int(v) for v in st]))
+        out.update(zip(["build_ms", "gmax_ms", "filter_ms", "finish_ms"], [float(v) for v in ms]))
+        return out
+
     def join_stats(self):
         """Counters (and, with option 'profile', CUDA-event milliseconds per stage) of the last range_search / self_join."""
         st = (C.c_int64 * 5)()

@@ -417,6 +417,49 @@ def _aps_from_diffusion(db, qdescs, bdescs, params):
             for q in range(qdescs.shape[0])]
 
 
+def _aps_from_ivf(db, qdescs, bdescs, params):
+    """Per-query AP with inverted-file ranking (extension; DESIGN.md section 4.10, rule I7): the lists are k-means lists
+    of the database rows (IVFIndex.train), each query ranks the union R_q of its nprobe best lists first, in exact
+    order, then every other row in exact order; a junk row ranks before a positive by (inside R_q, score, index)."""
+    from .ivf import IVFIndex
+    dim = qdescs.shape[1]
+    pad = (-dim) % 64                   # zero columns keep the scores and the norms
+    f = lambda a: torch.nn.functional.pad(_dev_f32(a), (0, pad)).contiguous() if pad else _dev_f32(a)
+    qd, bd = f(qdescs), f(bdescs)
+    offs, rows, flags = [0], [], []
+    for q in range(qd.shape[0]):
+        r, fl = db.rank_targets(q)
+        rows.append(r)
+        flags.append(fl)
+        offs.append(offs[-1] + len(r))
+    rows = np.concatenate(rows) if rows else np.zeros(0, np.int64)
+    flags = np.concatenate(flags) if flags else np.zeros(0, np.uint8)
+    index = IVFIndex.train(bd, params["n_lists"], seed=params.get("seed", 0))
+    try:
+        inside, sc, rank = index.rank_counts(qd, np.array(offs, np.int64), rows, flags, params["nprobe"])
+    finally:
+        index.close()
+    inside, sc, rank = inside.cpu().numpy(), sc.cpu().numpy(), rank.cpu().numpy()
+    return [db.eval_query_AP_from_truncated_counts(q, rows[offs[q]:offs[q + 1]], inside[offs[q]:offs[q + 1]],
+                                                   sc[offs[q]:offs[q + 1]], rank[offs[q]:offs[q + 1]])
+            for q in range(qd.shape[0])]
+
+
+def ivf_params(values):
+    """--ivf NLIST NPROBE -> the eval_model `ivf` dict (integers, 1 <= NPROBE <= NLIST; NLIST <= N is checked by the
+    k-means fit)."""
+    if len(values) != 2:
+        raise ValueError("--ivf takes NLIST NPROBE (got %d values)" % len(values))
+    out = {}
+    for key, v in zip(("n_lists", "nprobe"), values):
+        if float(v) != int(v) or int(v) < 1:
+            raise ValueError("--ivf: %s must be an integer >= 1 (got %r)" % ("NLIST" if key == "n_lists" else "NPROBE", v))
+        out[key] = int(v)
+    if out["nprobe"] > out["n_lists"]:
+        raise ValueError("--ivf: NPROBE must not exceed NLIST (got %d > %d)" % (out["nprobe"], out["n_lists"]))
+    return dict(out, seed=0)
+
+
 def diffusion_params(values):
     """--diffusion K KQ [GAMMA [ALPHA]] -> the eval_model `diffusion` dict (the paper's defaults for what is not given)."""
     from .diffusion import DEFAULTS, check_params
@@ -442,12 +485,16 @@ def diffusion_truncate(value):
 
 
 def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=None, aqe=None, adba=None, threads=8,
-               batch_size=16, save_feats=None, load_feats=None, dbg=(), rank_topk=0, dense_scores=False, diffusion=None):
+               batch_size=16, save_feats=None, load_feats=None, dbg=(), rank_topk=0, dense_scores=False, diffusion=None,
+               ivf=None):
     """Evaluate a network on a retrieval dataset (test_dir.py:97-180).  aqe / adba: dict(k=..., alpha=...).
     diffusion (extension): dict of dirb200.diffusion parameters (k, kq, gamma, alpha, iters, tol, and optionally
     truncate = m: each query solved on the subgraph of its own m nearest rows); the rows are then
     ranked by diffusion over the database's mutual-kNN graph, after whitening and alpha-DBA / alpha-QE.  Only datasets
     with relevance lists are graded that way (NotImplementedError otherwise).
+    ivf (extension): dict(n_lists=..., nprobe=..., seed=0): inverted-file ranking (rule I7): k-means lists of the
+    database rows after whitening and alpha-DBA, queries probed after alpha-QE (whose own search stays exact); relevance
+    lists only (NotImplementedError otherwise), not together with diffusion (ValueError).
     Ranking: datasets with relevance lists (Oxford/Paris style) are graded from GPU rank counts and label datasets
     from GPU threshold counts + the exact top-100 - no Q x N score matrix, no host argsort; dense_scores=True
     (extension) forces the literal matmul + per-query sort of the reference; rank_topk > 0 (extension) grades
@@ -491,7 +538,15 @@ def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=Non
     tops = None
     qn, bn = _dev_f32(qdescs), _dev_f32(bdescs)
     unit = bool(float((qn.norm(dim=1) - 1).abs().max()) < 1e-3 and float((bn.norm(dim=1) - 1).abs().max()) < 1e-3)
-    if diffusion is not None:
+    if ivf is not None and diffusion is not None:
+        raise ValueError("ivf and diffusion are two rankings: choose one")
+    if ivf is not None:
+        if not hasattr(db, "eval_query_AP_from_truncated_counts"):
+            raise NotImplementedError("inverted-file ranking grades datasets with relevance lists (Oxford / Paris "
+                                      "style) only; %s has none" % type(db).__name__)
+        aps = _aps_from_ivf(db, qn, bn, ivf)
+        scores = None
+    elif diffusion is not None:
         if not hasattr(db, "eval_query_AP_from_counts"):
             raise NotImplementedError("diffusion re-ranking grades datasets with relevance lists (Oxford / Paris "
                                       "style) only; %s has none" % type(db).__name__)
@@ -694,8 +749,14 @@ def test_dir_main(argv=None):
     parser.add_argument("--diffusion-truncate", type=float, default=None, metavar="M",
                         help="(extension, with --diffusion) truncated diffusion: solve each query on the subgraph of "
                              "its own M nearest rows and rank the other rows after them in exact-score order")
+    parser.add_argument("--ivf", type=float, nargs="+", metavar="NLIST NPROBE",
+                        help="(extension) rank by an inverted file: k-means lists of the database (NLIST centres, "
+                             "k-means++ seed 0); each query's NPROBE best lists first, in exact order, then the other rows")
     args = parser.parse_args(argv)
     try:
+        if args.ivf is not None and args.diffusion is not None:
+            raise ValueError("--ivf and --diffusion are two rankings: choose one")
+        ivf = ivf_params(args.ivf) if args.ivf is not None else None
         diffusion = diffusion_params(args.diffusion) if args.diffusion is not None else None
         if args.diffusion_truncate is not None:
             if diffusion is None:
@@ -713,7 +774,7 @@ def test_dir_main(argv=None):
     res = eval_model(dataset, net, args.trfs, pooling=args.pooling, gemp=args.gemp, detailed=args.detailed,
                      threads=args.threads, dbg=args.dbg, whiten=whiten, aqe=aqe, adba=adba,
                      save_feats=args.save_feats, load_feats=args.load_feats, rank_topk=args.rank_topk,
-                     dense_scores=args.dense_scores, diffusion=diffusion)
+                     dense_scores=args.dense_scores, diffusion=diffusion, ivf=ivf)
     # (the reference's '%s = %g' line raises on the list-valued entries that --detailed adds; print scalars only)
     print(" * " + "\n * ".join(["%s = %g" % p for p in res.items() if isinstance(p[1], (int, float))]))
     if args.out_json:

@@ -544,6 +544,28 @@ int dirb200_join_groups(const int64_t* labels_dev, int64_t n, void* ws_dev, int6
 int dirb200_index_nearest(dirb200_index* idx, const float* q32_dev, int Q, int64_t* labels_dev, double* scores_dev,
                           void* stream);
 int dirb200_index_nearest_stats(dirb200_index* idx, int64_t stats[3]);
+/* Inverted-file search (extension; DESIGN.md section 4.10, rules I2-I6).  dirb200_index_set_lists attaches caller-owned
+ * list buffers to an index whose database is set: db16_lists_dev [N][dim] fp16 rows in list order (list ascending, then
+ * row ascending), perm_dev [N] int64 (list position -> row of the index), cell_off_dev [K + 1] int64 (list c holds
+ * positions cell_off[c] .. cell_off[c + 1] - 1; empty lists allowed).  The original-order db32 / db16 stay, so
+ * exact search and rank counts still work on the handle.  K = 0, or a later dirb200_index_set_db, detaches the lists.
+ * Synchronises the stream (the offsets are checked on the host).
+ * dirb200_index_search_lists: probes_dev [Q][nprobe] int64 (distinct lists in [0, K) per query, 1 <= nprobe <= K) ->
+ * the exact top-k of the union of each query's probed lists, scores_dev / idx_dev [Q][k] ordered by (score desc, row
+ * asc) with the scores and tail padding (-inf, -1) of dirb200_index_search (rule I4); with every list probed, that
+ * search bit for bit.  Grouped tensor-core passes over a device-built table of (list, query tile, row tile) tiles
+ * (rule I5), exact re-scoring and the search's finish; a query block whose candidate lists overflow runs again at the
+ * exact count or in halves within option "ws_budget", else DIRB200_EOVERFLOW (rule I6).  Options eps16, cand_cap,
+ * ws_budget and profile apply.  Synchronises the stream three times per query block (table sizes, candidate counts,
+ * status).
+ * dirb200_index_lists_stats: {pairs, query rows issued (padding included), tiles, probed rows (sum over queries of the
+ * union's size), candidates, re-runs} of the last call; with option "profile", ms = CUDA-event milliseconds of {table
+ * build, GMAX pass + seed, FILTER pass + selection, finish}. */
+int dirb200_index_set_lists(dirb200_index* idx, const void* db16_lists_dev, const int64_t* perm_dev,
+                            const int64_t* cell_off_dev, int K, void* stream);
+int dirb200_index_search_lists(dirb200_index* idx, const float* q32_dev, int Q, int k, const int64_t* probes_dev,
+                               int nprobe, double* scores_dev, int64_t* idx_dev, void* stream);
+int dirb200_index_lists_stats(dirb200_index* idx, int64_t stats[6], double ms[4]);
 /* Spherical k-means (extension; DESIGN.md section 4.9, rules K4-K7) on unit fp32 rows x32_dev [n][d] (d a multiple of
  * 64, n < 2^29).  The assignment (rule K2) is dirb200_index_nearest of the rows against the centres.
  * dirb200_kmeans_stats: counts_dev [k] = cluster sizes of labels_dev [n]; out = {labels that differ from prev_dev (n
