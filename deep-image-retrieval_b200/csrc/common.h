@@ -39,6 +39,21 @@ const char* last_error();
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// Typed sub-buffers of one workspace, handed out in order; each piece is rounded up to `align` bytes, so `used` is the
+// sum of the rounded pieces.  With a null base the pointers are null and only `used` counts: a layout function
+// X_ws(void* base, ...) gives both the buffer's size (base = nullptr) and its pointers.
+struct Carver {
+  char* base;
+  size_t align, used = 0;
+  explicit Carver(void* b, size_t a = 256) : base(static_cast<char*>(b)), align(a) {}
+  template <typename T>
+  T* take(size_t n) {
+    T* p = base ? reinterpret_cast<T*>(base + used) : nullptr;
+    used += (n * sizeof(T) + align - 1) / align * align;
+    return p;
+  }
+};
+
 // Grow the device buffer *p of *cap bytes to `need` bytes (contents are not kept; no-op when it is large enough).
 // Pointer and capacity are cleared before the allocation and the capacity is set only once it succeeded, so after a
 // failed call the buffer is empty rather than a null pointer with a stale capacity.
@@ -90,12 +105,23 @@ inline bool first_launch_on_device(std::atomic<uint64_t>& mask) {
 int require_sm90();
 
 // Sorted top-k of Q candidate lists (search.cu, the deep search's finish): list q holds min(cnt[q], cap2) pairs
-// (rows[q * cap2 + i], sc[q * cap2 + i]), cap2 a multiple of SORT_RUN.  Runs of SORT_RUN are sorted in shared memory
-// by (score desc, row asc) into sc / run_ix (the same layout), then merged by rank into out_score / out_idx [Q][k]
-// ((-inf, -1) past the end of a short list).  Q <= 65535.
+// (rows[q * cap2 + i], sc[q * cap2 + i]), cap2 = sort_run_cap(longest list).  Runs of SORT_RUN are sorted in shared
+// memory by (score desc, row asc) into sc / run_ix (the same layout), then merged by rank into out_score / out_idx
+// [Q][k] (row + row_offset; (-inf, -1) past the end of a short list).  Q <= 65535.
 constexpr int SORT_RUN = 2048;
+inline int sort_run_cap(int64_t n) { return static_cast<int>(ceil_div(n, SORT_RUN) * SORT_RUN); }
+struct SortScratch {
+  int* rows;
+  double* sc;
+  int64_t* run_ix;
+};
+inline SortScratch take_sort_scratch(Carver& c, int64_t Q, int cap2) {
+  const size_t n = static_cast<size_t>(Q) * cap2;
+  return {c.take<int>(n), c.take<double>(n), c.take<int64_t>(n)};
+}
 int sort_runs_merge(const int* rows, const int* cnt, int cap2, double* sc, int64_t* run_ix, int Q, int k,
-                    unsigned long long* status, double* out_score, int64_t* out_idx, cudaStream_t stream);
+                    int64_t row_offset, unsigned long long* status, double* out_score, int64_t* out_idx,
+                    cudaStream_t stream);
 
 // Launch counter (the "gpu_launches" the benchmark reports): every kernel launch of this library bumps it.
 void count_launch(int n = 1);

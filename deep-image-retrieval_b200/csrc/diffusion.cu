@@ -461,25 +461,22 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_out_kernel(const int64_t* _
     if (i0 + e < N) row_ptr[i0 + e + 1] = excl + v[e];
 }
 
-inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
-
 // graph workspace: nbr int32 [N][k], w fp64 [N][k], cnt int32 [N], mutual uint8 [N][k], mcnt int64 [N], u fp64 [N],
 // scan tile sums
 struct GraphWs {
   int* nbr; double* w; int* cnt; uint8_t* mutual; int64_t* mcnt; double* u; int64_t* tiles; size_t total;
 };
 GraphWs graph_ws(void* base, int64_t N, int k) {
-  GraphWs g{};
-  size_t o = 0;
-  auto take = [&](size_t b) { const size_t at = o; o += align256(b); return static_cast<char*>(base) + at; };
-  g.nbr = reinterpret_cast<int*>(take(size_t(N) * k * 4));
-  g.w = reinterpret_cast<double*>(take(size_t(N) * k * 8));
-  g.cnt = reinterpret_cast<int*>(take(size_t(N) * 4));
-  g.mutual = reinterpret_cast<uint8_t*>(take(size_t(N) * k));
-  g.mcnt = reinterpret_cast<int64_t*>(take(size_t(N) * 8));
-  g.u = reinterpret_cast<double*>(take(size_t(N) * 8));
-  g.tiles = reinterpret_cast<int64_t*>(take(size_t(ceil_div(N, SCAN_TILE)) * 8));
-  g.total = o;
+  Carver c(base);
+  GraphWs g;
+  g.nbr = c.take<int>(size_t(N) * k);
+  g.w = c.take<double>(size_t(N) * k);
+  g.cnt = c.take<int>(N);
+  g.mutual = c.take<uint8_t>(size_t(N) * k);
+  g.mcnt = c.take<int64_t>(N);
+  g.u = c.take<double>(N);
+  g.tiles = c.take<int64_t>(ceil_div(N, SCAN_TILE));
+  g.total = c.used;
   return g;
 }
 
@@ -487,35 +484,33 @@ int64_t cg_blocks(int64_t N) { return ceil_div(N, RB); }
 
 struct SolveWs { double *r, *p, *ap, *part; CgState s; size_t total; };
 SolveWs solve_ws(void* base, int64_t N, int Q) {
-  SolveWs w{};
-  size_t o = 0;
-  auto take = [&](size_t b) { const size_t at = o; o += align256(b); return static_cast<char*>(base) + at; };
-  const size_t nq = size_t(N) * Q * 8;
-  w.r = reinterpret_cast<double*>(take(nq));
-  w.p = reinterpret_cast<double*>(take(nq));
-  w.ap = reinterpret_cast<double*>(take(nq));
-  w.part = reinterpret_cast<double*>(take(size_t(cg_blocks(N)) * Q * 8));
-  w.s.yy = reinterpret_cast<double*>(take(size_t(Q) * 8));
-  w.s.rr = reinterpret_cast<double*>(take(size_t(Q) * 8));
-  w.s.al = reinterpret_cast<double*>(take(size_t(Q) * 8));
-  w.s.be = reinterpret_cast<double*>(take(size_t(Q) * 8));
-  w.s.act = reinterpret_cast<int*>(take(size_t(Q) * 4));
-  w.total = o;
+  Carver c(base);
+  SolveWs w;
+  const size_t nq = size_t(N) * Q;
+  w.r = c.take<double>(nq);
+  w.p = c.take<double>(nq);
+  w.ap = c.take<double>(nq);
+  w.part = c.take<double>(size_t(cg_blocks(N)) * Q);
+  w.s.yy = c.take<double>(Q);
+  w.s.rr = c.take<double>(Q);
+  w.s.al = c.take<double>(Q);
+  w.s.be = c.take<double>(Q);
+  w.s.act = c.take<int>(Q);
+  w.total = c.used;
   return w;
 }
 
 struct RankWs { uint64_t* skey; int64_t* srow; int* spos; int* nflag; unsigned long long* hist; size_t hist_bytes, total; };
 RankWs rank_ws(void* base, int Q, int T) {
-  RankWs w{};
-  size_t o = 0;
-  auto take = [&](size_t b) { const size_t at = o; o += align256(b); return static_cast<char*>(base) + at; };
-  w.skey = reinterpret_cast<uint64_t*>(take(size_t(T) * 8));
-  w.srow = reinterpret_cast<int64_t*>(take(size_t(T) * 8));
-  w.spos = reinterpret_cast<int*>(take(size_t(T) * 4));
-  w.nflag = reinterpret_cast<int*>(take(size_t(Q) * 4));
+  Carver c(base);
+  RankWs w;
+  w.skey = c.take<uint64_t>(T);
+  w.srow = c.take<int64_t>(T);
+  w.spos = c.take<int>(T);
+  w.nflag = c.take<int>(Q);
   w.hist_bytes = (size_t(T) + Q) * 8;
-  w.hist = reinterpret_cast<unsigned long long*>(take(w.hist_bytes));
-  w.total = o;
+  w.hist = c.take<unsigned long long>(size_t(T) + Q);
+  w.total = c.used;
   return w;
 }
 
@@ -599,23 +594,20 @@ __global__ void __launch_bounds__(TK_THREADS) tk_compact_kernel(const double* __
 }
 
 struct TopkWs {
-  unsigned long long* hist; uint64_t* kp; uint32_t* vp; long long* r; int* cnt; int* rows; double* sc; int64_t* run_ix;
+  unsigned long long* hist; uint64_t* kp; uint32_t* vp; long long* r; int* cnt; SortScratch s;
   unsigned long long* status; size_t total;
 };
 TopkWs topk_ws(void* base, int Q, int cap2) {
-  TopkWs w{};
-  size_t o = 0;
-  auto take = [&](size_t b) { const size_t at = o; o += align256(b); return static_cast<char*>(base) + at; };
-  w.hist = reinterpret_cast<unsigned long long*>(take(size_t(Q) * 256 * 8));
-  w.kp = reinterpret_cast<uint64_t*>(take(size_t(Q) * 8));
-  w.vp = reinterpret_cast<uint32_t*>(take(size_t(Q) * 4));
-  w.r = reinterpret_cast<long long*>(take(size_t(Q) * 8));
-  w.cnt = reinterpret_cast<int*>(take(size_t(Q) * 4));
-  w.rows = reinterpret_cast<int*>(take(size_t(Q) * cap2 * 4));
-  w.sc = reinterpret_cast<double*>(take(size_t(Q) * cap2 * 8));
-  w.run_ix = reinterpret_cast<int64_t*>(take(size_t(Q) * cap2 * 8));
-  w.status = reinterpret_cast<unsigned long long*>(take(8 * 8));
-  w.total = o;
+  Carver c(base);
+  TopkWs w;
+  w.hist = c.take<unsigned long long>(size_t(Q) * 256);
+  w.kp = c.take<uint64_t>(Q);
+  w.vp = c.take<uint32_t>(Q);
+  w.r = c.take<long long>(Q);
+  w.cnt = c.take<int>(Q);
+  w.s = take_sort_scratch(c, Q, cap2);
+  w.status = c.take<unsigned long long>(8);
+  w.total = c.used;
   return w;
 }
 
@@ -628,8 +620,6 @@ __global__ void tk_init_kernel(int Q, int k, uint64_t* __restrict__ kp, uint32_t
   r[q] = k;
   cnt[q] = 0;
 }
-
-int topk_cap(int k) { return static_cast<int>(ceil_div(k, SORT_RUN) * SORT_RUN); }
 
 constexpr int RC_MAX_FLAGGED = 12000;       // the per-block histogram (nf + 1 counters) stays within 48 KB
 
@@ -783,7 +773,7 @@ int dirb200_diffusion_rank_count(const double* f_dev, int64_t N, int Q, const in
 
 size_t dirb200_diffusion_topk_workspace_bytes(int Q, int k) {
   if (Q < 1 || k < 1) return 0;
-  return topk_ws(nullptr, Q, topk_cap(k)).total;
+  return topk_ws(nullptr, Q, sort_run_cap(k)).total;
 }
 
 int dirb200_diffusion_topk(const double* f_dev, int64_t N, int Q, int k, void* ws_dev, double* scores_dev,
@@ -794,7 +784,7 @@ int dirb200_diffusion_topk(const double* f_dev, int64_t N, int Q, int k, void* w
   DIRB_REQUIRE(Q <= 65535, DIRB200_ENOTSUP, "diffusion_topk: at most 65535 queries per call (got %d)", Q);
   DIRB_REQUIRE(f_dev && ws_dev && scores_dev && idx_dev, DIRB200_EINVAL, "diffusion_topk: null argument");
   DIRB_TRY(require_sm90());
-  const int cap2 = topk_cap(k);
+  const int cap2 = sort_run_cap(k);
   TopkWs w = topk_ws(ws_dev, Q, cap2);
   DIRB_CUDA(cudaMemsetAsync(w.hist, 0, size_t(Q) * 256 * 8, stream));
   tk_init_kernel<<<static_cast<unsigned>(ceil_div(Q, 128)), 128, 0, stream>>>(Q, k, w.kp, w.vp, w.r, w.cnt);
@@ -803,10 +793,10 @@ int dirb200_diffusion_topk(const double* f_dev, int64_t N, int Q, int k, void* w
     tk_hist_kernel<<<grid, TK_THREADS, 0, stream>>>(f_dev, N, Q, pass, w.kp, w.vp, w.hist);
     tk_pick_kernel<<<static_cast<unsigned>(ceil_div(Q, 128)), 128, 0, stream>>>(Q, pass, w.hist, w.kp, w.vp, w.r);
   }
-  tk_compact_kernel<<<grid, TK_THREADS, 0, stream>>>(f_dev, N, Q, w.kp, w.vp, cap2, w.cnt, w.rows, w.sc);
+  tk_compact_kernel<<<grid, TK_THREADS, 0, stream>>>(f_dev, N, Q, w.kp, w.vp, cap2, w.cnt, w.s.rows, w.s.sc);
   count_launch(26);
   DIRB_CUDA(cudaGetLastError());
-  return sort_runs_merge(w.rows, w.cnt, cap2, w.sc, w.run_ix, Q, k, w.status, scores_dev, idx_dev, stream);
+  return sort_runs_merge(w.s.rows, w.cnt, cap2, w.s.sc, w.s.run_ix, Q, k, 0, w.status, scores_dev, idx_dev, stream);
 }
 
 }  // extern "C"

@@ -33,7 +33,6 @@ constexpr int CG_WARPS = 8;
 constexpr int SMEM_OPT_IN = 227 * 1024;     // dynamic shared memory a block of an H100 may opt into
 constexpr int KEY_SMEM_MAX = 128 * 1024;    // sort keys of R_q in shared memory up to 16384 rows
 
-inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
 int pow2_at_least(int m) { int P = 1; while (P < m) P <<= 1; return P; }
 bool keys_in_smem(int m) { return size_t(pow2_at_least(m)) * 8 <= size_t(KEY_SMEM_MAX); }
 size_t cg_smem_bytes(int m) { return size_t(m) * 4 * 8; }
@@ -309,29 +308,24 @@ __global__ void __launch_bounds__(256) trunc_rank_kernel(const int64_t* __restri
 // ------------------------------------------------------------------------------------------------ workspaces
 struct BuildWs { uint64_t* keys; size_t total; };
 BuildWs build_ws(void* base, int Q, int m) {
-  BuildWs w{};
-  w.keys = static_cast<uint64_t*>(base);
-  w.total = keys_in_smem(m) ? 256 : align256(size_t(Q) * pow2_at_least(m) * 8);
+  Carver c(base);
+  BuildWs w;
+  w.keys = c.take<uint64_t>(keys_in_smem(m) ? 1 : size_t(Q) * pow2_at_least(m));
+  w.total = c.used;
   return w;
 }
 
-struct TopkWs { int* rows32; double* sc; int64_t* run_ix; int* cnt; double* top_s; int64_t* top_i;
-                unsigned long long* status; size_t total; };
-int trunc_cap(int m) { return static_cast<int>(ceil_div(m, SORT_RUN) * SORT_RUN); }
+struct TopkWs { SortScratch s; int* cnt; double* top_s; int64_t* top_i; unsigned long long* status; size_t total; };
 TopkWs topk_ws(void* base, int Q, int m, int k) {
-  TopkWs w{};
-  size_t o = 0;
-  auto take = [&](size_t b) { const size_t at = o; o += align256(b); return static_cast<char*>(base) + at; };
-  const size_t qc = size_t(Q) * trunc_cap(m);
+  Carver c(base);
+  TopkWs w;
   const size_t qk = size_t(Q) * std::min(k, m);
-  w.rows32 = reinterpret_cast<int*>(take(qc * 4));
-  w.sc = reinterpret_cast<double*>(take(qc * 8));
-  w.run_ix = reinterpret_cast<int64_t*>(take(qc * 8));
-  w.cnt = reinterpret_cast<int*>(take(size_t(Q) * 4));
-  w.top_s = reinterpret_cast<double*>(take(qk * 8));
-  w.top_i = reinterpret_cast<int64_t*>(take(qk * 8));
-  w.status = reinterpret_cast<unsigned long long*>(take(8 * 8));
-  w.total = o;
+  w.s = take_sort_scratch(c, Q, sort_run_cap(m));
+  w.cnt = c.take<int>(Q);
+  w.top_s = c.take<double>(qk);
+  w.top_i = c.take<int64_t>(qk);
+  w.status = c.take<unsigned long long>(8);
+  w.total = c.used;
   return w;
 }
 
@@ -380,7 +374,9 @@ int dirb200_diffusion_trunc_build(const int64_t* row_ptr_dev, const int* col_dev
 
 size_t dirb200_diffusion_trunc_solve_workspace_bytes(int Q, int m) {
   if (Q < 1 || m < 1) return 0;
-  return cg_in_smem(m) ? 256 : align256(size_t(Q) * cg_smem_bytes(m));
+  Carver c(nullptr);
+  c.take<char>(cg_in_smem(m) ? 1 : size_t(Q) * cg_smem_bytes(m));
+  return c.used;
 }
 
 int dirb200_diffusion_trunc_solve(const int* lcnt_dev, const int* lcol_dev, const double* lval_dev, int kw,
@@ -426,12 +422,12 @@ int dirb200_diffusion_trunc_topk(const int64_t* rows_dev, const double* f_dev, i
   DIRB_REQUIRE(rows_dev && f_dev && ws_dev && scores_dev && idx_dev, DIRB200_EINVAL, "diffusion_trunc_topk: null argument");
   DIRB_TRY(require_sm90());
   TopkWs w = topk_ws(ws_dev, Q, m, k);
-  const int cap2 = trunc_cap(m);
+  const int cap2 = sort_run_cap(m);
   const int kk = std::min(k, m);
   trunc_gather_kernel<<<dim3(static_cast<unsigned>(ceil_div(m, 256)), Q), 256, 0, stream>>>(rows_dev, f_dev, m, cap2,
-                                                                                            w.rows32, w.sc, w.cnt);
+                                                                                            w.s.rows, w.s.sc, w.cnt);
   count_launch();
-  DIRB_TRY(sort_runs_merge(w.rows32, w.cnt, cap2, w.sc, w.run_ix, Q, kk, w.status, w.top_s, w.top_i, stream));
+  DIRB_TRY(sort_runs_merge(w.s.rows, w.cnt, cap2, w.s.sc, w.s.run_ix, Q, kk, 0, w.status, w.top_s, w.top_i, stream));
   trunc_emit_kernel<<<dim3(static_cast<unsigned>(ceil_div(k, 256)), Q), 256, 0, stream>>>(
       w.top_s, w.top_i, kk, list_score_dev, list_idx_dev, list_width, k, scores_dev, idx_dev);
   count_launch();

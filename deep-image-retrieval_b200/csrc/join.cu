@@ -20,8 +20,6 @@ namespace {
 constexpr int CC_THREADS = 256;
 constexpr int SCAN_THREADS = 1024;
 
-inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
-
 __global__ void cc_init_kernel(int64_t* __restrict__ parent, int64_t n) {
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x)
     parent[i] = i;
@@ -113,36 +111,24 @@ __global__ void __launch_bounds__(SCAN_THREADS) group_offsets_kernel(const int64
 }
 
 struct GroupWs {
-  int* size = nullptr;
-  int* rows = nullptr;
-  double* key = nullptr;
-  int64_t* run_ix = nullptr;
-  double* out_key = nullptr;
-  int* cnt = nullptr;
-  int64_t* counts = nullptr;
-  unsigned long long* status = nullptr;
-  size_t total = 0;
+  int* size;
+  SortScratch sort;
+  double* out_key;
+  int* cnt;
+  int64_t* counts;
+  unsigned long long* status;
+  size_t total;
 };
 GroupWs group_ws(void* base, int64_t n) {
+  Carver c(base);
   GroupWs w;
-  const size_t cap2 = static_cast<size_t>(ceil_div(std::max<int64_t>(n, 1), SORT_RUN) * SORT_RUN);
-  size_t off = 0;
-  auto carve = [&](size_t bytes) { size_t o = off; off += align256(bytes); return o; };
-  const size_t o_size = carve(static_cast<size_t>(n) * 4), o_rows = carve(cap2 * 4), o_key = carve(cap2 * 8),
-               o_run = carve(cap2 * 8), o_out = carve(static_cast<size_t>(n) * 8), o_cnt = carve(4), o_counts = carve(16),
-               o_status = carve(64);
-  w.total = off;
-  if (base) {
-    uint8_t* b = static_cast<uint8_t*>(base);
-    w.size = reinterpret_cast<int*>(b + o_size);
-    w.rows = reinterpret_cast<int*>(b + o_rows);
-    w.key = reinterpret_cast<double*>(b + o_key);
-    w.run_ix = reinterpret_cast<int64_t*>(b + o_run);
-    w.out_key = reinterpret_cast<double*>(b + o_out);
-    w.cnt = reinterpret_cast<int*>(b + o_cnt);
-    w.counts = reinterpret_cast<int64_t*>(b + o_counts);
-    w.status = reinterpret_cast<unsigned long long*>(b + o_status);
-  }
+  w.size = c.take<int>(n);
+  w.sort = take_sort_scratch(c, 1, sort_run_cap(std::max<int64_t>(n, 1)));
+  w.out_key = c.take<double>(n);
+  w.cnt = c.take<int>(1);
+  w.counts = c.take<int64_t>(2);
+  w.status = c.take<unsigned long long>(8);
+  w.total = c.used;
   return w;
 }
 
@@ -200,14 +186,14 @@ int dirb200_join_groups(const int64_t* labels_dev, int64_t n, void* ws_dev, int6
   DIRB_CUDA(cudaMemsetAsync(w.size, 0, static_cast<size_t>(n) * 4, stream));
   DIRB_CUDA(cudaMemsetAsync(w.cnt, 0, 4, stream));
   group_size_kernel<<<grid_for(n), CC_THREADS, 0, stream>>>(labels_dev, n, w.size);
-  group_gather_kernel<<<grid_for(n), CC_THREADS, 0, stream>>>(labels_dev, n, w.size, w.rows, w.key, w.cnt);
+  group_gather_kernel<<<grid_for(n), CC_THREADS, 0, stream>>>(labels_dev, n, w.size, w.sort.rows, w.sort.sc, w.cnt);
   count_launch(2);
   int m = 0;
   DIRB_CUDA(cudaMemcpyAsync(&m, w.cnt, 4, cudaMemcpyDeviceToHost, stream));
   DIRB_CUDA(cudaStreamSynchronize(stream));
   if (m > 0) {
-    const int cap2 = static_cast<int>(ceil_div(m, SORT_RUN) * SORT_RUN);
-    DIRB_TRY(sort_runs_merge(w.rows, w.cnt, cap2, w.key, w.run_ix, 1, m, w.status, w.out_key, members_dev, stream));
+    DIRB_TRY(sort_runs_merge(w.sort.rows, w.cnt, sort_run_cap(m), w.sort.sc, w.sort.run_ix, 1, m, 0, w.status, w.out_key,
+                             members_dev, stream));
   }
   group_offsets_kernel<<<1, SCAN_THREADS, 0, stream>>>(members_dev, labels_dev, m, group_off_dev, w.counts);
   count_launch();

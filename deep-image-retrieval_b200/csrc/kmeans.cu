@@ -35,7 +35,6 @@ constexpr int KM_COLS = 256;       // columns per block of the centre sums
 constexpr int PP_ROWS = 256;       // rows per block of a k-means++ weight launch
 constexpr double FIX32 = 4294967296.0;
 
-inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
 unsigned grid_for(int64_t n) { return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, KM_THREADS), 8192))); }
 
 // Inclusive scan of one value per thread over a block of KM_SCAN threads; *total receives the block's sum.
@@ -281,93 +280,83 @@ __global__ void __launch_bounds__(KM_SCAN) km_pp_select_kernel(const long long* 
 }
 
 struct SortWs {
-  int* rows = nullptr;
-  double* key = nullptr;
-  int64_t* run_ix = nullptr;
-  double* out_key = nullptr;
-  int64_t* order = nullptr;
-  int* cnt = nullptr;
-  unsigned long long* status = nullptr;
-  size_t total = 0;
+  SortScratch s;
+  double* out_key;
+  int64_t* order;
+  int* cnt;
+  unsigned long long* status;
 };
-// The sort buffers of n rows from `off` bytes into the workspace.
-SortWs sort_ws(uint8_t* b, size_t off, int64_t n) {
+// The sort buffers of n rows, taken from c.
+SortWs sort_ws(Carver& c, int64_t n) {
   SortWs w;
-  const size_t cap2 = static_cast<size_t>(ceil_div(std::max<int64_t>(n, 1), SORT_RUN) * SORT_RUN);
-  auto carve = [&](size_t bytes) { size_t o = off; off += align256(bytes); return o; };
-  const size_t o_rows = carve(cap2 * 4), o_key = carve(cap2 * 8), o_run = carve(cap2 * 8), o_out = carve(n * 8),
-               o_order = carve(n * 8), o_cnt = carve(4), o_status = carve(64);
-  w.total = off;
-  if (b) {
-    w.rows = reinterpret_cast<int*>(b + o_rows);
-    w.key = reinterpret_cast<double*>(b + o_key);
-    w.run_ix = reinterpret_cast<int64_t*>(b + o_run);
-    w.out_key = reinterpret_cast<double*>(b + o_out);
-    w.order = reinterpret_cast<int64_t*>(b + o_order);
-    w.cnt = reinterpret_cast<int*>(b + o_cnt);
-    w.status = reinterpret_cast<unsigned long long*>(b + o_status);
-  }
+  w.s = take_sort_scratch(c, 1, sort_run_cap(std::max<int64_t>(n, 1)));
+  w.out_key = c.take<double>(n);
+  w.order = c.take<int64_t>(n);
+  w.cnt = c.take<int>(1);
+  w.status = c.take<unsigned long long>(8);
   return w;
 }
 
 // Rows 0 .. n-1 into w.order by (label asc, row asc) when labels is given, else by (score asc, row asc).
 int order_rows(const SortWs& w, const int64_t* labels, const double* scores, int64_t n, cudaStream_t stream) {
   const int n32 = static_cast<int>(n);
-  km_keys_kernel<<<grid_for(n), KM_THREADS, 0, stream>>>(labels, scores, n, w.rows, w.key);
+  km_keys_kernel<<<grid_for(n), KM_THREADS, 0, stream>>>(labels, scores, n, w.s.rows, w.s.sc);
   count_launch();
   DIRB_CUDA(cudaMemcpyAsync(w.cnt, &n32, 4, cudaMemcpyHostToDevice, stream));
-  const int cap2 = static_cast<int>(ceil_div(n, SORT_RUN) * SORT_RUN);
-  return sort_runs_merge(w.rows, w.cnt, cap2, w.key, w.run_ix, 1, n32, w.status, w.out_key, w.order, stream);
+  return sort_runs_merge(w.s.rows, w.cnt, sort_run_cap(n), w.s.sc, w.s.run_ix, 1, n32, 0, w.status, w.out_key, w.order,
+                         stream);
+}
+
+// dirb200_kmeans_relocate: the moves counter, then the sort buffers
+struct RelocateWs {
+  long long* moves;
+  SortWs sort;
+  size_t total;
+};
+RelocateWs relocate_ws(void* base, int64_t n) {
+  Carver c(base);
+  RelocateWs w;
+  w.moves = c.take<long long>(1);
+  w.sort = sort_ws(c, n);
+  w.total = c.used;
+  return w;
 }
 
 struct UpdateWs {
-  int64_t* off = nullptr;
-  double* s = nullptr;
-  unsigned long long* zero = nullptr;
+  int64_t* off;
+  double* s;
+  unsigned long long* zero;
   SortWs sort;
-  size_t total = 0;
+  size_t total;
 };
 UpdateWs update_ws(void* base, int64_t n, int k, int d) {
+  Carver c(base);
   UpdateWs w;
-  uint8_t* b = static_cast<uint8_t*>(base);
-  size_t off = 0;
-  auto carve = [&](size_t bytes) { size_t o = off; off += align256(bytes); return o; };
-  const size_t o_off = carve(static_cast<size_t>(k + 1) * 8),
-               o_s = carve(static_cast<size_t>(k) * d * 8), o_zero = carve(8);
-  w.sort = sort_ws(b, off, n);
-  w.total = w.sort.total;
-  if (b) {
-    w.off = reinterpret_cast<int64_t*>(b + o_off);
-    w.s = reinterpret_cast<double*>(b + o_s);
-    w.zero = reinterpret_cast<unsigned long long*>(b + o_zero);
-  }
+  w.off = c.take<int64_t>(static_cast<size_t>(k) + 1);
+  w.s = c.take<double>(static_cast<size_t>(k) * d);
+  w.zero = c.take<unsigned long long>(1);
+  w.sort = sort_ws(c, n);
+  w.total = c.used;
   return w;
 }
 
 struct PpWs {
-  double* best = nullptr;
-  long long* w = nullptr;
-  long long* bsum = nullptr;
-  double* u = nullptr;
-  uint8_t* flag = nullptr;
-  size_t total = 0;
+  double* best;
+  long long* w;
+  long long* bsum;
+  double* u;
+  uint8_t* flag;
+  size_t total;
 };
 PpWs pp_ws(void* base, int64_t n, int k) {
+  Carver c(base);
   PpWs w;
-  const int64_t nb = ceil_div(n, PP_ROWS);
-  size_t off = 0;
-  auto carve = [&](size_t bytes) { size_t o = off; off += align256(bytes); return o; };
-  const size_t o_best = carve(n * 8), o_w = carve(n * 8), o_bsum = carve(nb * 8), o_u = carve(static_cast<size_t>(k) * 8),
-               o_flag = carve(n);
-  w.total = off;
-  if (base) {
-    uint8_t* b = static_cast<uint8_t*>(base);
-    w.best = reinterpret_cast<double*>(b + o_best);
-    w.w = reinterpret_cast<long long*>(b + o_w);
-    w.bsum = reinterpret_cast<long long*>(b + o_bsum);
-    w.u = reinterpret_cast<double*>(b + o_u);
-    w.flag = b + o_flag;
-  }
+  w.best = c.take<double>(n);
+  w.w = c.take<long long>(n);
+  w.bsum = c.take<long long>(ceil_div(n, PP_ROWS));
+  w.u = c.take<double>(k);
+  w.flag = c.take<uint8_t>(n);
+  w.total = c.used;
   return w;
 }
 
@@ -406,7 +395,7 @@ int dirb200_kmeans_stats(const int64_t* labels_dev, const double* scores_dev, co
 
 size_t dirb200_kmeans_relocate_workspace_bytes(int64_t n) {
   if (n < 1) return 0;
-  return sort_ws(nullptr, 256, n).total;
+  return relocate_ws(nullptr, n).total;
 }
 
 int dirb200_kmeans_relocate(int64_t* labels_dev, const double* scores_dev, int64_t n, int k, int* counts_dev,
@@ -415,14 +404,12 @@ int dirb200_kmeans_relocate(int64_t* labels_dev, const double* scores_dev, int64
                DIRB200_EINVAL, "bad arguments");
   DIRB_REQUIRE(n < KM_MAX_ROWS, DIRB200_ENOTSUP, "too many rows (%lld)", static_cast<long long>(n));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  uint8_t* b = static_cast<uint8_t*>(ws_dev);
-  long long* moves = reinterpret_cast<long long*>(b);
-  const SortWs w = sort_ws(b, 256, n);
-  DIRB_TRY(order_rows(w, nullptr, scores_dev, n, stream));
-  km_relocate_kernel<<<1, KM_SCAN, 0, stream>>>(w.order, n, k, labels_dev, counts_dev, moves);
+  const RelocateWs w = relocate_ws(ws_dev, n);
+  DIRB_TRY(order_rows(w.sort, nullptr, scores_dev, n, stream));
+  km_relocate_kernel<<<1, KM_SCAN, 0, stream>>>(w.sort.order, n, k, labels_dev, counts_dev, w.moves);
   count_launch();
   long long mv = 0;
-  DIRB_CUDA(cudaMemcpyAsync(&mv, moves, 8, cudaMemcpyDeviceToHost, stream));
+  DIRB_CUDA(cudaMemcpyAsync(&mv, w.moves, 8, cudaMemcpyDeviceToHost, stream));
   DIRB_CUDA(cudaStreamSynchronize(stream));
   DIRB_CUDA(cudaGetLastError());
   *moves_out = mv;

@@ -321,48 +321,46 @@ __global__ void count_scan_kernel(int Q, const int* __restrict__ thr_off, unsign
   }
 }
 
-struct WsLayout {
-  size_t m, qn, flags, band, over, list, total;
+struct CountGeWs {
+  double* m;
+  double* qn;
+  unsigned int* flags;          // 32 bytes: the F_* words, the band counter among them
+  unsigned long long* band;
+  int* q_over;
+  int* q_list;
+  size_t total;
 };
-WsLayout ws_layout(int Q, int T, int band_cap) {
-  WsLayout l{};
-  size_t off = 0;
-  auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-  l.m = carve(static_cast<size_t>(T) * 8);
-  l.qn = carve(static_cast<size_t>(Q) * 8);
-  l.flags = carve(32);
-  l.band = carve(static_cast<size_t>(band_cap) * 8);
-  l.over = carve(static_cast<size_t>(Q) * 4);
-  l.list = carve(static_cast<size_t>(Q) * 4);
-  l.total = off;
-  return l;
+CountGeWs count_ge_ws(void* base, int Q, int T, int band_cap) {
+  Carver c(base);
+  CountGeWs w;
+  w.m = c.take<double>(T);
+  w.qn = c.take<double>(Q);
+  w.flags = c.take<unsigned int>(8);
+  w.band = c.take<unsigned long long>(band_cap);
+  w.q_over = c.take<int>(Q);
+  w.q_list = c.take<int>(Q);
+  w.total = c.used;
+  return w;
 }
 
 }  // namespace
 
-size_t count_ge_ws_bytes(int Q, int T, int band_cap) { return ws_layout(Q, T, band_cap).total; }
+size_t count_ge_ws_bytes(int Q, int T, int band_cap) { return count_ge_ws(nullptr, Q, T, band_cap).total; }
 
 int count_ge_run(const CountGeArgs& a, void* ws, CountGeStats* st, cudaStream_t stream) {
   const int Q = a.Q, T = a.T, D = a.D;
   const int64_t N = a.N;
-  const WsLayout l = ws_layout(Q, T, a.band_cap);
-  uint8_t* w = static_cast<uint8_t*>(ws);
-  double* m = reinterpret_cast<double*>(w + l.m);
-  double* qn = reinterpret_cast<double*>(w + l.qn);
-  unsigned int* flags = reinterpret_cast<unsigned int*>(w + l.flags);
-  unsigned long long* band_cnt = reinterpret_cast<unsigned long long*>(flags + F_BAND);
-  unsigned long long* band = reinterpret_cast<unsigned long long*>(w + l.band);
-  int* q_over = reinterpret_cast<int*>(w + l.over);
-  int* q_list = reinterpret_cast<int*>(w + l.list);
+  const CountGeWs w = count_ge_ws(ws, Q, T, a.band_cap);
+  unsigned long long* band_cnt = reinterpret_cast<unsigned long long*>(w.flags + F_BAND);
   unsigned long long* diff = reinterpret_cast<unsigned long long*>(a.count);
   *st = CountGeStats{};
 
-  DIRB_CUDA(cudaMemsetAsync(flags, 0, 32, stream));
-  count_prep_kernel<<<static_cast<unsigned>(ceil_div(Q, 8)), 256, 0, stream>>>(a.q32, Q, D, a.thr_off, T, a.thr, m, qn,
-                                                                               diff, q_over, flags);
+  DIRB_CUDA(cudaMemsetAsync(w.flags, 0, 32, stream));
+  count_prep_kernel<<<static_cast<unsigned>(ceil_div(Q, 8)), 256, 0, stream>>>(a.q32, Q, D, a.thr_off, T, a.thr, w.m, w.qn,
+                                                                               diff, w.q_over, w.flags);
   count_launch();
   if (N > 0) {
-    row_norm_max_kernel<<<static_cast<unsigned>(ceil_div(N, 8)), 256, 0, stream>>>(a.db32, N, D, flags);
+    row_norm_max_kernel<<<static_cast<unsigned>(ceil_div(N, 8)), 256, 0, stream>>>(a.db32, N, D, w.flags);
     count_launch();
     static std::atomic<uint64_t> attr_done{0};
     if (first_launch_on_device(attr_done))
@@ -370,19 +368,19 @@ int count_ge_run(const CountGeArgs& a, void* ws, CountGeStats* st, cudaStream_t 
     const double u = ldexp(1.0, -53);
     const double gamma = D * u / (1.0 - D * u);
     const dim3 grid(static_cast<unsigned>(ceil_div(N, CG_BN)), static_cast<unsigned>(ceil_div(Q, CG_BM)));
-    count_ge_gemm_kernel<<<grid, CG_THREADS, CG_SMEM, stream>>>(a.q32, Q, a.db32, N, D, a.offset, a.thr_off, m, qn,
-                                                                a.skip_row, a.eps, 4.0 * gamma, flags, diff, band,
-                                                                band_cnt, a.band_cap, q_over);
+    count_ge_gemm_kernel<<<grid, CG_THREADS, CG_SMEM, stream>>>(a.q32, Q, a.db32, N, D, a.offset, a.thr_off, w.m, w.qn,
+                                                                a.skip_row, a.eps, 4.0 * gamma, w.flags, diff, w.band,
+                                                                band_cnt, a.band_cap, w.q_over);
     count_launch();
-    count_band_kernel<<<4 * num_sms(), 256, 0, stream>>>(a.q32, a.db32, D, a.thr_off, a.thr, band, band_cnt, a.band_cap,
-                                                         q_over, diff);
+    count_band_kernel<<<4 * num_sms(), 256, 0, stream>>>(a.q32, a.db32, D, a.thr_off, a.thr, w.band, band_cnt, a.band_cap,
+                                                         w.q_over, diff);
     count_launch();
   }
   DIRB_CUDA(cudaGetLastError());
   std::vector<int> over(Q);
   unsigned int hflags[8];
-  DIRB_CUDA(cudaMemcpyAsync(over.data(), q_over, static_cast<size_t>(Q) * 4, cudaMemcpyDeviceToHost, stream));
-  DIRB_CUDA(cudaMemcpyAsync(hflags, flags, 32, cudaMemcpyDeviceToHost, stream));
+  DIRB_CUDA(cudaMemcpyAsync(over.data(), w.q_over, static_cast<size_t>(Q) * 4, cudaMemcpyDeviceToHost, stream));
+  DIRB_CUDA(cudaMemcpyAsync(hflags, w.flags, 32, cudaMemcpyDeviceToHost, stream));
   DIRB_CUDA(cudaStreamSynchronize(stream));
   DIRB_REQUIRE((hflags[F_ERR] & 2u) == 0, DIRB200_EINVAL, "count_ge: threshold offsets must be a CSR running from 0 to T");
   DIRB_REQUIRE((hflags[F_ERR] & 1u) == 0, DIRB200_EINVAL,
@@ -396,13 +394,13 @@ int count_ge_run(const CountGeArgs& a, void* ws, CountGeStats* st, cudaStream_t 
   st->fallback = static_cast<int64_t>(list.size());
   if (!list.empty()) {
     const int n = static_cast<int>(list.size());
-    DIRB_CUDA(cudaMemcpyAsync(q_list, list.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, stream));
-    count_clear_kernel<<<n, 256, 0, stream>>>(q_list, n, a.thr_off, diff);
+    DIRB_CUDA(cudaMemcpyAsync(w.q_list, list.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, stream));
+    count_clear_kernel<<<n, 256, 0, stream>>>(w.q_list, n, a.thr_off, diff);
     count_launch();
     const int gx = static_cast<int>(std::min<int64_t>(ceil_div(N, 8), 4 * static_cast<int64_t>(num_sms())));
     for (int i0 = 0; i0 < n; i0 += 65535) {
       const unsigned ny = static_cast<unsigned>(std::min(65535, n - i0));
-      count_exact_kernel<<<dim3(gx, ny), 256, 0, stream>>>(a.q32, a.db32, N, D, a.offset, q_list + i0, a.thr_off, a.thr,
+      count_exact_kernel<<<dim3(gx, ny), 256, 0, stream>>>(a.q32, a.db32, N, D, a.offset, w.q_list + i0, a.thr_off, a.thr,
                                                             a.skip_row, diff);
       count_launch();
     }

@@ -575,36 +575,36 @@ static int setup_workspace(dirb200_net* n, int chunk, int H, int W, Workspace* w
   const int* h = w->sz.h;
   const int* wd = w->sz.w;
   const size_t c = chunk;
-  size_t off = 0;
-  auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 1023) / 1024 * 1024; return o; };
   // the fused stem reads the images and writes the pooled map: neither intermediate exists
   const bool unfused = !stem_fused(n);
-  const size_t o_sws = carve(unfused ? std::max(c * H * W * 8 * 2, stem_workspace_bytes(chunk, H, W)) : 0);
-  const size_t o_stem = carve(unfused || n->debug_taps ? c * h[1] * wd[1] * 64 * 2 : 0);
-  size_t o_stage[4], o_scr[4];
-  for (int s = 0; s < 4; ++s) o_stage[s] = carve(c * h[2 + s] * wd[2 + s] * n->stage_ch[s] * 2);
+  const size_t sws = unfused ? std::max(c * H * W * 8, stem_workspace_bytes(chunk, H, W) / 2) : 0;
+  const size_t stem = unfused || n->debug_taps ? c * h[1] * wd[1] * 64 : 0;
   size_t scr = 0;   // largest tensor inside any stage: conv1 output at the stage's input resolution, or a block output
   for (int s = 1; s < 5; ++s) {
-    scr = std::max(scr, c * h[1 + s] * wd[1 + s] * (n->stage_ch[s] / 4) * 2);
-    scr = std::max(scr, c * h[2 + s] * wd[2 + s] * n->stage_ch[s] * 2);
+    scr = std::max(scr, c * h[1 + s] * wd[1 + s] * (n->stage_ch[s] / 4));
+    scr = std::max(scr, c * h[2 + s] * wd[2 + s] * n->stage_ch[s]);
   }
   if (n->fpn)   // the merged / smoothed layer3 map of the FPN head lives in a scratch tensor
-    scr = std::max(scr, c * h[5] * wd[5] * n->stage_ch[3] * 2);
-  for (int i = 0; i < 4; ++i) o_scr[i] = carve(scr);
+    scr = std::max(scr, c * h[5] * wd[5] * n->stage_ch[3]);
   size_t head_floats = head_workspace_floats(chunk, h[6] * wd[6], n->stage_ch[4], n->out_dim);
   if (n->fpn) {
     const size_t partial = std::max(head_partial_floats(chunk, h[5] * wd[5], n->stage_ch[3]),
                                     head_partial_floats(chunk, h[6] * wd[6], n->stage_ch[4]));
     head_floats = partial + c * (n->feat_in() + std::max(n->out_dim, n->feat_in()));
   }
-  const size_t o_head = carve(head_floats * 4);
-  DIRB_TRY(grow_device(&n->ws, &n->ws_bytes, off));
-  uint8_t* ws = static_cast<uint8_t*>(n->ws);
-  w->stem_ws = unfused ? reinterpret_cast<__half*>(ws + o_sws) : nullptr;
-  w->stem_out = unfused || n->debug_taps ? reinterpret_cast<__half*>(ws + o_stem) : nullptr;
-  for (int s = 0; s < 4; ++s) w->stage_out[s] = reinterpret_cast<__half*>(ws + o_stage[s]);
-  for (int i = 0; i < 4; ++i) w->scratch[i] = reinterpret_cast<__half*>(ws + o_scr[i]);
-  w->head_ws = reinterpret_cast<float*>(ws + o_head);
+  auto layout = [&](void* base) {
+    Carver cv(base, 1024);
+    __half* stem_ws = cv.take<__half>(sws);
+    __half* stem_out = cv.take<__half>(stem);
+    w->stem_ws = unfused ? stem_ws : nullptr;
+    w->stem_out = unfused || n->debug_taps ? stem_out : nullptr;
+    for (int s = 0; s < 4; ++s) w->stage_out[s] = cv.take<__half>(c * h[2 + s] * wd[2 + s] * n->stage_ch[s]);
+    for (int i = 0; i < 4; ++i) w->scratch[i] = cv.take<__half>(scr);
+    w->head_ws = cv.take<float>(head_floats);
+    return cv.used;
+  };
+  DIRB_TRY(grow_device(&n->ws, &n->ws_bytes, layout(nullptr)));
+  layout(n->ws);
   return 0;
 }
 

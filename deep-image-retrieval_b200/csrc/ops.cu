@@ -787,18 +787,21 @@ __global__ void split_f16_kernel(const float* __restrict__ x, const float* __res
 static int whiten_tc(const float* x, int64_t N, int D, const float* comp, const float* mean, const float* colscale,
                      int Dout, float* y, cudaStream_t stream) {
   const size_t xe = static_cast<size_t>(N) * D, ce = static_cast<size_t>(Dout) * D;
-  auto al = [](size_t b) { return (b + 1023) & ~size_t(1023); };
-  const size_t o_xh = 0, o_xl = o_xh + al(xe * 2), o_ch = o_xl + al(xe * 2), o_cl = o_ch + al(ce * 2);
-  const size_t o_ws = o_cl + al(ce * 2), o_cs = o_ws + 1024, total_bytes = o_cs + al(static_cast<size_t>(Dout) * 4);
+  __half *xh, *xl, *ch, *cl;
+  float *ws, *cs;
+  auto layout = [&](void* base) {
+    Carver c(base, 1024);
+    xh = c.take<__half>(xe);
+    xl = c.take<__half>(xe);
+    ch = c.take<__half>(ce);
+    cl = c.take<__half>(ce);
+    ws = c.take<float>(256);
+    cs = c.take<float>(Dout);
+    return c.used;
+  };
   void* base = nullptr;
-  DIRB_TRY(scratch_acquire(total_bytes, stream, &base));
-  uint8_t* b8 = static_cast<uint8_t*>(base);
-  __half* xh = reinterpret_cast<__half*>(b8 + o_xh);
-  __half* xl = reinterpret_cast<__half*>(b8 + o_xl);
-  __half* ch = reinterpret_cast<__half*>(b8 + o_ch);
-  __half* cl = reinterpret_cast<__half*>(b8 + o_cl);
-  float* ws = reinterpret_cast<float*>(b8 + o_ws);
-  float* cs = reinterpret_cast<float*>(b8 + o_cs);
+  DIRB_TRY(scratch_acquire(layout(nullptr), stream, &base));
+  layout(base);
   DIRB_CUDA(cudaMemsetAsync(ws, 0, 32, stream));
   const unsigned gx = static_cast<unsigned>(std::min<int64_t>(ceil_div(ceil_div(xe, 4), 256), num_sms() * 16));
   const unsigned gc = static_cast<unsigned>(std::min<int64_t>(ceil_div(ceil_div(ce, 4), 256), num_sms() * 16));

@@ -467,9 +467,9 @@ __global__ void __launch_bounds__(FIN_THREADS) search_finish_kernel(
 // of search_finish_kernel, but they live in global memory and each step runs over many blocks per query:
 //   deep_compact_kernel   survivors (fp16-path score >= max(sel, kth_k) - band) -> surv_row[q][cap2], surv_cnt[q]
 //   deep_rescore_kernel   one warp per survivor: exact score -> surv_sc[q][cap2]
-//   deep_run_sort_kernel  runs of DEEP_RUN survivors bitonic-sorted in shared memory -> (score, global index) in place
+//   deep_run_sort_kernel  runs of SORT_RUN survivors bitonic-sorted in shared memory -> (score, global index) in place
 //   merge_runs_kernel     rank-based merge of the sorted runs, first k entries (also dirb200_topk_merge at large G*k)
-constexpr int DEEP_RUN = 2048;
+// The last two are sort_runs_merge.
 
 __global__ void deep_compact_kernel(const unsigned long long* __restrict__ cand, const int* __restrict__ cnt, int cap,
                                     const float* __restrict__ kth_k, const float* __restrict__ sel, float band,
@@ -522,13 +522,13 @@ __global__ void __launch_bounds__(FIN_THREADS) deep_run_sort_kernel(const int* _
                                                                     int64_t offset, double* __restrict__ surv_sc,
                                                                     int64_t* __restrict__ run_ix,
                                                                     unsigned long long* __restrict__ status) {
-  __shared__ double sc[DEEP_RUN];
-  __shared__ int ix[DEEP_RUN];
+  __shared__ double sc[SORT_RUN];
+  __shared__ int ix[SORT_RUN];
   const int q = blockIdx.y;
   const int ns = min(surv_cnt[q], cap2);
-  const int base = blockIdx.x * DEEP_RUN;
+  const int base = blockIdx.x * SORT_RUN;
   if (base >= ns) return;                                  // uniform over the block
-  const int n = min(DEEP_RUN, ns - base);
+  const int n = min(SORT_RUN, ns - base);
   const int64_t o = static_cast<int64_t>(q) * cap2 + base;
   int P = 2;
   while (P < n) P <<= 1;
@@ -555,7 +555,7 @@ __global__ void __launch_bounds__(FIN_THREADS) deep_run_sort_kernel(const int* _
       __syncthreads();
     }
   }
-  for (int i = threadIdx.x; i < DEEP_RUN; i += FIN_THREADS) {
+  for (int i = threadIdx.x; i < SORT_RUN; i += FIN_THREADS) {
     const bool ok = i < n;
     surv_sc[o + i] = ok ? sc[i] : -INFINITY;
     run_ix[o + i] = ok ? static_cast<int64_t>(ix[i]) + offset : -1;
@@ -935,17 +935,16 @@ __global__ void join_emit_kernel(const double* __restrict__ out_sc, const int64_
 
 }  // namespace
 
-static_assert(DEEP_RUN == SORT_RUN, "sort_runs_merge's run length is the deep finish's");
-
 int sort_runs_merge(const int* rows, const int* cnt, int cap2, double* sc, int64_t* run_ix, int Q, int k,
-                    unsigned long long* status, double* out_score, int64_t* out_idx, cudaStream_t stream) {
-  const int runs = cap2 / DEEP_RUN;
-  deep_run_sort_kernel<<<dim3(runs, Q), FIN_THREADS, 0, stream>>>(rows, cnt, cap2, 0, sc, run_ix, status);
+                    int64_t row_offset, unsigned long long* status, double* out_score, int64_t* out_idx,
+                    cudaStream_t stream) {
+  const int runs = cap2 / SORT_RUN;
+  deep_run_sort_kernel<<<dim3(runs, Q), FIN_THREADS, 0, stream>>>(rows, cnt, cap2, row_offset, sc, run_ix, status);
   const int64_t n = static_cast<int64_t>(Q) * k;
   fill_empty_result_kernel<<<static_cast<unsigned>(ceil_div(n, 256)), 256, 0, stream>>>(out_score, out_idx, n);
-  const int64_t elems = static_cast<int64_t>(runs) * std::min(DEEP_RUN, k);
+  const int64_t elems = static_cast<int64_t>(runs) * std::min(SORT_RUN, k);
   merge_runs_kernel<<<dim3(static_cast<unsigned>(ceil_div(elems, 256)), Q), 256, 0, stream>>>(
-      sc, run_ix, runs, DEEP_RUN, DEEP_RUN, cap2, cnt, cap2, Q, k, out_score, out_idx);
+      sc, run_ix, runs, SORT_RUN, SORT_RUN, cap2, cnt, cap2, Q, k, out_score, out_idx);
   count_launch(3);
   DIRB_CUDA(cudaGetLastError());
   return 0;
@@ -967,6 +966,26 @@ struct TmapCache {
     es.push_back(e);
     *out = &es.back().m;
     return 0;
+  }
+};
+
+// CUDA events marking the phases of a call (option "profile"), created on first use.
+template <int N>
+struct PhaseEvents {
+  cudaEvent_t ev[N] = {};
+  void mark(int i, cudaStream_t stream) {
+    if (i >= N) return;
+    if (!ev[i]) cudaEventCreate(&ev[i]);
+    cudaEventRecord(ev[i], stream);
+  }
+  float ms(int i, int j) const {       // 0 when either event is missing or incomplete
+    float t = 0;
+    if (cudaEventElapsedTime(&t, ev[i], ev[j]) != cudaSuccess) t = 0;
+    return t;
+  }
+  void destroy() {
+    for (auto e : ev)
+      if (e) cudaEventDestroy(e);
   }
 };
 
@@ -1015,11 +1034,9 @@ struct dirb200_index {
     int64_t S_ld = 0;
     bool small = false;
     int ks = 0;
-    // deep path (k > 1024): survivors in global memory
-    int* surv_row = nullptr;
+    // deep path (k > 1024): survivors in global memory, in sort_runs_merge's layout
+    SortScratch surv{};
     int* surv_cnt = nullptr;
-    double* surv_sc = nullptr;
-    int64_t* run_ix = nullptr;
   } pend;
   // range search / self-join: workspace, options and the last result (CSR, kept until the next call)
   int join_cap = 0;                // candidate capacity per row of the first filter pass (0 = min(columns, 4096))
@@ -1033,9 +1050,9 @@ struct dirb200_index {
   std::vector<int64_t> res_off;    // host CSR offsets of the last result
   int64_t join_stats[5] = {0, 0, 0, 0, 0};   // candidates, pairs, filter re-runs, filter launches, tiles
   double join_ms[3] = {0, 0, 0};   // option profile: filter passes, exact re-scoring, sort + compaction
+  PhaseEvents<4> jev;
   int nearest_cap = 16;             // dirb200_index_nearest: most candidate groups before a row is re-scored in full
   int64_t nearest_stats[3] = {0, 0, 0};   // rows with > 1 candidate group, rows re-scored in full, centres re-scored
-  cudaEvent_t jev[4] = {};
   // inverted lists (dirb200_index_set_lists): caller-owned fp16 rows in list order, list position -> row, K + 1 offsets
   const __half* l16 = nullptr;
   const int64_t* lperm = nullptr;
@@ -1045,57 +1062,62 @@ struct dirb200_index {
   size_t lws_bytes[2] = {0, 0};
   int64_t lists_stats[6] = {0, 0, 0, 0, 0, 0};   // pairs, query rows issued, tiles, probed rows, candidates, re-runs
   double lists_ms[4] = {0, 0, 0, 0};             // option profile: table build, GMAX pass + seed, FILTER pass, finish
-  cudaEvent_t lev[5] = {};
+  PhaseEvents<5> lev;
   TmapCache tmaps;
   int profile = 0;                 // option "profile": time the phases of a search with CUDA events
-  cudaEvent_t ev[10] = {};
+  PhaseEvents<10> ev;              // separate from jev / lev: the list search's finish marks these
   double phase_ms[9] = {};
 };
 
 // Similarity GEMM on the persistent wgmma kernel (conv_pers.cuh): A = queries [Q][D], B = database rows [rows][D],
 // 128 x 128 tiles, K = D.  Tiles are ordered query-tile-fastest, so CTAs running at the same time share the streamed
 // database tile (L2) and the database is read from HBM once.  Encoded tensor maps are kept per (base, rows) in the
-// handle: a search re-uses the same three maps every call.
+// handle: a search re-uses the same three maps every call.  With a tile table (PERS_EPI_SIM_LGMAX / _LFILTER, the list
+// search) the launch runs its n_tiles entries instead of the Q x rows grid, A rows being the table's query slots.
 struct SimArgs {
   float* dense = nullptr; int64_t dense_ld = 0;
   const float* thr = nullptr; unsigned long long* cand = nullptr; int* cand_cnt = nullptr; int cand_cap = 0;
   const int* gate = nullptr;
+  const int4* tiles = nullptr; int64_t n_tiles = 0; const int* slot_q = nullptr; const int64_t* gbase = nullptr;
 };
-static int sim_gemm(dirb200_index* h, int epi, const __half* q16, int Q, const __half* db16, int64_t rows, int D,
+static int sim_gemm(dirb200_index* h, int epi, const __half* q16, int64_t Q, const __half* db16, int64_t rows, int D,
                     const SimArgs& a, cudaStream_t stream) {
   constexpr int BN = 128;
-  const CUtensorMap *tmA, *tmB;
-  {
-    TmapCache& c = h->tmaps;
-    DIRB_TRY(c.get(q16, D, Q, 128, &tmA));
-    CUtensorMap a_copy = *tmA;                    // `get` may reallocate the vector: copy before the second lookup
-    DIRB_TRY(c.get(db16, D, rows, BN, &tmB));
-    CUtensorMap b_copy = *tmB;
-    ConvPersParams p{};
-    p.a_spatial = 0;
-    p.taps = 1; p.kw_taps = 1; p.cin_blocks = D / 64; p.stride = 1; p.pad = 0;
-    p.tw = 128; p.th = 1; p.nb = 1; p.tiles_w = 1; p.tiles_h = 1;
-    p.M = Q;
-    p.N = static_cast<int>(rows);
-    p.n_tiles = static_cast<int>(ceil_div(rows, BN));
-    p.m_tiles = static_cast<int>(ceil_div(Q, 128));
-    p.m_fastest = 1;
-    // the self-join launches the tiles on or above the diagonal only (decode_tile_tri)
-    const int64_t total = epi == PERS_EPI_SIM_JOIN
-                              ? static_cast<int64_t>(p.m_tiles) * p.n_tiles - static_cast<int64_t>(p.m_tiles) * (p.m_tiles - 1) / 2
-                              : static_cast<int64_t>(p.m_tiles) * p.n_tiles;
-    DIRB_REQUIRE(total < (int64_t(1) << 31), DIRB200_ENOTSUP, "too many tiles");
-    p.total_tiles = static_cast<int>(total);
-    p.dense = a.dense; p.dense_ld = a.dense_ld;
-    p.thr = a.thr; p.cand = a.cand; p.cand_cnt = a.cand_cnt; p.cand_cap = a.cand_cap;
-    p.gate = a.gate;
-    if (epi == PERS_EPI_SIM_DENSE)
-      return conv_pers_launch<BN, 6, PERS_EPI_SIM_DENSE>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
-    if (epi == PERS_EPI_SIM_GMAX)
-      return conv_pers_launch<BN, 6, PERS_EPI_SIM_GMAX>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
-    if (epi == PERS_EPI_SIM_JOIN)
-      return conv_pers_launch<BN, 6, PERS_EPI_SIM_JOIN>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
-    return conv_pers_launch<BN, 6, PERS_EPI_SIM_FILTER>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
+  DIRB_REQUIRE(Q < (int64_t(1) << 31), DIRB200_ENOTSUP, "too many tiles");
+  const CUtensorMap* tm;
+  DIRB_TRY(h->tmaps.get(q16, D, Q, 128, &tm));
+  const CUtensorMap a_copy = *tm;                 // `get` may reallocate the vector: copy before the second lookup
+  DIRB_TRY(h->tmaps.get(db16, D, rows, BN, &tm));
+  const CUtensorMap b_copy = *tm;
+  ConvPersParams p{};
+  p.a_spatial = 0;
+  p.taps = 1; p.kw_taps = 1; p.cin_blocks = D / 64; p.stride = 1; p.pad = 0;
+  p.tw = 128; p.th = 1; p.nb = 1; p.tiles_w = 1; p.tiles_h = 1;
+  p.M = static_cast<int>(Q);
+  p.N = static_cast<int>(rows);
+  p.n_tiles = static_cast<int>(ceil_div(rows, BN));
+  p.m_tiles = static_cast<int>(ceil_div(Q, 128));
+  p.m_fastest = 1;
+  int64_t total = static_cast<int64_t>(p.m_tiles) * p.n_tiles;
+  // the self-join launches the tiles on or above the diagonal only (decode_tile_tri)
+  if (epi == PERS_EPI_SIM_JOIN) total -= static_cast<int64_t>(p.m_tiles) * (p.m_tiles - 1) / 2;
+  if (a.tiles) total = a.n_tiles;
+  DIRB_REQUIRE(total < (int64_t(1) << 31), DIRB200_ENOTSUP, "too many tiles");
+  p.total_tiles = static_cast<int>(total);
+  p.dense = a.dense; p.dense_ld = a.dense_ld;
+  p.thr = a.thr; p.cand = a.cand; p.cand_cnt = a.cand_cnt; p.cand_cap = a.cand_cap;
+  p.gate = a.gate;
+  p.tiles = a.tiles; p.slot_q = a.slot_q; p.gbase = a.gbase;
+  if (a.tiles) p.perm = h->lperm;
+  const int sms = num_sms();
+  switch (epi) {
+    case PERS_EPI_SIM_DENSE: return conv_pers_launch<BN, 6, PERS_EPI_SIM_DENSE>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
+    case PERS_EPI_SIM_GMAX: return conv_pers_launch<BN, 6, PERS_EPI_SIM_GMAX>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
+    case PERS_EPI_SIM_JOIN: return conv_pers_launch<BN, 6, PERS_EPI_SIM_JOIN>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
+    case PERS_EPI_SIM_LGMAX: return conv_pers_launch<BN, 6, PERS_EPI_SIM_LGMAX>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
+    case PERS_EPI_SIM_LFILTER:
+      return conv_pers_launch<BN, 6, PERS_EPI_SIM_LFILTER>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
+    default: return conv_pers_launch<BN, 6, PERS_EPI_SIM_FILTER>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
   }
 }
 
@@ -1183,10 +1205,11 @@ __global__ void __launch_bounds__(NEAREST_THREADS) nearest_kernel(const float* _
 }  // namespace
 }  // namespace dirb
 
-// Grow the search workspace to `need` bytes.  Cached query maps point into it, so they are dropped when it moves.
-static int grow_ws(dirb200_index* h, size_t need) {
-  if (need > h->ws_bytes) h->tmaps.es.clear();
-  return grow_device(&h->ws, &h->ws_bytes, need);
+// Grow one of the index's workspaces (ws, jws, jws2, lws[i]) to `need` bytes.  Cached query maps may point into the
+// buffer, so they are dropped when it moves.
+static int grow_ws(dirb200_index* h, void** buf, size_t* bytes, size_t need) {
+  if (need > *bytes) h->tmaps.es.clear();
+  return grow_device(buf, bytes, need);
 }
 
 extern "C" {
@@ -1251,11 +1274,7 @@ int dirb200_index_check(dirb200_index* h) {
   h->stats[3] = static_cast<int64_t>(h->h_status[ST_RETRIES]);
   if (h->profile && h->pend.mark_i >= 2) {
     for (double& v : h->phase_ms) v = 0;
-    for (int i = 0; i + 1 < h->pend.mark_i && i < 9; ++i) {
-      float ms = 0;
-      cudaEventElapsedTime(&ms, h->ev[i], h->ev[i + 1]);
-      h->phase_ms[i] = ms;
-    }
+    for (int i = 0; i + 1 < h->pend.mark_i && i < 9; ++i) h->phase_ms[i] = h->ev.ms(i, i + 1);
   }
   DIRB_REQUIRE((err & 1ull) == 0, DIRB200_EOVERFLOW,
                "candidate buffer overflow not resolved after %d retry passes (raise option cand_cap)", h->retries);
@@ -1289,13 +1308,13 @@ int dirb200_index_last_profile(dirb200_index* h, double out9[9]) {
 int dirb200_index_destroy(dirb200_index* h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
-  for (auto e : h->ev) if (e) cudaEventDestroy(e);
+  h->ev.destroy();
+  h->jev.destroy();
+  h->lev.destroy();
   if (h->status_ev) cudaEventDestroy(h->status_ev);
   if (h->ws) cudaFree(h->ws);
-  for (auto e : h->jev) if (e) cudaEventDestroy(e);
   if (h->jws) cudaFree(h->jws);
   if (h->jws2) cudaFree(h->jws2);
-  for (auto e : h->lev) if (e) cudaEventDestroy(e);
   for (void* b : h->lws) if (b) cudaFree(b);
   if (h->res_sc) cudaFree(h->res_sc);
   if (h->res_ix) cudaFree(h->res_ix);
@@ -1303,12 +1322,6 @@ int dirb200_index_destroy(dirb200_index* h) {
   if (h->h_status) cudaFreeHost(h->h_status);
   delete h;
   return 0;
-}
-
-static void mark_phase(dirb200_index* h, cudaStream_t stream) {
-  if (!h->profile || h->pend.mark_i >= 10) return;
-  if (!h->ev[h->pend.mark_i]) cudaEventCreate(&h->ev[h->pend.mark_i]);
-  cudaEventRecord(h->ev[h->pend.mark_i++], stream);
 }
 
 // Phase 1: fp16 queries, seed pass, filter pass (+ device-gated retry passes), local k-th / k_shard-th candidate
@@ -1351,38 +1364,37 @@ static SearchSizes search_sizes(const dirb200_index* h, int k) {
   z.cap = (cap + 255) / 256 * 256;
   z.deep = k > DEEP_K;
   // survivors: the shallow finish sorts up to cap2 of them in shared memory; the deep one keeps 2k (at most N) in
-  // global memory, whole runs of DEEP_RUN
-  z.cap2 = z.deep ? static_cast<int>(ceil_div(std::min<int64_t>(2 * static_cast<int64_t>(k), N), DEEP_RUN) * DEEP_RUN)
-                  : (k > 256 ? 2048 : 1024);
+  // global memory for sort_runs_merge
+  z.cap2 = z.deep ? sort_run_cap(std::min<int64_t>(2 * static_cast<int64_t>(k), N)) : (k > 256 ? 2048 : 1024);
   return z;
 }
 
-// Byte offsets of the search workspace for Q queries.
-struct SearchLayout {
-  size_t q16 = 0, dense = 0, thr = 0, cnt = 0, cand = 0, kthk = 0, gates = 0, status = 0;
-  size_t surv_row = 0, surv_cnt = 0, surv_sc = 0, run_ix = 0, total = 0;
+// The search workspace of Q queries.
+struct SearchWs {
+  __half* q16;
+  float *dense, *thr, *kth_k;
+  int *cnt, *gates, *surv_cnt = nullptr;
+  unsigned long long *cand, *status;
+  SortScratch surv{};
+  size_t total;
 };
-static SearchLayout search_layout(const dirb200_index* h, const SearchSizes& z, int Q) {
-  SearchLayout L;
-  size_t off = 0;
-  auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-  const size_t q = static_cast<size_t>(Q);
-  L.q16 = carve(q * h->dim * 2);
-  L.dense = carve(q * z.S_ld * 4);
-  L.thr = carve(q * 4);
-  L.cnt = carve(q * 4);
-  L.cand = carve(q * z.cap * 8);
-  L.kthk = carve(q * 4);
-  L.gates = carve(8 * 4);
-  L.status = carve(ST_WORDS * 8);
+static SearchWs search_ws(void* base, const dirb200_index* h, const SearchSizes& z, int Q) {
+  Carver c(base);
+  SearchWs w;
+  w.q16 = c.take<__half>(static_cast<size_t>(Q) * h->dim);
+  w.dense = c.take<float>(static_cast<size_t>(Q) * z.S_ld);
+  w.thr = c.take<float>(Q);
+  w.cnt = c.take<int>(Q);
+  w.cand = c.take<unsigned long long>(static_cast<size_t>(Q) * z.cap);
+  w.kth_k = c.take<float>(Q);
+  w.gates = c.take<int>(8);
+  w.status = c.take<unsigned long long>(ST_WORDS);
   if (z.deep) {
-    L.surv_row = carve(q * z.cap2 * 4);
-    L.surv_cnt = carve(q * 4);
-    L.surv_sc = carve(q * z.cap2 * 8);
-    L.run_ix = carve(q * z.cap2 * 8);
+    w.surv = take_sort_scratch(c, Q, z.cap2);
+    w.surv_cnt = c.take<int>(Q);
   }
-  L.total = off;
-  return L;
+  w.total = c.used;
+  return w;
 }
 
 // Largest query block whose workspace fits option ws_budget (at least 1).  Launches with a grid row per query (the
@@ -1393,7 +1405,7 @@ static int search_max_queries(const dirb200_index* h, int k) {
   int lo = 1, hi = (z.small || z.deep) ? 65535 : (1 << 30);
   while (lo < hi) {
     const int mid = lo + (hi - lo + 1) / 2;
-    if (static_cast<double>(search_layout(h, z, mid).total) <= h->ws_budget) lo = mid; else hi = mid - 1;
+    if (static_cast<double>(search_ws(nullptr, h, z, mid).total) <= h->ws_budget) lo = mid; else hi = mid - 1;
   }
   return lo;
 }
@@ -1438,53 +1450,44 @@ static int search_begin_seed(dirb200_index* h, const float* q32, int Q, int k, i
   P.cap = z.cap;
   P.cap2 = z.cap2;
   P.band = band;
-  const SearchLayout L = search_layout(h, z, Q);
-  DIRB_TRY(grow_ws(h, L.total));
-  uint8_t* w = static_cast<uint8_t*>(h->ws);
-  __half* q16 = reinterpret_cast<__half*>(w + L.q16);
-  float* dense = reinterpret_cast<float*>(w + L.dense);
-  float* thr = reinterpret_cast<float*>(w + L.thr);
-  int* gates = reinterpret_cast<int*>(w + L.gates);
-  P.cnt = reinterpret_cast<int*>(w + L.cnt);
-  P.cand = reinterpret_cast<unsigned long long*>(w + L.cand);
-  P.kth_k = reinterpret_cast<float*>(w + L.kthk);
-  P.status = reinterpret_cast<unsigned long long*>(w + L.status);
-  if (z.deep) {
-    P.surv_row = reinterpret_cast<int*>(w + L.surv_row);
-    P.surv_cnt = reinterpret_cast<int*>(w + L.surv_cnt);
-    P.surv_sc = reinterpret_cast<double*>(w + L.surv_sc);
-    P.run_ix = reinterpret_cast<int64_t*>(w + L.run_ix);
-  }
+  DIRB_TRY(grow_ws(h, &h->ws, &h->ws_bytes, search_ws(nullptr, h, z, Q).total));
+  const SearchWs w = search_ws(h->ws, h, z, Q);
+  P.cnt = w.cnt;
+  P.cand = w.cand;
+  P.kth_k = w.kth_k;
+  P.status = w.status;
+  P.surv = w.surv;
+  P.surv_cnt = w.surv_cnt;
   const int D = h->dim;
   int* cnt = P.cnt;
 
-  mark_phase(h, stream);  // 0
+  if (h->profile) h->ev.mark(P.mark_i++, stream);  // 0
   // ---- 1. queries to fp16, counters / gates / status cleared
   {
     const int64_t n = static_cast<int64_t>(Q) * D;
     const int64_t threads = std::max<int64_t>(ceil_div(n, 4), std::max<int64_t>(Q, 8));
-    search_prep_kernel<<<static_cast<unsigned>(ceil_div(threads, 256)), 256, 0, stream>>>(q32, q16, n, cnt, Q, gates, 8, P.status);
+    search_prep_kernel<<<static_cast<unsigned>(ceil_div(threads, 256)), 256, 0, stream>>>(q32, w.q16, n, cnt, Q, w.gates, 8, P.status);
     count_launch();
   }
-  mark_phase(h, stream);  // 1: convert
+  if (h->profile) h->ev.mark(P.mark_i++, stream);  // 1: convert
   // ---- 2. seed pass over the first S rows
   {
     SimArgs a;
-    a.dense = dense;
+    a.dense = w.dense;
     a.dense_ld = S_ld;
-    DIRB_TRY(sim_gemm(h, use_gmax ? PERS_EPI_SIM_GMAX : PERS_EPI_SIM_DENSE, q16, Q, h->db16, S, D, a, stream));
-    mark_phase(h, stream);  // 2: seed GEMM
+    DIRB_TRY(sim_gemm(h, use_gmax ? PERS_EPI_SIM_GMAX : PERS_EPI_SIM_DENSE, w.q16, Q, h->db16, S, D, a, stream));
+    if (h->profile) h->ev.mark(P.mark_i++, stream);  // 2: seed GEMM
     const int n_vals = use_gmax ? static_cast<int>(ceil_div(S, 32)) : static_cast<int>(S);
     const int kk = static_cast<int>(std::min<int64_t>(k, n_vals));
     const int kk2 = seed2 ? static_cast<int>(std::min<int64_t>(k_shard, n_vals)) : 0;
-    kth_dense_kernel<<<Q, SEL_THREADS, 0, stream>>>(dense, S_ld, n_vals, kk, band, thr, kk2, seed2);
+    kth_dense_kernel<<<Q, SEL_THREADS, 0, stream>>>(w.dense, S_ld, n_vals, kk, band, w.thr, kk2, seed2);
     count_launch();
-    mark_phase(h, stream);  // 3: k-th of the seed scores
+    if (h->profile) h->ev.mark(P.mark_i++, stream);  // 3: k-th of the seed scores
   }
-  P.thr = thr;
-  P.dense = dense;
-  P.q16 = q16;
-  P.gates = gates;
+  P.thr = w.thr;
+  P.dense = w.dense;
+  P.q16 = w.q16;
+  P.gates = w.gates;
   P.S_ld = S_ld;
   P.small = small;
   P.ks = std::min<int>(k_shard, static_cast<int>(std::min<int64_t>(k, N)));
@@ -1526,13 +1529,13 @@ static int search_begin_filter(dirb200_index* h, cudaStream_t stream) {
       a.gate = gate_in;
       DIRB_TRY(sim_gemm(h, PERS_EPI_SIM_FILTER, q16, Q, h->db16, N, D, a, stream));
     }
-    if (r == 0) mark_phase(h, stream);  // 4: filter pass
+    if (r == 0 && h->profile) h->ev.mark(P.mark_i++, stream);  // 4: filter pass
     cand_kth_kernel<<<Q, SEL_THREADS, 0, stream>>>(cand, cnt, cap, k, ks, band, P.kth_k, sel_dev, thr, N, gate_in, gates + r,
                                                    r == h->retries ? 1 : 0, P.status);
     count_launch();
-    if (r == 0) mark_phase(h, stream);  // 5: candidate selection
+    if (r == 0 && h->profile) h->ev.mark(P.mark_i++, stream);  // 5: candidate selection
   }
-  mark_phase(h, stream);  // 6: gated retry passes (empty launches unless a list overflowed)
+  if (h->profile) h->ev.mark(P.mark_i++, stream);  // 6: gated retry passes (empty launches unless a list overflowed)
   DIRB_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1557,8 +1560,9 @@ static int post_status_copy(dirb200_index* h, cudaStream_t stream) {
   return 0;
 }
 
+// collect: wait for the search and raise its errors now (dirb200_index_check); otherwise the caller collects them.
 static int search_finish_impl(dirb200_index* h, const float* q32, const float* sel_dev, double* scores_dev, int64_t* idx_dev,
-                              cudaStream_t stream, const PeerX& px, unsigned long long* x_status) {
+                              cudaStream_t stream, const PeerX& px, unsigned long long* x_status, bool collect) {
   auto& P = h->pend;
   DIRB_REQUIRE(P.active, DIRB200_ESTATE, "dirb200_index_search_finish without a matching _begin");
   DIRB_CUDA(cudaSetDevice(h->device));
@@ -1578,39 +1582,29 @@ static int search_finish_impl(dirb200_index* h, const float* q32, const float* s
     h->stats[4] = launches_total() - P.launches0;
     return 0;
   }
-  if (P.surv_row != nullptr) {              // deep path, k > 1024 (never through peer memory: exchange windows hold k <= 1024)
+  if (P.surv.rows != nullptr) {             // deep path, k > 1024 (never through peer memory: exchange windows hold k <= 1024)
     DIRB_REQUIRE(px.world == 0, DIRB200_ENOTSUP, "peer-exchange search needs k <= 1024");
     const int64_t sms = num_sms();
     DIRB_CUDA(cudaMemsetAsync(P.surv_cnt, 0, static_cast<size_t>(Q) * 4, stream));
     const unsigned gc = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(8 * sms, Q), ceil_div(P.cap, 256))));
-    deep_compact_kernel<<<dim3(gc, Q), 256, 0, stream>>>(P.cand, P.cnt, P.cap, P.kth_k, sel_dev, P.band, P.surv_row, P.surv_cnt,
+    deep_compact_kernel<<<dim3(gc, Q), 256, 0, stream>>>(P.cand, P.cnt, P.cap, P.kth_k, sel_dev, P.band, P.surv.rows, P.surv_cnt,
                                                          cap2, P.status);
     count_launch();
-    mark_phase(h, stream);  // 7: survivor compaction
+    if (h->profile) h->ev.mark(P.mark_i++, stream);  // 7: survivor compaction
     const unsigned gr = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(32 * sms, Q), ceil_div(cap2, 8))));
-    deep_rescore_kernel<<<dim3(gr, Q), 256, 0, stream>>>(q32, h->db32, h->dim, P.surv_row, P.surv_cnt, cap2, P.surv_sc);
+    deep_rescore_kernel<<<dim3(gr, Q), 256, 0, stream>>>(q32, h->db32, h->dim, P.surv.rows, P.surv_cnt, cap2, P.surv.sc);
     count_launch();
-    mark_phase(h, stream);  // 8: exact re-scoring
-    const int runs = cap2 / DEEP_RUN;
-    deep_run_sort_kernel<<<dim3(runs, Q), FIN_THREADS, 0, stream>>>(P.surv_row, P.surv_cnt, cap2, h->offset, P.surv_sc, P.run_ix,
-                                                                    P.status);
-    count_launch();
-    const int64_t n = static_cast<int64_t>(Q) * k;
-    fill_empty_result_kernel<<<static_cast<unsigned>(ceil_div(n, 256)), 256, 0, stream>>>(scores_dev, idx_dev, n);
-    count_launch();
-    const int64_t elems = static_cast<int64_t>(runs) * std::min(DEEP_RUN, k);
-    merge_runs_kernel<<<dim3(static_cast<unsigned>(ceil_div(elems, 256)), Q), 256, 0, stream>>>(
-        P.surv_sc, P.run_ix, runs, DEEP_RUN, DEEP_RUN, cap2, P.surv_cnt, cap2, Q, k, scores_dev, idx_dev);
-    count_launch();
-    DIRB_CUDA(cudaGetLastError());
-    mark_phase(h, stream);  // 9: run sort + merge
+    if (h->profile) h->ev.mark(P.mark_i++, stream);  // 8: exact re-scoring
+    DIRB_TRY(sort_runs_merge(P.surv.rows, P.surv_cnt, cap2, P.surv.sc, P.surv.run_ix, Q, k, h->offset, P.status, scores_dev,
+                             idx_dev, stream));
+    if (h->profile) h->ev.mark(P.mark_i++, stream);  // 9: run sort + merge
   } else {
     const size_t smem = static_cast<size_t>(cap2) * 12;
     search_finish_kernel<<<Q, FIN_THREADS, smem, stream>>>(P.cand, P.cnt, P.cap, P.kth_k, sel_dev, P.band, q32, h->db32, h->dim,
                                                            cap2, h->offset, k, scores_dev, idx_dev, P.status, px);
     count_launch();
     DIRB_CUDA(cudaGetLastError());
-    mark_phase(h, stream);  // 7: survivors + exact re-scoring + sort
+    if (h->profile) h->ev.mark(P.mark_i++, stream);  // 7: survivors + exact re-scoring + sort
   }
   h->status_cap2 = cap2;
   h->status_band = P.band;
@@ -1618,14 +1612,14 @@ static int search_finish_impl(dirb200_index* h, const float* q32, const float* s
   h->stats[4] = launches_total() - P.launches0;
   if (px.world > 0) return 0;               // sharded search over peer memory: the merge (phase 3) can still raise error bits
   DIRB_TRY(post_status_copy(h, stream));
-  if (!h->deferred) return dirb200_index_check(h);
-  return 0;
+  return collect ? dirb200_index_check(h) : 0;
 }
 
 int dirb200_index_search_finish(dirb200_index* h, const float* q32, const float* sel_dev, double* scores_dev,
                                 int64_t* idx_dev, void* stream_) {
   DIRB_REQUIRE(h && q32 && sel_dev && scores_dev && idx_dev, DIRB200_EINVAL, "null argument");
-  return search_finish_impl(h, q32, sel_dev, scores_dev, idx_dev, static_cast<cudaStream_t>(stream_), PeerX{}, nullptr);
+  return search_finish_impl(h, q32, sel_dev, scores_dev, idx_dev, static_cast<cudaStream_t>(stream_), PeerX{}, nullptr,
+                            !h->deferred);
 }
 
 int dirb200_index_search_max_queries(dirb200_index* h, int k, int* q_max) {
@@ -1694,26 +1688,24 @@ int dirb200_index_rank_count(dirb200_index* h, const float* q32, int Q, const in
   const int64_t N = h->N;
   int cap = h->count_cap > 0 ? h->count_cap : 32768;
   cap = std::max(1024, (cap + 255) / 256 * 256);
-  size_t off = 0;
-  auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-  const size_t o_q16 = carve(static_cast<size_t>(Q) * D * 2);
-  const size_t o_thr = carve(static_cast<size_t>(Q) * 4);
-  const size_t o_cnt = carve(static_cast<size_t>(Q) * 4);
-  const size_t o_cand = carve(static_cast<size_t>(Q) * cap * 8);
-  const size_t o_gates = carve(8 * 4);
-  const size_t o_status = carve(ST_WORDS * 8);
-  const size_t o_over = carve(static_cast<size_t>(Q) * 4);
-  const size_t o_qlist = carve(static_cast<size_t>(Q) * 4);
-  DIRB_TRY(grow_ws(h, off));
-  uint8_t* w = static_cast<uint8_t*>(h->ws);
-  __half* q16 = reinterpret_cast<__half*>(w + o_q16);
-  float* thr = reinterpret_cast<float*>(w + o_thr);
-  int* cnt = reinterpret_cast<int*>(w + o_cnt);
-  unsigned long long* cand = reinterpret_cast<unsigned long long*>(w + o_cand);
-  int* gates = reinterpret_cast<int*>(w + o_gates);
-  unsigned long long* status = reinterpret_cast<unsigned long long*>(w + o_status);
-  int* q_over = reinterpret_cast<int*>(w + o_over);
-  int* q_list = reinterpret_cast<int*>(w + o_qlist);
+  __half* q16;
+  float* thr;
+  int *cnt, *gates, *q_over, *q_list;
+  unsigned long long *cand, *status;
+  auto layout = [&](void* base) {
+    Carver c(base);
+    q16 = c.take<__half>(static_cast<size_t>(Q) * D);
+    thr = c.take<float>(Q);
+    cnt = c.take<int>(Q);
+    cand = c.take<unsigned long long>(static_cast<size_t>(Q) * cap);
+    gates = c.take<int>(8);
+    status = c.take<unsigned long long>(ST_WORDS);
+    q_over = c.take<int>(Q);
+    q_list = c.take<int>(Q);
+    return c.used;
+  };
+  DIRB_TRY(grow_ws(h, &h->ws, &h->ws_bytes, layout(nullptr)));
+  layout(h->ws);
   {
     const int64_t n = static_cast<int64_t>(Q) * D;
     const int64_t threads = std::max<int64_t>(ceil_div(n, 4), std::max<int64_t>(Q, 8));
@@ -1788,7 +1780,7 @@ int dirb200_index_count_ge(dirb200_index* h, const float* q32, int Q, const int*
   h->pend.active = false;                        // shares the search workspace
   const int64_t launches0 = launches_total();
   const int cap = h->band_cap > 0 ? h->band_cap : (1 << 20);
-  DIRB_TRY(grow_ws(h, count_ge_ws_bytes(Q, T, cap)));
+  DIRB_TRY(grow_ws(h, &h->ws, &h->ws_bytes, count_ge_ws_bytes(Q, T, cap)));
   CountGeArgs a;
   a.q32 = q32; a.Q = Q;
   a.db32 = h->db32; a.N = h->N; a.offset = h->offset; a.D = h->dim;
@@ -1832,27 +1824,46 @@ struct JoinRun {
   cudaStream_t stream;
 };
 
-size_t join_filter_bytes(int M, int D, int cap, bool tri) {
-  const size_t m = static_cast<size_t>(M);
-  auto r = [](size_t b) { return (b + 255) / 256 * 256; };
-  return (tri ? 0 : r(m * D * 2)) + r(m * 4) + r(m * 4) + r(m * static_cast<size_t>(cap) * 8) + r(ST_WORDS * 8);
+// Filter pass of M rows (jws): their fp16 copy (none in a self-join, whose rows are the database's), thresholds, counts,
+// candidate lists and status.
+struct JoinFilterWs {
+  __half* a16;
+  float* thr;
+  int* cnt;
+  unsigned long long *cand, *status;
+  size_t total;
+};
+JoinFilterWs join_filter_ws(void* base, int M, int D, int cap, bool tri) {
+  Carver c(base);
+  JoinFilterWs w;
+  w.a16 = tri ? nullptr : c.take<__half>(static_cast<size_t>(M) * D);
+  w.thr = c.take<float>(M);
+  w.cnt = c.take<int>(M);
+  w.cand = c.take<unsigned long long>(static_cast<size_t>(M) * cap);
+  w.status = c.take<unsigned long long>(ST_WORDS);
+  w.total = c.used;
+  return w;
 }
-size_t join_sort_bytes(int nq, int K) {
-  const size_t m = static_cast<size_t>(nq);
-  const size_t cap2 = static_cast<size_t>(ceil_div(std::max(K, 1), DEEP_RUN) * DEEP_RUN);
-  auto r = [](size_t b) { return (b + 255) / 256 * 256; };
-  return r(m * cap2 * 4) + 2 * r(m * cap2 * 8) + 2 * r(m * static_cast<size_t>(std::max(K, 1)) * 8) + r(m * 4) + r(m * 8);
-}
-
-void join_mark(dirb200_index* h, int i, cudaStream_t stream) {
-  if (!h->profile) return;
-  if (!h->jev[i]) cudaEventCreate(&h->jev[i]);
-  cudaEventRecord(h->jev[i], stream);
-}
-void join_accumulate(dirb200_index* h, int i0, int i1, int slot) {
-  if (!h->profile) return;
-  float ms = 0;
-  if (cudaEventElapsedTime(&ms, h->jev[i0], h->jev[i1]) == cudaSuccess) h->join_ms[slot] += ms;
+// Re-scoring and sort buffers of nq rows of at most K candidates (jws2): the sorted top-K of each and its kept prefix.
+struct JoinSortWs {
+  SortScratch s;
+  double* out_sc;
+  int64_t* out_ix;
+  int* kept;
+  int64_t* off;
+  size_t total;
+};
+JoinSortWs join_sort_ws(void* base, int nq, int K) {
+  Carver c(base);
+  JoinSortWs w;
+  const size_t nk = static_cast<size_t>(nq) * std::max(K, 1);
+  w.s = take_sort_scratch(c, nq, sort_run_cap(std::max(K, 1)));
+  w.out_sc = c.take<double>(nk);
+  w.out_ix = c.take<int64_t>(nk);
+  w.kept = c.take<int>(nq);
+  w.off = c.take<int64_t>(nq);
+  w.total = c.used;
+  return w;
 }
 
 // Appends n more result entries, keeping the ones already there.
@@ -1892,17 +1903,14 @@ int join_rows(const JoinRun& R, int64_t r0, int M, int64_t col0, int cap) {
   unsigned long long* status = nullptr;
   size_t used = 0;
   for (int pass = 0;; ++pass) {
-    used = join_filter_bytes(M, D, cap, R.tri);
-    DIRB_TRY(grow_device(&h->jws, &h->jws_bytes, used));
-    uint8_t* w = static_cast<uint8_t*>(h->jws);
-    size_t off = 0;
-    auto carve = [&](size_t bytes) { uint8_t* p = w + off; off += (bytes + 255) / 256 * 256; return p; };
-    __half* a16 = R.tri ? const_cast<__half*>(h->db16) + r0 * D : reinterpret_cast<__half*>(carve(static_cast<size_t>(M) * D * 2));
-    float* thr = reinterpret_cast<float*>(carve(static_cast<size_t>(M) * 4));
-    cnt = reinterpret_cast<int*>(carve(static_cast<size_t>(M) * 4));
-    cand = reinterpret_cast<unsigned long long*>(carve(static_cast<size_t>(M) * cap * 8));
-    status = reinterpret_cast<unsigned long long*>(carve(ST_WORDS * 8));
-    join_mark(h, 0, stream);
+    used = join_filter_ws(nullptr, M, D, cap, R.tri).total;
+    DIRB_TRY(grow_ws(h, &h->jws, &h->jws_bytes, used));
+    const JoinFilterWs f = join_filter_ws(h->jws, M, D, cap, R.tri);
+    __half* a16 = R.tri ? const_cast<__half*>(h->db16) + r0 * D : f.a16;
+    cnt = f.cnt;
+    cand = f.cand;
+    status = f.status;
+    if (h->profile) h->jev.mark(0, stream);
     if (R.tri) {
       DIRB_CUDA(cudaMemsetAsync(cnt, 0, static_cast<size_t>(M) * 4, stream));
     } else {
@@ -1911,10 +1919,10 @@ int join_rows(const JoinRun& R, int64_t r0, int M, int64_t col0, int cap) {
       search_prep_kernel<<<static_cast<unsigned>(ceil_div(threads, 256)), 256, 0, stream>>>(a32, a16, n, cnt, M, nullptr, 0, status);
       count_launch();
     }
-    fill_f32_kernel<<<static_cast<unsigned>(ceil_div(M, 256)), 256, 0, stream>>>(thr, M, R.thr);
+    fill_f32_kernel<<<static_cast<unsigned>(ceil_div(M, 256)), 256, 0, stream>>>(f.thr, M, R.thr);
     count_launch();
     SimArgs a;
-    a.thr = thr;
+    a.thr = f.thr;
     a.cand = cand;
     a.cand_cnt = cnt;
     a.cand_cap = cap;
@@ -1922,16 +1930,17 @@ int join_rows(const JoinRun& R, int64_t r0, int M, int64_t col0, int cap) {
     const int64_t mt = ceil_div(M, 128), nt = ceil_div(ncols, 128);
     h->join_stats[3] += 1;
     h->join_stats[4] += R.tri ? mt * nt - mt * (mt - 1) / 2 : mt * nt;
-    join_mark(h, 1, stream);
+    if (h->profile) h->jev.mark(1, stream);
     DIRB_CUDA(cudaMemcpyAsync(cnt_h.data(), cnt, static_cast<size_t>(M) * 4, cudaMemcpyDeviceToHost, stream));
     DIRB_CUDA(cudaStreamSynchronize(stream));
-    join_accumulate(h, 0, 1, 0);
+    if (h->profile) h->join_ms[0] += h->jev.ms(0, 1);
     const int cmax = *std::max_element(cnt_h.begin(), cnt_h.end());
     if (cmax <= cap) break;
     // overflow: the counts are exact, so one re-run at capacity cmax captures every candidate (rule J6)
     DIRB_REQUIRE(pass == 0, DIRB200_EOVERFLOW, "candidate count changed between two filter passes");
     const int cap_new = static_cast<int>(std::min<int64_t>(ceil_div(cmax, 256) * 256, ncols));
-    if (join_filter_bytes(M, D, cap_new, R.tri) + join_sort_bytes(1, cmax) <= budget) {
+    const size_t sort1 = join_sort_ws(nullptr, 1, cmax).total;
+    if (join_filter_ws(nullptr, M, D, cap_new, R.tri).total + sort1 <= budget) {
       cap = cap_new;
       h->join_stats[2] += 1;
       continue;
@@ -1939,7 +1948,7 @@ int join_rows(const JoinRun& R, int64_t r0, int M, int64_t col0, int cap) {
     const int step = R.tri ? 128 : 1;           // a self-join block starts at a tile boundary
     DIRB_REQUIRE(M > step, DIRB200_EOVERFLOW,
                  "row %lld has %d candidates within eps16 of tau: %zu bytes of workspace needed, option ws_budget is %.0f",
-                 static_cast<long long>(r0), cmax, join_filter_bytes(1, D, cap_new, R.tri) + join_sort_bytes(1, cmax),
+                 static_cast<long long>(r0), cmax, join_filter_ws(nullptr, 1, D, cap_new, R.tri).total + sort1,
                  h->ws_budget);
     const int half = static_cast<int>(ceil_div(ceil_div(M, step), 2) * step);
     h->join_stats[2] += 1;
@@ -1953,42 +1962,34 @@ int join_rows(const JoinRun& R, int64_t r0, int M, int64_t col0, int cap) {
     int nq = 0, K = 0;
     while (q0 + nq < M && nq < 65535) {
       const int K2 = std::max(K, cnt_h[q0 + nq]);
-      if (nq > 0 && join_sort_bytes(nq + 1, K2) > sort_budget) break;
+      if (nq > 0 && join_sort_ws(nullptr, nq + 1, K2).total > sort_budget) break;
       K = K2;
       ++nq;
     }
-    DIRB_REQUIRE(join_sort_bytes(nq, K) <= sort_budget || nq > 1, DIRB200_EOVERFLOW,
+    DIRB_REQUIRE(join_sort_ws(nullptr, nq, K).total <= sort_budget || nq > 1, DIRB200_EOVERFLOW,
                  "row %lld has %d candidates within eps16 of tau: %zu bytes of workspace needed, option ws_budget is %.0f",
-                 static_cast<long long>(r0 + q0), K, used + join_sort_bytes(1, K), h->ws_budget);
+                 static_cast<long long>(r0 + q0), K, used + join_sort_ws(nullptr, 1, K).total, h->ws_budget);
     const int64_t base = h->res_off.back();
     if (K == 0) {
       for (int q = 0; q < nq; ++q) h->res_off.push_back(base);
       q0 += nq;
       continue;
     }
-    const int cap2 = static_cast<int>(ceil_div(K, DEEP_RUN) * DEEP_RUN);
-    DIRB_TRY(grow_device(&h->jws2, &h->jws2_bytes, join_sort_bytes(nq, K)));
-    uint8_t* w = static_cast<uint8_t*>(h->jws2);
-    size_t off = 0;
-    auto carve = [&](size_t bytes) { uint8_t* p = w + off; off += (bytes + 255) / 256 * 256; return p; };
-    int* rows = reinterpret_cast<int*>(carve(static_cast<size_t>(nq) * cap2 * 4));
-    double* sc = reinterpret_cast<double*>(carve(static_cast<size_t>(nq) * cap2 * 8));
-    int64_t* run_ix = reinterpret_cast<int64_t*>(carve(static_cast<size_t>(nq) * cap2 * 8));
-    double* out_sc = reinterpret_cast<double*>(carve(static_cast<size_t>(nq) * K * 8));
-    int64_t* out_ix = reinterpret_cast<int64_t*>(carve(static_cast<size_t>(nq) * K * 8));
-    int* kept = reinterpret_cast<int*>(carve(static_cast<size_t>(nq) * 4));
-    int64_t* off_d = reinterpret_cast<int64_t*>(carve(static_cast<size_t>(nq) * 8));
-    join_mark(h, 1, stream);
+    const int cap2 = sort_run_cap(K);
+    DIRB_TRY(grow_ws(h, &h->jws2, &h->jws2_bytes, join_sort_ws(nullptr, nq, K).total));
+    const JoinSortWs w = join_sort_ws(h->jws2, nq, K);
+    if (h->profile) h->jev.mark(1, stream);
     const int64_t sms = num_sms();
     const unsigned gr = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(32 * sms, nq), ceil_div(K, 8))));
-    join_rescore_kernel<<<dim3(gr, nq), 256, 0, stream>>>(cand, cnt, cap, q0, a32, h->db32, D, col0, cap2, rows, sc);
+    join_rescore_kernel<<<dim3(gr, nq), 256, 0, stream>>>(cand, cnt, cap, q0, a32, h->db32, D, col0, cap2, w.s.rows,
+                                                          w.s.sc);
     count_launch();
-    join_mark(h, 2, stream);
-    DIRB_TRY(sort_runs_merge(rows, cnt + q0, cap2, sc, run_ix, nq, K, status, out_sc, out_ix, stream));
-    join_kept_kernel<<<static_cast<unsigned>(ceil_div(nq, 256)), 256, 0, stream>>>(out_sc, K, cnt, q0, nq, R.tau, kept);
+    if (h->profile) h->jev.mark(2, stream);
+    DIRB_TRY(sort_runs_merge(w.s.rows, cnt + q0, cap2, w.s.sc, w.s.run_ix, nq, K, 0, status, w.out_sc, w.out_ix, stream));
+    join_kept_kernel<<<static_cast<unsigned>(ceil_div(nq, 256)), 256, 0, stream>>>(w.out_sc, K, cnt, q0, nq, R.tau, w.kept);
     count_launch();
     std::vector<int> kept_h(nq);
-    DIRB_CUDA(cudaMemcpyAsync(kept_h.data(), kept, static_cast<size_t>(nq) * 4, cudaMemcpyDeviceToHost, stream));
+    DIRB_CUDA(cudaMemcpyAsync(kept_h.data(), w.kept, static_cast<size_t>(nq) * 4, cudaMemcpyDeviceToHost, stream));
     DIRB_CUDA(cudaStreamSynchronize(stream));
     std::vector<int64_t> off_h(nq);
     int64_t t = base;
@@ -2001,16 +2002,18 @@ int join_rows(const JoinRun& R, int64_t r0, int M, int64_t col0, int cap) {
     }
     if (t > base) {
       DIRB_TRY(join_reserve(h, base, t - base, stream));
-      DIRB_CUDA(cudaMemcpyAsync(off_d, off_h.data(), static_cast<size_t>(nq) * 8, cudaMemcpyHostToDevice, stream));
+      DIRB_CUDA(cudaMemcpyAsync(w.off, off_h.data(), static_cast<size_t>(nq) * 8, cudaMemcpyHostToDevice, stream));
       const unsigned ge = static_cast<unsigned>(std::min<int64_t>(ceil_div(kmax, 256), 64));
-      join_emit_kernel<<<dim3(ge, nq), 256, 0, stream>>>(out_sc, out_ix, K, kept, off_d, h->offset, h->res_sc + base,
+      join_emit_kernel<<<dim3(ge, nq), 256, 0, stream>>>(w.out_sc, w.out_ix, K, w.kept, w.off, h->offset, h->res_sc + base,
                                                           h->res_ix + base);
       count_launch();
     }
-    join_mark(h, 3, stream);
+    if (h->profile) h->jev.mark(3, stream);
     DIRB_CUDA(cudaStreamSynchronize(stream));    // off_h / kept_h leave scope; the timing events are complete
-    join_accumulate(h, 1, 2, 1);
-    join_accumulate(h, 2, 3, 2);
+    if (h->profile) {
+      h->join_ms[1] += h->jev.ms(1, 2);
+      h->join_ms[2] += h->jev.ms(2, 3);
+    }
     DIRB_CUDA(cudaGetLastError());
     q0 += nq;
   }
@@ -2037,7 +2040,8 @@ int join_block_rows(const dirb200_index* h, int cap, bool tri) {
   int lo = step, hi = std::min(65535 / step * step, l2_rows);
   while (lo < hi) {
     const int mid = (lo + hi + step) / 2 / step * step;
-    if (static_cast<double>(join_filter_bytes(mid, h->dim, cap, tri)) <= 0.5 * h->ws_budget) lo = mid; else hi = mid - step;
+    if (static_cast<double>(join_filter_ws(nullptr, mid, h->dim, cap, tri).total) <= 0.5 * h->ws_budget) lo = mid;
+    else hi = mid - step;
   }
   return lo;
 }
@@ -2119,13 +2123,19 @@ int dirb200_index_nearest(dirb200_index* h, const float* q32_dev, int Q, int64_t
   const size_t per_q = static_cast<size_t>(D) * 2 + static_cast<size_t>(ng) * 4;
   const int64_t fit = static_cast<int64_t>(std::max(0.0, h->ws_budget - 4096.0) / static_cast<double>(per_q));
   const int qb = static_cast<int>(std::min<int64_t>(Q, std::max<int64_t>(128, fit / 128 * 128)));
-  const size_t o_g = (static_cast<size_t>(qb) * D * 2 + 255) & ~size_t(255);
-  const size_t o_st = (o_g + static_cast<size_t>(qb) * ng * 4 + 255) & ~size_t(255);
-  DIRB_TRY(grow_ws(h, o_st + 64));
-  uint8_t* w = static_cast<uint8_t*>(h->ws);
-  __half* q16 = reinterpret_cast<__half*>(w);
-  float* G = reinterpret_cast<float*>(w + o_g);
-  unsigned long long* st = reinterpret_cast<unsigned long long*>(w + o_st);
+  __half* q16;
+  float* G;
+  unsigned long long* st;
+  auto layout = [&](void* base) {
+    Carver c(base);
+    q16 = c.take<__half>(static_cast<size_t>(qb) * D);
+    G = c.take<float>(static_cast<size_t>(qb) * ng);
+    const size_t total = c.used + 64;          // the status words, the last piece, are not rounded up
+    st = c.take<unsigned long long>(8);
+    return total;
+  };
+  DIRB_TRY(grow_ws(h, &h->ws, &h->ws_bytes, layout(nullptr)));
+  layout(h->ws);
   DIRB_CUDA(cudaMemsetAsync(st, 0, 24, stream));
   for (int q0 = 0; q0 < Q; q0 += qb) {
     const int nq = std::min(qb, Q - q0);
@@ -2344,7 +2354,7 @@ int dirb200_index_search_sharded_phase(dirb200_index* h, dirb200_exchange* x, in
     return 0;
   }
   if (phase == 3)            // MIN over the shards + survivors + exact re-scoring -> ordered list into every peer's window
-    return search_finish_impl(h, q32, x->sel_local, nullptr, nullptr, stream, px, x->status);
+    return search_finish_impl(h, q32, x->sel_local, nullptr, nullptr, stream, px, x->status, false);
   DIRB_REQUIRE(phase == 4 && scores_dev && idx_dev, DIRB200_EINVAL, "phase is 1 .. 4 (4 needs the output buffers)");
   const int n = x->world * k;
   const int threads = std::min(1024, (n + 31) / 32 * 32);
@@ -2624,41 +2634,62 @@ __global__ void ivf_count_kernel(const int* __restrict__ cnt, int nq, long long*
 }  // namespace
 }  // namespace dirb
 
-// One grouped pass of the persistent kernel over a device-built tile table (see above).
-static int list_gemm(dirb200_index* h, int epi, const __half* q16, int64_t slots, const int4* tiles, int64_t n_tiles,
-                     const int* slot_q, const int64_t* gbase, const SimArgs& a, cudaStream_t stream) {
-  constexpr int BN = 128;
-  const int D = h->dim;
-  DIRB_REQUIRE(n_tiles < (int64_t(1) << 31) && slots < (int64_t(1) << 31), DIRB200_ENOTSUP, "too many tiles");
-  const CUtensorMap* tm;
-  DIRB_TRY(h->tmaps.get(q16, D, slots, 128, &tm));
-  const CUtensorMap a_copy = *tm;
-  DIRB_TRY(h->tmaps.get(h->l16, D, h->N, BN, &tm));
-  const CUtensorMap b_copy = *tm;
-  ConvPersParams p{};
-  p.a_spatial = 0;
-  p.taps = 1; p.kw_taps = 1; p.cin_blocks = D / 64; p.stride = 1; p.pad = 0;
-  p.tw = 128; p.th = 1; p.nb = 1; p.tiles_w = 1; p.tiles_h = 1;
-  p.M = static_cast<int>(slots);
-  p.N = static_cast<int>(h->N);
-  p.total_tiles = static_cast<int>(n_tiles);
-  p.dense = a.dense;
-  p.thr = a.thr; p.cand = a.cand; p.cand_cnt = a.cand_cnt; p.cand_cap = a.cand_cap;
-  p.tiles = tiles; p.slot_q = slot_q; p.perm = h->lperm; p.gbase = gbase;
-  if (epi == PERS_EPI_SIM_LGMAX)
-    return conv_pers_launch<BN, 6, PERS_EPI_SIM_LGMAX>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
-  return conv_pers_launch<BN, 6, PERS_EPI_SIM_LFILTER>(a_copy, b_copy, a_copy, a_copy, p, num_sms(), stream);
+// List search of nq queries probing np of K lists, part 1 (lws[0]): the (list, query) pair marks and per-query list
+// positions, the pair counts and offsets, and the table totals.  It survives the re-runs of part 2.
+struct ListPairWs {
+  int *M, *loc, *pc;
+  long long *qgroups, *tot;
+  int64_t *seg_off, *tile_off, *qgoff;
+  size_t total;
+};
+static ListPairWs list_pair_ws(void* base, int K, int nq, int np) {
+  Carver c(base);
+  ListPairWs w;
+  w.M = c.take<int>(static_cast<size_t>(K) * nq);
+  w.loc = c.take<int>(static_cast<size_t>(nq) * np);
+  w.qgroups = c.take<long long>(nq);
+  w.pc = c.take<int>(K);
+  w.seg_off = c.take<int64_t>(static_cast<size_t>(K) + 1);
+  w.tile_off = c.take<int64_t>(static_cast<size_t>(K) + 1);
+  w.qgoff = c.take<int64_t>(static_cast<size_t>(nq) + 1);
+  w.tot = c.take<long long>(LT_WORDS);
+  w.total = c.used;
+  return w;
 }
 
-static void list_mark(dirb200_index* h, int i, cudaStream_t stream) {
-  if (!h->profile) return;
-  if (!h->lev[i]) cudaEventCreate(&h->lev[i]);
-  cudaEventRecord(h->lev[i], stream);
-}
-
-static int lists_grow(dirb200_index* h, int i, size_t need) {
-  if (need > h->lws_bytes[i]) h->tmaps.es.clear();   // cached query maps may point into the buffer that moves
-  return grow_device(&h->lws[i], &h->lws_bytes[i], need);
+// Part 2 (lws[1]): the tile table, packed queries, group maxima, candidate lists and the finish's buffers.
+struct ListWs {
+  __half* q16;
+  int *slot_q, *cnt, *gates, *surv_cnt = nullptr;
+  int64_t* gbase;
+  int4* tiles;
+  float *G, *thr, *kth_k, *sel;
+  unsigned long long *cand, *status;
+  SortScratch surv{};
+  size_t total;
+};
+static ListWs list_ws(void* base, int64_t slots, int64_t n_tiles, int64_t groups, int D, int nq, int cap,
+                      const SearchSizes& z) {
+  Carver c(base);
+  ListWs w;
+  w.q16 = c.take<__half>(static_cast<size_t>(slots) * D);
+  w.slot_q = c.take<int>(slots);
+  w.gbase = c.take<int64_t>(slots);
+  w.tiles = c.take<int4>(n_tiles);
+  w.G = c.take<float>(groups);
+  w.thr = c.take<float>(nq);
+  w.cnt = c.take<int>(nq);
+  w.cand = c.take<unsigned long long>(static_cast<size_t>(nq) * cap);
+  w.kth_k = c.take<float>(nq);
+  w.sel = c.take<float>(nq);
+  w.gates = c.take<int>(8);
+  w.status = c.take<unsigned long long>(ST_WORDS);
+  if (z.deep) {
+    w.surv = take_sort_scratch(c, nq, z.cap2);
+    w.surv_cnt = c.take<int>(nq);
+  }
+  w.total = c.used;
+  return w;
 }
 
 // One block of nq queries.  *split = 1: the block's workspace does not fit option ws_budget (nothing was written).
@@ -2667,35 +2698,23 @@ static int lists_block(dirb200_index* h, const float* q32, int nq, int k, const 
   const int K = h->lists_k, D = h->dim;
   const int64_t N = h->N;
   *split = 0;
-  auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
   // ---- 1. pair counts and offsets
-  const size_t oM = 0, oLoc = oM + al(static_cast<size_t>(K) * nq * 4), oQg = oLoc + al(static_cast<size_t>(nq) * np * 4);
-  const size_t oPc = oQg + al(static_cast<size_t>(nq) * 8), oSeg = oPc + al(static_cast<size_t>(K) * 4);
-  const size_t oTo = oSeg + al(static_cast<size_t>(K + 1) * 8), oQgo = oTo + al(static_cast<size_t>(K + 1) * 8);
-  const size_t oTot = oQgo + al(static_cast<size_t>(nq + 1) * 8), bytesA = oTot + al(LT_WORDS * 8);
+  const size_t bytesA = list_pair_ws(nullptr, K, nq, np).total;
   if (nq > 1 && static_cast<double>(bytesA) > h->ws_budget) { *split = 1; return 0; }
-  DIRB_TRY(lists_grow(h, 0, bytesA));
-  uint8_t* wa = static_cast<uint8_t*>(h->lws[0]);
-  int* M = reinterpret_cast<int*>(wa + oM);
-  int* loc = reinterpret_cast<int*>(wa + oLoc);
-  long long* qgroups = reinterpret_cast<long long*>(wa + oQg);
-  int* pc = reinterpret_cast<int*>(wa + oPc);
-  int64_t* seg_off = reinterpret_cast<int64_t*>(wa + oSeg);
-  int64_t* tile_off = reinterpret_cast<int64_t*>(wa + oTo);
-  int64_t* qgoff = reinterpret_cast<int64_t*>(wa + oQgo);
-  long long* tot = reinterpret_cast<long long*>(wa + oTot);
-  list_mark(h, 0, stream);
-  DIRB_CUDA(cudaMemsetAsync(M, 0, static_cast<size_t>(K) * nq * 4, stream));
-  DIRB_CUDA(cudaMemsetAsync(tot, 0, LT_WORDS * 8, stream));
+  DIRB_TRY(grow_ws(h, &h->lws[0], &h->lws_bytes[0], bytesA));
+  const ListPairWs pw = list_pair_ws(h->lws[0], K, nq, np);
+  if (h->profile) h->lev.mark(0, stream);
+  DIRB_CUDA(cudaMemsetAsync(pw.M, 0, static_cast<size_t>(K) * nq * 4, stream));
+  DIRB_CUDA(cudaMemsetAsync(pw.tot, 0, LT_WORDS * 8, stream));
   const int64_t npairs = static_cast<int64_t>(nq) * np;
-  ivf_mark_kernel<<<static_cast<unsigned>(ceil_div(npairs, IVF_THREADS)), IVF_THREADS, 0, stream>>>(probes, nq, np, K, M, tot);
+  ivf_mark_kernel<<<static_cast<unsigned>(ceil_div(npairs, IVF_THREADS)), IVF_THREADS, 0, stream>>>(probes, nq, np, K, pw.M, pw.tot);
   ivf_query_groups_kernel<<<static_cast<unsigned>(ceil_div(nq, IVF_THREADS)), IVF_THREADS, 0, stream>>>(
-      probes, nq, np, K, h->lcell_off, loc, qgroups, tot);
-  ivf_list_count_kernel<<<K, IVF_THREADS, 0, stream>>>(M, nq, pc);
-  ivf_scan_kernel<<<1, IVF_SCAN, 0, stream>>>(pc, h->lcell_off, K, qgroups, nq, seg_off, tile_off, qgoff, tot);
+      probes, nq, np, K, h->lcell_off, pw.loc, pw.qgroups, pw.tot);
+  ivf_list_count_kernel<<<K, IVF_THREADS, 0, stream>>>(pw.M, nq, pw.pc);
+  ivf_scan_kernel<<<1, IVF_SCAN, 0, stream>>>(pw.pc, h->lcell_off, K, pw.qgroups, nq, pw.seg_off, pw.tile_off, pw.qgoff, pw.tot);
   count_launch(4);
   long long ht[LT_WORDS];
-  DIRB_CUDA(cudaMemcpyAsync(ht, tot, sizeof(ht), cudaMemcpyDeviceToHost, stream));
+  DIRB_CUDA(cudaMemcpyAsync(ht, pw.tot, sizeof(ht), cudaMemcpyDeviceToHost, stream));
   DIRB_CUDA(cudaStreamSynchronize(stream));
   DIRB_CUDA(cudaGetLastError());
   DIRB_REQUIRE((ht[LT_ERR] & 1) == 0, DIRB200_EINVAL, "a probe lies outside [0, %d)", K);
@@ -2707,66 +2726,49 @@ static int lists_block(dirb200_index* h, const float* q32, int nq, int k, const 
   const int cap2 = z.cap2;
   const float band = static_cast<float>(2.0 * h->eps16);
   for (int run = 0;; ++run) {
-    const size_t oQ16 = 0, oSq = al(static_cast<size_t>(slots) * D * 2), oGb = oSq + al(static_cast<size_t>(slots) * 4);
-    const size_t oTl = oGb + al(static_cast<size_t>(slots) * 8), oG = oTl + al(static_cast<size_t>(n_tiles) * 16);
-    const size_t oThr = oG + al(static_cast<size_t>(groups) * 4), oCnt = oThr + al(static_cast<size_t>(nq) * 4);
-    const size_t oCand = oCnt + al(static_cast<size_t>(nq) * 4), oKth = oCand + al(static_cast<size_t>(nq) * cap * 8);
-    const size_t oSel = oKth + al(static_cast<size_t>(nq) * 4), oGates = oSel + al(static_cast<size_t>(nq) * 4);
-    const size_t oSt = oGates + al(8 * 4), oSurv = oSt + al(ST_WORDS * 8);
-    size_t bytesB = oSurv;
-    const size_t surv_row = bytesB, surv_cnt = surv_row + al(static_cast<size_t>(nq) * cap2 * 4);
-    const size_t surv_sc = surv_cnt + al(static_cast<size_t>(nq) * 4), run_ix = surv_sc + al(static_cast<size_t>(nq) * cap2 * 8);
-    if (z.deep) bytesB = run_ix + al(static_cast<size_t>(nq) * cap2 * 8);
+    const size_t bytesB = list_ws(nullptr, slots, n_tiles, groups, D, nq, cap, z).total;
     if (static_cast<double>(bytesA + bytesB) > h->ws_budget) {
       if (nq > 1) { *split = 1; return 0; }
       DIRB_REQUIRE(false, DIRB200_EOVERFLOW,
                    "the list search of one query needs %.0f bytes (%d candidates) and option ws_budget is %.0f bytes",
                    static_cast<double>(bytesA + bytesB), cap, h->ws_budget);
     }
-    DIRB_TRY(lists_grow(h, 1, bytesB));
-    uint8_t* wb = static_cast<uint8_t*>(h->lws[1]);
-    __half* q16 = reinterpret_cast<__half*>(wb + oQ16);
-    int* slot_q = reinterpret_cast<int*>(wb + oSq);
-    int64_t* gbase = reinterpret_cast<int64_t*>(wb + oGb);
-    int4* tiles = reinterpret_cast<int4*>(wb + oTl);
-    float* G = reinterpret_cast<float*>(wb + oG);
-    float* thr = reinterpret_cast<float*>(wb + oThr);
-    int* cnt = reinterpret_cast<int*>(wb + oCnt);
-    unsigned long long* cand = reinterpret_cast<unsigned long long*>(wb + oCand);
-    float* kth_k = reinterpret_cast<float*>(wb + oKth);
-    float* sel = reinterpret_cast<float*>(wb + oSel);
-    int* gates = reinterpret_cast<int*>(wb + oGates);
-    unsigned long long* status = reinterpret_cast<unsigned long long*>(wb + oSt);
-    if (run > 0) list_mark(h, 0, stream);
-    ivf_list_fill_kernel<<<K, IVF_THREADS, 0, stream>>>(M, nq, np, pc, h->lcell_off, seg_off, tile_off, qgoff, loc, slot_q, gbase,
-                                                         tiles);
+    DIRB_TRY(grow_ws(h, &h->lws[1], &h->lws_bytes[1], bytesB));
+    const ListWs w = list_ws(h->lws[1], slots, n_tiles, groups, D, nq, cap, z);
+    if (run > 0 && h->profile) h->lev.mark(0, stream);
+    ivf_list_fill_kernel<<<K, IVF_THREADS, 0, stream>>>(pw.M, nq, np, pw.pc, h->lcell_off, pw.seg_off, pw.tile_off, pw.qgoff,
+                                                         pw.loc, w.slot_q, w.gbase, w.tiles);
     const int64_t packs = std::max<int64_t>(slots * (D / 4), nq);
-    ivf_pack_kernel<<<static_cast<unsigned>(ceil_div(packs, IVF_THREADS)), IVF_THREADS, 0, stream>>>(q32, D, slot_q, slots, q16, cnt,
-                                                                                                     nq);
-    DIRB_CUDA(cudaMemsetAsync(gates, 0, 8 * 4, stream));
-    DIRB_CUDA(cudaMemsetAsync(status, 0, ST_WORDS * 8, stream));
-    DIRB_CUDA(cudaMemsetAsync(tot + LT_MAXCNT, 0, 16, stream));
+    ivf_pack_kernel<<<static_cast<unsigned>(ceil_div(packs, IVF_THREADS)), IVF_THREADS, 0, stream>>>(q32, D, w.slot_q, slots,
+                                                                                                     w.q16, w.cnt, nq);
+    DIRB_CUDA(cudaMemsetAsync(w.gates, 0, 8 * 4, stream));
+    DIRB_CUDA(cudaMemsetAsync(w.status, 0, ST_WORDS * 8, stream));
+    DIRB_CUDA(cudaMemsetAsync(pw.tot + LT_MAXCNT, 0, 16, stream));
     count_launch(2);
-    list_mark(h, 1, stream);
+    if (h->profile) h->lev.mark(1, stream);
     SimArgs a;
+    a.tiles = w.tiles;
+    a.n_tiles = n_tiles;
+    a.slot_q = w.slot_q;
+    a.gbase = w.gbase;
     if (n_tiles > 0) {
-      a.dense = G;
-      DIRB_TRY(list_gemm(h, PERS_EPI_SIM_LGMAX, q16, slots, tiles, n_tiles, slot_q, gbase, a, stream));
+      a.dense = w.G;
+      DIRB_TRY(sim_gemm(h, PERS_EPI_SIM_LGMAX, w.q16, slots, h->l16, N, D, a, stream));
     }
-    ivf_seed_kernel<<<nq, SEL_THREADS, 0, stream>>>(G, qgoff, k, band, thr);
+    ivf_seed_kernel<<<nq, SEL_THREADS, 0, stream>>>(w.G, pw.qgoff, k, band, w.thr);
     count_launch();
-    list_mark(h, 2, stream);
+    if (h->profile) h->lev.mark(2, stream);
     if (n_tiles > 0) {
-      a = SimArgs();
-      a.thr = thr;
-      a.cand = cand;
-      a.cand_cnt = cnt;
+      a.dense = nullptr;
+      a.thr = w.thr;
+      a.cand = w.cand;
+      a.cand_cnt = w.cnt;
       a.cand_cap = cap;
-      DIRB_TRY(list_gemm(h, PERS_EPI_SIM_LFILTER, q16, slots, tiles, n_tiles, slot_q, gbase, a, stream));
+      DIRB_TRY(sim_gemm(h, PERS_EPI_SIM_LFILTER, w.q16, slots, h->l16, N, D, a, stream));
     }
-    ivf_count_kernel<<<static_cast<unsigned>(ceil_div(nq, IVF_THREADS)), IVF_THREADS, 0, stream>>>(cnt, nq, tot);
+    ivf_count_kernel<<<static_cast<unsigned>(ceil_div(nq, IVF_THREADS)), IVF_THREADS, 0, stream>>>(w.cnt, nq, pw.tot);
     count_launch();
-    DIRB_CUDA(cudaMemcpyAsync(ht + LT_MAXCNT, tot + LT_MAXCNT, 16, cudaMemcpyDeviceToHost, stream));
+    DIRB_CUDA(cudaMemcpyAsync(ht + LT_MAXCNT, pw.tot + LT_MAXCNT, 16, cudaMemcpyDeviceToHost, stream));
     DIRB_CUDA(cudaStreamSynchronize(stream));
     DIRB_CUDA(cudaGetLastError());
     if (ht[LT_MAXCNT] > cap) {               // rule I6: run the block again with room for every match
@@ -2776,9 +2778,10 @@ static int lists_block(dirb200_index* h, const float* q32, int nq, int k, const 
       ++h->lists_stats[5];
       continue;
     }
-    cand_kth_kernel<<<nq, SEL_THREADS, 0, stream>>>(cand, cnt, cap, k, k, band, kth_k, sel, thr, N, nullptr, gates, 1, status);
+    cand_kth_kernel<<<nq, SEL_THREADS, 0, stream>>>(w.cand, w.cnt, cap, k, k, band, w.kth_k, w.sel, w.thr, N, nullptr, w.gates,
+                                                    1, w.status);
     count_launch();
-    list_mark(h, 3, stream);
+    if (h->profile) h->lev.mark(3, stream);
     auto& P = h->pend;
     P = dirb200_index::Pending();
     P.active = true;
@@ -2787,36 +2790,24 @@ static int lists_block(dirb200_index* h, const float* q32, int nq, int k, const 
     P.cap = cap;
     P.cap2 = cap2;
     P.band = band;
-    P.cnt = cnt;
-    P.cand = cand;
-    P.status = status;
-    P.kth_k = kth_k;
-    P.sel_dev = sel;
+    P.cnt = w.cnt;
+    P.cand = w.cand;
+    P.status = w.status;
+    P.kth_k = w.kth_k;
+    P.sel_dev = w.sel;
     P.launches0 = launches_total();
-    if (z.deep) {
-      P.surv_row = reinterpret_cast<int*>(wb + surv_row);
-      P.surv_cnt = reinterpret_cast<int*>(wb + surv_cnt);
-      P.surv_sc = reinterpret_cast<double*>(wb + surv_sc);
-      P.run_ix = reinterpret_cast<int64_t*>(wb + run_ix);
-    }
-    const int deferred = h->deferred;
-    h->deferred = 0;                          // the list search always collects its status
-    const int rc = search_finish_impl(h, q32, sel, out_sc, out_ix, stream, PeerX{}, nullptr);
-    h->deferred = deferred;
-    DIRB_TRY(rc);
-    list_mark(h, 4, stream);
+    P.surv = w.surv;
+    P.surv_cnt = w.surv_cnt;
+    DIRB_TRY(search_finish_impl(h, q32, w.sel, out_sc, out_ix, stream, PeerX{}, nullptr, true));
+    if (h->profile) h->lev.mark(4, stream);
     h->lists_stats[0] += ht[LT_PAIRS];
     h->lists_stats[1] += slots;
     h->lists_stats[2] += n_tiles;
     h->lists_stats[3] += ht[LT_ROWS];
     h->lists_stats[4] += ht[LT_CAND];
     if (h->profile) {
-      DIRB_CUDA(cudaEventSynchronize(h->lev[4]));
-      for (int i = 0; i < 4; ++i) {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, h->lev[i], h->lev[i + 1]);
-        h->lists_ms[i] += ms;
-      }
+      DIRB_CUDA(cudaEventSynchronize(h->lev.ev[4]));
+      for (int i = 0; i < 4; ++i) h->lists_ms[i] += h->lev.ms(i, i + 1);
     }
     return 0;
   }
