@@ -152,6 +152,13 @@ SIGNATURES = {
     "dirb200_kmeans_update": (i32, [p, i64, i32, p, p, i32, p, p, C.POINTER(i64), p]),
     "dirb200_kmeans_pp_workspace_bytes": (C.c_size_t, [i64, i32]),
     "dirb200_kmeans_pp": (i32, [p, i64, i32, i64, p, i32, p, p, p]),
+    # product quantisation of the inverted lists: codeword assignment / encoding, codebook update, ADC tables, and
+    # the scan, selection and exact refinement of one query block
+    "dirb200_pq_assign": (i32, [p, i64, i32, p, p, p, i32, p, i32, p]),
+    "dirb200_pq_update": (i32, [p, i64, i32, p, p, p, i32, p, p, p]),
+    "dirb200_pq_tables": (i32, [p, i32, i32, p, i32, p, p]),
+    "dirb200_pq_search_ws_bytes": (C.c_size_t, [i32, i64, i32]),
+    "dirb200_pq_search": (i32, [p, i32, i32, p, i32, p, p, i32, p, p, p, p, i64, p, i32, i32, p, p, p, p, p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -434,11 +434,22 @@ def _aps_from_ivf(db, qdescs, bdescs, params):
         offs.append(offs[-1] + len(r))
     rows = np.concatenate(rows) if rows else np.zeros(0, np.int64)
     flags = np.concatenate(flags) if flags else np.zeros(0, np.uint8)
-    index = IVFIndex.train(bd, params["n_lists"], seed=params.get("seed", 0))
-    try:
-        inside, sc, rank = index.rank_counts(qd, np.array(offs, np.int64), rows, flags, params["nprobe"])
-    finally:
-        index.close()
+    if params.get("pq"):
+        from .ivfpq import IVFPQIndex
+        index = IVFPQIndex.train(bd, params["n_lists"], params["pq"], seed=params.get("seed", 0))
+        exact = ops.Index(bd)
+        try:
+            inside, sc, rank = index.rank_counts(qd, np.array(offs, np.int64), rows, flags, params["nprobe"],
+                                                 refine=params.get("refine"), exact=exact)
+        finally:
+            exact.close()
+            index.close()
+    else:
+        index = IVFIndex.train(bd, params["n_lists"], seed=params.get("seed", 0))
+        try:
+            inside, sc, rank = index.rank_counts(qd, np.array(offs, np.int64), rows, flags, params["nprobe"])
+        finally:
+            index.close()
     inside, sc, rank = inside.cpu().numpy(), sc.cpu().numpy(), rank.cpu().numpy()
     return [db.eval_query_AP_from_truncated_counts(q, rows[offs[q]:offs[q + 1]], inside[offs[q]:offs[q + 1]],
                                                    sc[offs[q]:offs[q + 1]], rank[offs[q]:offs[q + 1]])
@@ -458,6 +469,23 @@ def ivf_params(values):
     if out["nprobe"] > out["n_lists"]:
         raise ValueError("--ivf: NPROBE must not exceed NLIST (got %d > %d)" % (out["nprobe"], out["n_lists"]))
     return dict(out, seed=0)
+
+
+def pq_params(ivf, pq, refine):
+    """--pq M [--refine R] on top of --ivf -> the `pq` / `refine` entries of eval_model's `ivf` dict (M one of 8, 16,
+    32, 64, 128; R an integer >= 1, default 400)."""
+    if pq is None:
+        if refine is not None:
+            raise ValueError("--refine needs --pq")
+        return ivf
+    if ivf is None:
+        raise ValueError("--pq needs --ivf")
+    from .ivfpq import MS, RANK_REFINE
+    if pq not in MS:
+        raise ValueError("--pq: M must be one of %s (got %r)" % (MS, pq))
+    if refine is not None and refine < 1:
+        raise ValueError("--refine: R must be an integer >= 1 (got %r)" % (refine,))
+    return dict(ivf, pq=pq, refine=RANK_REFINE if refine is None else refine)
 
 
 def diffusion_params(values):
@@ -494,7 +522,9 @@ def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=Non
     with relevance lists are graded that way (NotImplementedError otherwise).
     ivf (extension): dict(n_lists=..., nprobe=..., seed=0): inverted-file ranking (rule I7): k-means lists of the
     database rows after whitening and alpha-DBA, queries probed after alpha-QE (whose own search stays exact); relevance
-    lists only (NotImplementedError otherwise), not together with diffusion (ValueError).
+    lists only (NotImplementedError otherwise), not together with diffusion (ValueError).  With pq=M (and refine=R,
+    default 400) the lists hold product-quantisation codes and the ranking is rule P8's: the best R probed rows by ADC
+    score first, in exact order, then every other row.
     Ranking: datasets with relevance lists (Oxford/Paris style) are graded from GPU rank counts and label datasets
     from GPU threshold counts + the exact top-100 - no Q x N score matrix, no host argsort; dense_scores=True
     (extension) forces the literal matmul + per-query sort of the reference; rank_topk > 0 (extension) grades
@@ -752,11 +782,16 @@ def test_dir_main(argv=None):
     parser.add_argument("--ivf", type=float, nargs="+", metavar="NLIST NPROBE",
                         help="(extension) rank by an inverted file: k-means lists of the database (NLIST centres, "
                              "k-means++ seed 0); each query's NPROBE best lists first, in exact order, then the other rows")
+    parser.add_argument("--pq", type=int, default=None, metavar="M",
+                        help="(extension, with --ivf) product-quantisation codes of M bytes per row in the lists: each "
+                             "query's best R probed rows by ADC score first, in exact order, then the other rows")
+    parser.add_argument("--refine", type=int, default=None, metavar="R",
+                        help="(extension, with --pq) rows re-ranked exactly per query (default 400)")
     args = parser.parse_args(argv)
     try:
         if args.ivf is not None and args.diffusion is not None:
             raise ValueError("--ivf and --diffusion are two rankings: choose one")
-        ivf = ivf_params(args.ivf) if args.ivf is not None else None
+        ivf = pq_params(ivf_params(args.ivf) if args.ivf is not None else None, args.pq, args.refine)
         diffusion = diffusion_params(args.diffusion) if args.diffusion is not None else None
         if args.diffusion_truncate is not None:
             if diffusion is None:

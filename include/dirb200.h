@@ -596,6 +596,33 @@ size_t dirb200_kmeans_pp_workspace_bytes(int64_t n, int k);
 int dirb200_kmeans_pp(const float* x32_dev, int64_t n, int d, int64_t first, const double* u_host, int k, void* ws_dev,
                       int64_t* chosen_dev, void* stream);
 
+/* Product quantisation of the inverted lists (DESIGN.md section 4.11, rules P1-P8).  D % 64 == 0, M in {8, 16, 32, 64,
+ * 128} dividing D with D / M <= 256 (else DIRB200_ENOTSUP).  Codebooks are [M][256][D / M] fp32; a row's residual is
+ * fl32(x - centres_dev[labels_dev[row]]).  None of these synchronises the stream.
+ * Rule P4: codes_dev = the nearest codeword of each (row, sub-space), row-major [n][M] (m_major = 0) or [M][n]. */
+int dirb200_pq_assign(const float* x_dev, int64_t n, int D, const int64_t* labels_dev, const float* centres_dev,
+                      const float* codebooks_dev, int M, uint8_t* codes_dev, int m_major, void* stream);
+/* Rule P3's update from the m-major codes of dirb200_pq_assign: codeword j of sub-space m = fl32(s / count), s the
+ * sequential fp64 sum of its members' residuals in row order; a codeword without members keeps its value.
+ * *empty_dev (device int64) = codewords without members. */
+int dirb200_pq_update(const float* x_dev, int64_t n, int D, const int64_t* labels_dev, const float* centres_dev,
+                      const uint8_t* codes_dev, int M, float* codebooks_dev, int64_t* empty_dev, void* stream);
+/* Rule P5's tables: tables_dev [Q][M][256] = fl32(sum over t ascending of q_{m,t} C_m[j][t]) in fp64, no FMA. */
+int dirb200_pq_tables(const float* q_dev, int Q, int D, const float* codebooks_dev, int M, float* tables_dev,
+                      void* stream);
+/* Rules P5-P7 for one block of Q <= 65535 queries: the ADC scores of the rows of each query's probes (probes_dev /
+ * probe_scores_dev [Q][nprobe], the exact centre scores), the first min(R, |R(q)|) in (a desc, row asc) order, and
+ * their first k (k <= R) in (e desc, row asc) order -> out_scores fp64 / out_rows int64 [Q][k], padded (-inf, -1).
+ * codes_dev [N][M] and perm_dev [N] are in list order, list_off_dev [K + 1] the lists' offsets, qoff_dev [Q + 1] the
+ * offsets of the queries' probed rows in the block (qoff_dev[Q] = total).  rows: the [N][D] fp32 rows, device memory
+ * or pinned host memory (read in place; pageable memory is DIRB200_EINVAL).  ms: null, or 3 doubles receiving the
+ * milliseconds of the scan, the selection and the refinement (then the stream is synchronised). */
+size_t dirb200_pq_search_ws_bytes(int Q, int64_t total, int R);
+int dirb200_pq_search(const float* q_dev, int Q, int D, const float* tables_dev, int M, const int64_t* probes_dev,
+                      const double* probe_scores_dev, int nprobe, const uint8_t* codes_dev, const int64_t* perm_dev,
+                      const int64_t* list_off_dev, const int64_t* qoff_dev, int64_t total, const float* rows, int R,
+                      int k, void* ws_dev, double* out_scores, int64_t* out_rows, double* ms, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
