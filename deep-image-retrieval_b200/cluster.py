@@ -16,24 +16,11 @@ import json
 import numpy as np
 import torch
 
-from . import lib, ops
-from .duplicates import _device, _rows, add_input_args, check_input_args, load_input
+from . import inputs, lib, ops
+from .duplicates import add_input_args, check_input_args, load_input
 
-NORM_SLACK = 1e-3          # what ops.Index accepts as unit norm
 MAX_ROWS = (1 << 29) - 1   # k-means++ weights are up to 2^34 units of 2^-32 each; their int64 total holds 2^29 rows
 INITS = ("k-means++", "random")
-
-
-def _ws(nbytes, device):
-    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
-
-
-def _check_unit(x, name):
-    if x.shape[0]:
-        nrm = torch.linalg.vector_norm(x, dim=1)
-        worst = float((nrm - 1.0).abs().max())
-        if not worst <= NORM_SLACK:
-            raise ValueError("%s rows must be unit-norm (largest |norm - 1| is %.4g)" % (name, worst))
 
 
 NEAREST_MAX_K = 16384      # measured on an H100 (results/h100_kmeans.json): nearest() beats search(X, 1) up to 16384 centres
@@ -66,7 +53,7 @@ def kmeans_pp_rows(x, k, seed):
     first = int(rs.randint(n))
     u = np.ascontiguousarray(rs.random_sample(k - 1), dtype=np.float64)
     chosen = torch.empty(k, dtype=torch.int64, device=x.device)
-    ws = _ws(lib.raw("dirb200_kmeans_pp_workspace_bytes")(n, k), x.device)
+    ws = ops.workspace(lib.raw("dirb200_kmeans_pp_workspace_bytes")(n, k), x.device)
     lib.call("dirb200_kmeans_pp", ops._ptr(x), n, d, first, u.ctypes.data_as(C.c_void_p), k, ops._ptr(ws), ops._ptr(chosen),
              ops._stream())
     rows = chosen.cpu().numpy()
@@ -95,19 +82,15 @@ class SphericalKMeans:
         self.seed = seed
 
     def _params(self, n, d):
-        k = self.n_clusters
-        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or k < 1:
-            raise ValueError("n_clusters must be an integer >= 1 (got %r)" % (k,))
+        k = inputs.check_int(self.n_clusters, "n_clusters")
         if k > n:
             raise ValueError("n_clusters = %d exceeds the number of rows (%d)" % (k, n))
         if n > MAX_ROWS:
             raise ValueError("at most %d rows can be clustered (got %d)" % (MAX_ROWS, n))
         if d % 64:
             raise ValueError("the descriptor dimension must be a multiple of 64 (got %d)" % d)
-        m = self.max_iter
-        if isinstance(m, bool) or not isinstance(m, (int, np.integer)) or m < 0:
-            raise ValueError("max_iter must be an integer >= 0 (got %r)" % (m,))
-        return int(k)
+        inputs.check_int(self.max_iter, "max_iter", 0)
+        return k
 
     def _initial_centres(self, x, k):
         n, d = x.shape
@@ -120,23 +103,23 @@ class SphericalKMeans:
             else:
                 raise ValueError("init must be one of %s or a (K, D) array (got %r)" % (INITS, init))
             return x[torch.from_numpy(np.asarray(rows, np.int64)).to(x.device)].contiguous()
-        c = _rows(init, x.device, "init")
+        c = inputs.rows(init, x.device, "init")
         if tuple(c.shape) != (k, d):
             raise ValueError("init must have shape (%d, %d) (got %s)" % (k, d, tuple(c.shape)))
-        _check_unit(c, "init")
+        inputs.check_unit(c, "init")
         return c.clone()
 
     def fit(self, X, device=None):
         """X: (N, D) unit descriptors - a CUDA fp32 tensor, a host array / tensor / memmap or a DescriptorStore."""
-        x = _rows(X, _device(device), "X")
+        x = inputs.rows(X, device, "X")
         n, d = x.shape
         k = self._params(n, d)
-        _check_unit(x, "X")
+        inputs.check_unit(x, "X")
         centres = self._initial_centres(x, k)
         dev = x.device
         counts = torch.empty(k, dtype=torch.int32, device=dev)
-        ws_stats = _ws(lib.raw("dirb200_kmeans_stats_workspace_bytes")(n, k), dev)
-        ws_upd = _ws(lib.raw("dirb200_kmeans_update_workspace_bytes")(n, k, d), dev)
+        ws_stats = ops.workspace(lib.raw("dirb200_kmeans_stats_workspace_bytes")(n, k), dev)
+        ws_upd = ops.workspace(lib.raw("dirb200_kmeans_update_workspace_bytes")(n, k, d), dev)
         ws_rel = None
         out = (C.c_int64 * 3)()
         one = C.c_int64()
@@ -151,7 +134,7 @@ class SphericalKMeans:
                 break
             if empty:
                 if ws_rel is None:
-                    ws_rel = _ws(lib.raw("dirb200_kmeans_relocate_workspace_bytes")(n), dev)
+                    ws_rel = ops.workspace(lib.raw("dirb200_kmeans_relocate_workspace_bytes")(n), dev)
                 lib.call("dirb200_kmeans_relocate", ops._ptr(labels), ops._ptr(scores), n, k, ops._ptr(counts),
                          ops._ptr(ws_rel), C.byref(one), ops._stream())
                 stats["relocations"] += one.value
@@ -172,10 +155,10 @@ class SphericalKMeans:
         """Rule K2 against the fitted centres -> labels int64 (N,) (CUDA)."""
         if not hasattr(self, "cluster_centers_"):
             raise ValueError("fit() first")
-        x = _rows(X, self.cluster_centers_.device if device is None else torch.device(device), "X")
+        x = inputs.rows(X, self.cluster_centers_.device if device is None else torch.device(device), "X")
         if x.shape[1] != self.cluster_centers_.shape[1]:
             raise ValueError("X has dimension %d, the centres %d" % (x.shape[1], self.cluster_centers_.shape[1]))
-        _check_unit(x, "X")
+        inputs.check_unit(x, "X")
         if x.shape[0] == 0:
             return torch.empty(0, dtype=torch.int64, device=x.device)
         return assign(x, self.cluster_centers_.to(x.device))[0]

@@ -14,7 +14,7 @@ from collections import OrderedDict
 import numpy as np
 import torch
 
-from . import ops
+from . import inputs, ops
 
 
 def typename(x):
@@ -28,23 +28,13 @@ def tonumpy(x):
     return x
 
 
-def _dev():
-    return torch.device("cuda", torch.cuda.current_device())
-
-
-def _to_dev_f32(x):
-    if typename(x) == torch.__name__:
-        return x.to(_dev(), torch.float32).contiguous()
-    return torch.from_numpy(np.ascontiguousarray(np.asarray(x, dtype=np.float32))).to(_dev())
-
-
 def matmul(A, B):
     """scores = A . B^T as a host ndarray (common.py:30-38); fp64-accumulated on the GPU, fp32 out."""
     if typename(A) == np.__name__:
         B = tonumpy(B)
     elif typename(B) != torch.__name__:
         raise TypeError("matrices must be either numpy or torch type")
-    return ops.scores_exact(_to_dev_f32(A), _to_dev_f32(B)).cpu().numpy()
+    return ops.scores_exact(inputs.rows(A), inputs.rows(B)).cpu().numpy()
 
 
 def pool(x, pooling="mean", gemp=3):
@@ -53,7 +43,7 @@ def pool(x, pooling="mean", gemp=3):
         return x[0]
     if pooling not in ("mean", "gem"):
         raise ValueError("Bad pooling mode: " + str(pooling))
-    return ops.pool_scales([_to_dev_f32(v) for v in x], pooling, gemp, l2=False)
+    return ops.pool_scales([inputs.rows(v) for v in x], pooling, gemp, l2=False)
 
 
 def torch_set_gpu(gpus, seed=None, randomize=True):
@@ -159,23 +149,23 @@ def _pca_arrays(pca, whitenp, whitenv, whitenm, use_sklearn):
         comp = np.asarray(pca["W"], dtype=np.float64).T
         mean = np.asarray(pca["means"], dtype=np.float64)
         cs = None
-    f = lambda a: None if a is None else torch.from_numpy(np.ascontiguousarray(a.astype(np.float32))).to(_dev())
+    f = lambda a: None if a is None else torch.from_numpy(np.ascontiguousarray(a.astype(np.float32))).to(inputs.device())
     return f(comp), f(mean), f(cs)
 
 
 def transform(pca, X, whitenp=0.5, whitenv=None, whitenm=1.0, use_sklearn=True):
     """common.py:221-232 (projection + whitening scale, no L2)."""
     comp, mean, cs = _pca_arrays(pca, whitenp, whitenv, whitenm, use_sklearn)
-    return ops.whiten(_to_dev_f32(X), comp, mean, cs, l2norm=False).cpu().numpy()
+    return ops.whiten(inputs.rows(X), comp, mean, cs, l2norm=False).cpu().numpy()
 
 
 def whiten_features(X, pca, l2norm=True, whitenp=0.5, whitenv=None, whitenm=1.0, use_sklearn=True):
     """common.py:235-239."""
     comp, mean, cs = _pca_arrays(pca, whitenp, whitenv, whitenm, use_sklearn)
-    return ops.whiten(_to_dev_f32(X), comp, mean, cs, l2norm=l2norm).cpu().numpy()
+    return ops.whiten(inputs.rows(X), comp, mean, cs, l2norm=l2norm).cpu().numpy()
 
 
 def whiten_features_gpu(X, pca, l2norm=True, whitenp=0.5, whitenv=None, whitenm=1.0, want_f16=False):
     """Device-resident variant (no host round trip) for the search pipeline."""
     comp, mean, cs = _pca_arrays(pca, whitenp, whitenv, whitenm, True)
-    return ops.whiten(_to_dev_f32(X), comp, mean, cs, l2norm=l2norm, want_f16=want_f16)
+    return ops.whiten(inputs.rows(X), comp, mean, cs, l2norm=l2norm, want_f16=want_f16)

@@ -28,6 +28,7 @@ import numpy as np
 import torch
 
 from . import lib, ops
+from .inputs import rows64
 
 # Iscen et al. 2017, experiments on global descriptors (see DESIGN.md section 4.7): k = 50 mutual neighbours, the
 # kq = 10 nearest rows seed a query, gamma = 3, alpha = 0.99, 20 conjugate-gradient iterations.  tol = 0 keeps the
@@ -67,14 +68,6 @@ class Graph(NamedTuple):
     val: torch.Tensor
 
 
-def _rows64(x):
-    """(N, D) fp32 CUDA rows, D zero-padded to a multiple of 64 (the search's layout; zero columns change no score)."""
-    t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
-    t = t.to(device="cuda", dtype=torch.float32)
-    pad = (-t.shape[1]) % 64
-    return (torch.nn.functional.pad(t, (0, pad)) if pad else t).contiguous()
-
-
 class Weights(NamedTuple):
     """The graph before normalisation, on the CSR of Graph: a fp64 (nnz,) = A_ij, u fp64 (N,) = 1/sqrt(d_i)."""
     a: torch.Tensor
@@ -94,7 +87,7 @@ def graph_from_knn(idx, scores, k, gamma, weights=False):
         raise ValueError("diffusion: neighbour indices must lie in [0, %d) or be -1" % idx.shape[0])
     n, width = idx.shape
     dev = idx.device
-    ws = torch.empty(lib.raw("dirb200_diffusion_graph_workspace_bytes")(n, int(k)), dtype=torch.uint8, device=dev)
+    ws = ops.workspace(lib.raw("dirb200_diffusion_graph_workspace_bytes")(n, int(k)), dev)
     row_ptr = torch.empty(n + 1, dtype=torch.int64, device=dev)
     col = torch.empty(n * int(k), dtype=torch.int32, device=dev)
     val = torch.empty(n * int(k), dtype=torch.float64, device=dev)
@@ -136,7 +129,7 @@ class Diffusion:
         check_params(k=k, gamma=gamma)
         self.k, self.gamma, self.ws_budget = int(k), float(gamma), int(ws_budget)
         self.dim = bdescs.shape[1]
-        self.db = _rows64(bdescs)
+        self.db = rows64(bdescs)
         self.n = self.db.shape[0]
         if self.n < 1:
             raise ValueError("diffusion: the database is empty")
@@ -158,7 +151,7 @@ class Diffusion:
         check_params(kq=kq, alpha=alpha, iters=iters, tol=tol)
         if qdescs.shape[1] != self.dim:
             raise ValueError("diffusion: query dimension %d differs from the database's %d" % (qdescs.shape[1], self.dim))
-        q = _rows64(qdescs)
+        q = rows64(qdescs)
         nq, n = q.shape[0], self.n
         qb = min(int(q_block) if q_block else self.query_block(nq), MAX_Q_BLOCK)
         g = self.graph
@@ -170,7 +163,7 @@ class Diffusion:
             y = torch.empty((n, b), dtype=torch.float64, device=dev)
             lib.call("dirb200_diffusion_seeds", ops._ptr(idx), ops._ptr(sc), b, int(kq), self.gamma, n, ops._ptr(y),
                      ops._stream())
-            ws = torch.empty(lib.raw("dirb200_diffusion_solve_workspace_bytes")(n, b), dtype=torch.uint8, device=dev)
+            ws = ops.workspace(lib.raw("dirb200_diffusion_solve_workspace_bytes")(n, b), dev)
             f = torch.empty((n, b), dtype=torch.float64, device=dev)
             it = torch.empty(b, dtype=torch.int32, device=dev)
             res = torch.empty(b, dtype=torch.float64, device=dev)
@@ -211,26 +204,30 @@ class Diffusion:
         idx = torch.empty((nq, k), dtype=torch.int64, device="cuda")
         for q0, fb, _, _ in self._blocks(qdescs, kq, alpha, iters, tol, q_block):
             b = fb.shape[1]
-            ws = torch.empty(lib.raw("dirb200_diffusion_topk_workspace_bytes")(b, k), dtype=torch.uint8, device=fb.device)
+            ws = ops.workspace(lib.raw("dirb200_diffusion_topk_workspace_bytes")(b, k), fb.device)
             lib.call("dirb200_diffusion_topk", ops._ptr(fb), self.n, b, k, ops._ptr(ws), ops._ptr(scores[q0:q0 + b]),
                      ops._ptr(idx[q0:q0 + b]), ops._stream())
         return scores, idx
 
-    def rank_counts(self, qdescs, t_off, t_rows, t_flags, kq=DEFAULTS["kq"], alpha=DEFAULTS["alpha"],
-                    iters=DEFAULTS["iters"], tol=DEFAULTS["tol"], q_block=None):
-        """For the targets of each query (host CSR: t_off int (Q+1,), t_rows int64 (T,), t_flags uint8 (T,)) ->
-        (f at each target fp64 (T,), rows ranking before each flagged target int64 (T,); 0 when unflagged), CUDA
-        tensors: the contract of ops.Index.rank_counts with f in place of the exact score."""
+    def _targets(self, nq, t_off, t_rows, t_flags):
+        """The targets of nq queries (host CSR) -> (off int64 (nq+1,), rows int64 (T,), flags uint8 (T,)), checked."""
         off = np.ascontiguousarray(t_off, dtype=np.int64)
         rows = np.ascontiguousarray(t_rows, dtype=np.int64)
         flags = np.ascontiguousarray(t_flags, dtype=np.uint8)
-        nq = qdescs.shape[0]
         if off.shape != (nq + 1,) or off[0] != 0 or off[-1] != rows.shape[0] or np.any(np.diff(off) < 0):
             raise ValueError("diffusion: t_off must be non-decreasing offsets from 0 to len(t_rows), one per query + 1")
         if flags.shape != rows.shape:
             raise ValueError("diffusion: t_flags must have the shape of t_rows")
         if rows.size and (rows.min() < 0 or rows.max() >= self.n):
             raise ValueError("diffusion: target rows must lie in [0, %d)" % self.n)
+        return off, rows, flags
+
+    def rank_counts(self, qdescs, t_off, t_rows, t_flags, kq=DEFAULTS["kq"], alpha=DEFAULTS["alpha"],
+                    iters=DEFAULTS["iters"], tol=DEFAULTS["tol"], q_block=None):
+        """For the targets of each query (host CSR: t_off int (Q+1,), t_rows int64 (T,), t_flags uint8 (T,)) ->
+        (f at each target fp64 (T,), rows ranking before each flagged target int64 (T,); 0 when unflagged), CUDA
+        tensors: the contract of ops.Index.rank_counts with f in place of the exact score."""
+        off, rows, flags = self._targets(qdescs.shape[0], t_off, t_rows, t_flags)
         T = rows.shape[0]
         scores = torch.zeros(T, dtype=torch.float64, device="cuda")
         above = torch.zeros(T, dtype=torch.int64, device="cuda")
@@ -243,8 +240,7 @@ class Diffusion:
             o_d = torch.from_numpy(o).to(fb.device)
             r_d = torch.from_numpy(rows[lo:hi]).to(fb.device)
             f_d = torch.from_numpy(flags[lo:hi]).to(fb.device)
-            ws = torch.empty(lib.raw("dirb200_diffusion_rank_count_workspace_bytes")(b, hi - lo), dtype=torch.uint8,
-                             device=fb.device)
+            ws = ops.workspace(lib.raw("dirb200_diffusion_rank_count_workspace_bytes")(b, hi - lo), fb.device)
             lib.call("dirb200_diffusion_rank_count", ops._ptr(fb), self.n, b, o.ctypes.data_as(C.c_void_p), ops._ptr(o_d),
                      ops._ptr(r_d), ops._ptr(f_d), hi - lo, ops._ptr(ws), ops._ptr(scores[lo:hi]), ops._ptr(above[lo:hi]),
                      ops._stream())
@@ -270,7 +266,7 @@ class Diffusion:
             raise ValueError("diffusion: kq = %d exceeds the truncation depth m' = min(m, N) = %d" % (kq, m))
         if qdescs.shape[1] != self.dim:
             raise ValueError("diffusion: query dimension %d differs from the database's %d" % (qdescs.shape[1], self.dim))
-        q = _rows64(qdescs)
+        q = rows64(qdescs)
         nq, n, kw = q.shape[0], self.n, self.ell
         depth = max(int(depth), m)
         qb = min(int(q_block) if q_block else self.trunc_query_block(nq, m, depth), MAX_Q_BLOCK)
@@ -285,11 +281,11 @@ class Diffusion:
                         torch.empty((b, kw, m), dtype=torch.int32, device=dev),
                         torch.empty((b, kw, m), dtype=torch.float64, device=dev),
                         *(torch.empty((b, m), dtype=torch.float64, device=dev) for _ in range(3)))
-            ws = torch.empty(lib.raw("dirb200_diffusion_trunc_build_workspace_bytes")(b, m), dtype=torch.uint8, device=dev)
+            ws = ops.workspace(lib.raw("dirb200_diffusion_trunc_build_workspace_bytes")(b, m), dev)
             lib.call("dirb200_diffusion_trunc_build", ops._ptr(g.row_ptr), ops._ptr(g.col), ops._ptr(w.a), n, kw,
                      ops._ptr(li), ops._ptr(ls), b, m, int(kq), self.gamma, ops._ptr(ws), *(ops._ptr(t) for t in loc),
                      ops._stream())
-            ws = torch.empty(lib.raw("dirb200_diffusion_trunc_solve_workspace_bytes")(b, m), dtype=torch.uint8, device=dev)
+            ws = ops.workspace(lib.raw("dirb200_diffusion_trunc_solve_workspace_bytes")(b, m), dev)
             f = torch.empty((b, m), dtype=torch.float64, device=dev)
             it = torch.empty(b, dtype=torch.int32, device=dev)
             res = torch.empty(b, dtype=torch.float64, device=dev)
@@ -330,8 +326,7 @@ class Diffusion:
         idx = torch.empty((nq, k), dtype=torch.int64, device="cuda")
         for q0, ls, li, loc, fb, _, _ in self._trunc_blocks(qdescs, m, kq, alpha, iters, tol, q_block, depth=k):
             b, mm = fb.shape
-            ws = torch.empty(lib.raw("dirb200_diffusion_trunc_topk_workspace_bytes")(b, mm, k), dtype=torch.uint8,
-                             device=fb.device)
+            ws = ops.workspace(lib.raw("dirb200_diffusion_trunc_topk_workspace_bytes")(b, mm, k), fb.device)
             lib.call("dirb200_diffusion_trunc_topk", ops._ptr(loc.rows), ops._ptr(fb), b, mm, ops._ptr(li), ops._ptr(ls),
                      li.shape[1], k, ops._ptr(ws), ops._ptr(scores[q0:q0 + b]), ops._ptr(idx[q0:q0 + b]), ops._stream())
         return scores, idx
@@ -342,16 +337,7 @@ class Diffusion:
         R_q, value fp64 (T,): f' inside R_q and the exact score outside, above int64 (T,): rows ranking before each
         flagged target, 0 when unflagged), CUDA tensors.  Every row of R_q ranks before every row outside it, so a
         target outside R_q keeps its exact rank count (ops.Index.rank_counts)."""
-        off = np.ascontiguousarray(t_off, dtype=np.int64)
-        rows = np.ascontiguousarray(t_rows, dtype=np.int64)
-        flags = np.ascontiguousarray(t_flags, dtype=np.uint8)
-        nq = qdescs.shape[0]
-        if off.shape != (nq + 1,) or off[0] != 0 or off[-1] != rows.shape[0] or np.any(np.diff(off) < 0):
-            raise ValueError("diffusion: t_off must be non-decreasing offsets from 0 to len(t_rows), one per query + 1")
-        if flags.shape != rows.shape:
-            raise ValueError("diffusion: t_flags must have the shape of t_rows")
-        if rows.size and (rows.min() < 0 or rows.max() >= self.n):
-            raise ValueError("diffusion: target rows must lie in [0, %d)" % self.n)
+        off, rows, flags = self._targets(qdescs.shape[0], t_off, t_rows, t_flags)
         T = rows.shape[0]
         inside = torch.zeros(T, dtype=torch.uint8, device="cuda")
         value = torch.zeros(T, dtype=torch.float64, device="cuda")
@@ -369,7 +355,7 @@ class Diffusion:
                      ops._ptr(above[lo:hi]), ops._stream())
         out = inside == 0
         if T and bool(out.any()):
-            sc, ab = self.index.rank_counts(_rows64(qdescs), off, rows, flags)
+            sc, ab = self.index.rank_counts(rows64(qdescs), off, rows, flags)
             value = torch.where(out, sc, value)
             above = torch.where(out & torch.from_numpy(flags != 0).to(above.device), ab, above)
         return inside.bool(), value, above

@@ -19,10 +19,8 @@ from typing import NamedTuple
 import numpy as np
 import torch
 
-from . import ops
+from . import inputs, ops
 from .store import DescriptorStore
-
-NORM_SLACK = 1e-3          # what ops.Index accepts as unit norm
 
 
 class Duplicates(NamedTuple):
@@ -51,27 +49,6 @@ def check_tau(tau):
     return t
 
 
-def _rows(x, device, name):
-    """Descriptors (a CUDA / host tensor, an array or a DescriptorStore) -> contiguous fp32 (N, D) on `device`."""
-    if isinstance(x, DescriptorStore):
-        return x.load_rows_to_device(0, len(x), device)[0]
-    if isinstance(x, torch.Tensor):
-        t = x
-    else:
-        t = torch.from_numpy(np.array(x, dtype=np.float32, order="C"))     # a copy: memory maps are read-only
-    if t.dim() != 2:
-        raise ValueError("%s must be a 2-D array of descriptors (got shape %s)" % (name, tuple(t.shape)))
-    return t.to(device=device, dtype=torch.float32).contiguous()
-
-
-def _check_norms(x, name, eps16):
-    if eps16 is None and x.shape[0]:
-        worst = float(torch.linalg.vector_norm(x, dim=1).max())
-        if worst > 1.0 + NORM_SLACK:
-            raise ValueError("%s rows are not unit-norm (max norm %.4g): normalise them, or pass eps16 = "
-                             "1.2e-3*max|q|*max|row| + 2^-24*sqrt(D)*(max|q| + max|row|) (see ops.Index)" % (name, worst))
-
-
 def _index(x, eps16):
     idx = ops.Index(x, check_norms=False)
     if eps16 is not None:
@@ -82,18 +59,15 @@ def _index(x, eps16):
     return idx
 
 
-def _device(device):
-    return torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-
-
 def near_duplicates(descs, tau, eps16=None, row_block=None, device=None) -> Duplicates:
     """Every pair i < j of rows with exact score >= tau, its connected components and the groups they form.
     descs: (N, D) descriptors - a CUDA tensor, a host array / tensor or a DescriptorStore.  Rows must be unit-norm
     unless eps16 (the bound on |fp16-path score - exact score|, ops.Index's recipe) is given.  row_block: rows joined
     per tensor-core launch sequence (a multiple of 128; the result does not depend on it)."""
     tau = check_tau(tau)
-    x = _rows(descs, _device(device), "descs")
-    _check_norms(x, "descs", eps16)
+    x = inputs.rows(descs, device, "descs")
+    if eps16 is None:
+        inputs.check_norm_at_most_1(x, "descs")
     n = x.shape[0]
     if n == 0:
         z = torch.zeros(1, dtype=torch.int64, device=x.device)
@@ -113,13 +87,14 @@ def overlap(qdescs, bdescs, tau, eps16=None, device=None):
     desc, r asc) -> CSR (offsets int64 (Q+1,), rows int64, scores fp64), CUDA tensors.  Same inputs as near_duplicates;
     both sets must have the same dimension."""
     tau = check_tau(tau)
-    dev = _device(device)
-    q = _rows(qdescs, dev, "qdescs")
-    b = _rows(bdescs, dev, "bdescs")
+    dev = inputs.device(device)
+    q = inputs.rows(qdescs, dev, "qdescs")
+    b = inputs.rows(bdescs, dev, "bdescs")
     if q.shape[1] != b.shape[1]:
         raise ValueError("the two sets have different dimensions (%d and %d)" % (q.shape[1], b.shape[1]))
-    _check_norms(q, "qdescs", eps16)
-    _check_norms(b, "bdescs", eps16)
+    if eps16 is None:
+        inputs.check_norm_at_most_1(q, "qdescs")
+        inputs.check_norm_at_most_1(b, "bdescs")
     if q.shape[0] == 0:
         return (torch.zeros(1, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int64, device=dev),
                 torch.empty(0, dtype=torch.float64, device=dev))

@@ -12,11 +12,9 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from . import lib, ops
-from .cluster import SphericalKMeans, _check_unit, assign
-from .duplicates import _device, _rows
-from .ivf import _check_k
-from .store import DescriptorStore
+from . import inputs, lib, ops
+from .cluster import SphericalKMeans, assign
+from .ivf import InvertedLists
 
 MS = (8, 16, 32, 64, 128)       # rule P2
 MAX_SUB = 256                   # the kernels' largest sub-vector D / M
@@ -27,22 +25,6 @@ MAX_QUERIES = 65535             # queries per dirb200_pq_search
 
 def _i(v):
     return int(v.item()) if isinstance(v, torch.Tensor) else int(v)
-
-
-class _Source:
-    """Rows [a, b) of X as a contiguous fp32 device tensor, whatever holds X."""
-
-    def __init__(self, X, device):
-        if isinstance(X, DescriptorStore):
-            self.n, self.d = len(X), X.dim
-            self.get = lambda a, b: X.load_rows_to_device(a, b, device)[0]
-            return
-        if not isinstance(X, torch.Tensor) and not hasattr(X, "shape"):
-            X = np.asarray(X, np.float32)
-        if len(X.shape) != 2:
-            raise ValueError("X must be a 2-D array of descriptors (got shape %s)" % (tuple(X.shape),))
-        self.n, self.d = int(X.shape[0]), int(X.shape[1])
-        self.get = lambda a, b: _rows(X[a:b], device, "X")
 
 
 def _plan(n, chunk_rows, train_rows):
@@ -68,7 +50,7 @@ def _check_shape(d, M):
     return int(M)
 
 
-class IVFPQIndex:
+class IVFPQIndex(InvertedLists):
     """IVFPQIndex(X, centres, M): X (N, D) unit rows (a CUDA tensor, a host array / memmap or a DescriptorStore),
     centres a (K, D) array of unit rows or a fitted SphericalKMeans, M codes per row (rule P2).
 
@@ -83,16 +65,13 @@ class IVFPQIndex:
 
     def __init__(self, X, centres, M, train_size=None, pq_iter=25, seed=0, rows="device", chunk_rows=1 << 16,
                  device=None):
-        if isinstance(centres, SphericalKMeans):
-            if not hasattr(centres, "cluster_centers_"):
-                raise ValueError("the SphericalKMeans has not been fitted")
-            centres = centres.cluster_centers_
+        centres = self._centres_of(centres)
         if rows not in ("device", "host"):
             raise ValueError("rows must be 'device' or 'host' (got %r)" % (rows,))
-        dev = X.device if isinstance(X, torch.Tensor) and X.is_cuda and device is None else _device(device)
-        src = _Source(X, dev)
+        dev = inputs.device(device, X)
+        src = inputs.Rows(X)
         n, d = src.n, src.d
-        c = _rows(centres, dev, "centres")
+        c = inputs.rows(centres, dev, "centres")
         if n < 1 or c.shape[0] < 1:
             raise ValueError("need at least one row and one centre")
         if n >= 1 << 31:
@@ -100,17 +79,14 @@ class IVFPQIndex:
         if c.shape[1] != d:
             raise ValueError("X has dimension %d, the centres %d" % (d, c.shape[1]))
         self.M = _check_shape(d, M)
-        chunk_rows = _check_k(chunk_rows, "chunk_rows")
+        chunk_rows = inputs.check_int(chunk_rows, "chunk_rows")
         pq_iter = int(pq_iter)
         if pq_iter < 0:
             raise ValueError("pq_iter must be >= 0 (got %d)" % pq_iter)
-        T = min(n, TRAIN_SIZE) if train_size is None else _check_k(train_size, "train_size")
-        if T > n:
-            raise ValueError("train_size = %d exceeds the number of rows (%d)" % (T, n))
+        T = min(n, TRAIN_SIZE) if train_size is None else inputs.check_int(train_size, "train_size", 1, n)
         if T < 256:
             raise ValueError("the codebooks need at least 256 training rows (got %d)" % T)
-        _check_unit(c, "centres")
-        k = c.shape[0]
+        inputs.check_unit(c, "centres")
         rng = np.random.default_rng(seed)
         train_rows = np.sort(rng.choice(n, T, replace=False))
         init = rng.choice(T, 256, replace=False)
@@ -127,19 +103,14 @@ class IVFPQIndex:
         plan = _plan(n, chunk_rows, train_rows)
         self.chunks_ = len(plan)
         for a, b, lo, hi in plan:
-            xc = src.get(a, b)
-            _check_unit(xc, "X")
+            xc = src.get(a, b, dev)
+            inputs.check_unit(xc, "X")
             labels[a:b] = assign(xc, c)[0]
             if hi > lo:
                 xt[lo:hi] = xc[torch.from_numpy(train_rows[lo:hi] - a).to(dev)]
             if self.rows_ is not X:
                 self.rows_[a:b].copy_(xc)
-        self.perm_ = torch.sort(labels, stable=True).indices
-        self.list_sizes_ = torch.bincount(labels, minlength=k)
-        self.cell_off_ = torch.zeros(k + 1, dtype=torch.int64, device=dev)
-        torch.cumsum(self.list_sizes_, 0, out=self.cell_off_[1:])
-        self.centres_ = c
-        self._centres = ops.Index(c, check_norms=False)
+        self._set_lists(labels, c)
 
         # rule P3: codebooks from the residuals of the training rows
         lt = labels[torch.from_numpy(train_rows).to(dev)].contiguous()
@@ -180,53 +151,30 @@ class IVFPQIndex:
         The lists are fitted on the device: on every row when X is a CUDA tensor or has at most fit_rows rows (default:
         as many as a quarter of the free device memory holds), else on fit_rows rows drawn without replacement by
         numpy.random.default_rng(seed) (sorted)."""
-        dev = X.device if isinstance(X, torch.Tensor) and X.is_cuda and device is None else _device(device)
-        src = _Source(X, dev)
+        dev = inputs.device(device, X)
+        src = inputs.Rows(X)
         if fit_rows is None:
             fit_rows = max(n_lists, torch.cuda.mem_get_info(dev)[0] // (4 * 4 * src.d))
         if isinstance(X, torch.Tensor) and X.is_cuda or src.n <= fit_rows:
-            xf = src.get(0, src.n)
+            xf = src.get(0, src.n, dev)
         else:
             sel = np.sort(np.random.default_rng(seed).choice(src.n, int(fit_rows), replace=False))
             xf = torch.empty((len(sel), src.d), dtype=torch.float32, device=dev)
             for a, b, lo, hi in _plan(src.n, 1 << 16, sel):
                 if hi > lo:
-                    xf[lo:hi] = src.get(a, b)[torch.from_numpy(sel[lo:hi] - a).to(dev)]
+                    xf[lo:hi] = src.get(a, b, dev)[torch.from_numpy(sel[lo:hi] - a).to(dev)]
         km = SphericalKMeans(n_lists, init="k-means++", max_iter=max_iter, seed=seed).fit(xf)
         del xf
         index = cls(X, km, M, seed=seed, device=dev, **kw)
         index.kmeans_ = km
         return index
 
-    @property
-    def n_lists(self):
-        return self.centres_.shape[0]
-
-    def _queries(self, q):
-        q = _rows(q, self.centres_.device, "q")
-        if q.shape[1] != self.centres_.shape[1]:
-            raise ValueError("queries have dimension %d, the index %d" % (q.shape[1], self.centres_.shape[1]))
-        _check_unit(q, "q")
-        return q
-
-    def _nprobe(self, nprobe):
-        nprobe = _check_k(nprobe, "nprobe")
-        if nprobe > self.n_lists:
-            raise ValueError("nprobe must be in [1, %d] (got %d)" % (self.n_lists, nprobe))
-        return nprobe
-
-    def probe(self, q, nprobe):
-        """Rule I3: the nprobe best lists of each query (score desc, ties to the smaller centre) -> int64 (Q, nprobe)."""
-        return self._centres.search(self._queries(q), self._nprobe(nprobe))[1]
-
     def search(self, q, k, nprobe, refine=None):
         """Rules P5-P7 -> (scores fp64 (Q, k), rows int64 (Q, k)): the exact top-k of the best refine (R, default 4k)
         probed rows by ADC score, padded with (-inf, -1)."""
         q = self._queries(q)
-        k = _check_k(k, "k")
-        R = 4 * k if refine is None else _check_k(refine, "refine")
-        if R < k:
-            raise ValueError("refine must be >= k (got %d < %d)" % (R, k))
+        k = inputs.check_int(k, "k")
+        R = 4 * k if refine is None else inputs.check_int(refine, "refine", k)
         nprobe = self._nprobe(nprobe)
         R = max(k, min(R, self.perm_.shape[0]))       # C_q never holds more than N rows
         dev = q.device
@@ -255,7 +203,7 @@ class IVFPQIndex:
             qq = q[q0:q0 + qb]
             qoff = torch.from_numpy(cum[q0:q0 + qb + 1] - cum[q0]).to(dev)
             tables = torch.empty((qb, self.M, 256), dtype=torch.float32, device=dev)
-            ws = torch.empty(max(1, lib.raw("dirb200_pq_search_ws_bytes")(qb, total, R)), dtype=torch.uint8, device=dev)
+            ws = ops.workspace(lib.raw("dirb200_pq_search_ws_bytes")(qb, total, R), dev)
             if ev:
                 ev[0].record()
             lib.call("dirb200_pq_tables", ops._ptr(qq), qb, d, ops._ptr(self.codebooks_), self.M, ops._ptr(tables), s)
@@ -284,7 +232,7 @@ class IVFPQIndex:
         largest C_q."""
         q = self._queries(q)
         nprobe = self._nprobe(nprobe)
-        R = RANK_REFINE if refine is None else _check_k(refine, "refine")
+        R = RANK_REFINE if refine is None else inputs.check_int(refine, "refine")
         off = np.ascontiguousarray(t_off, dtype=np.int64)
         own = exact is None
         if own:
@@ -296,22 +244,7 @@ class IVFPQIndex:
                 exact.close()
         depth = max(1, min(R, int(self.list_sizes_[self._centres.search(q, nprobe)[1]].sum(1).max())))
         lsc, lix = self.search(q, depth, nprobe, refine=max(R, depth))
-        cq = (lix >= 0).sum(1)
-        dev = q.device
-        rows = torch.as_tensor(np.ascontiguousarray(t_rows, dtype=np.int64)).to(dev)
-        flags = torch.as_tensor(np.ascontiguousarray(t_flags, dtype=np.uint8)).to(dev)
-        t_q = torch.from_numpy(np.repeat(np.arange(q.shape[0]), np.diff(off))).to(dev)
-        a_in = torch.zeros_like(a_all)
-        inside = torch.zeros(rows.shape[0], dtype=torch.bool, device=dev)
-        step = max(1, (1 << 24) // depth)
-        for t0 in range(0, rows.shape[0], step):
-            tq, tr, ts = t_q[t0:t0 + step], rows[t0:t0 + step], sc[t0:t0 + step]
-            ls, li = lsc[tq], lix[tq]
-            before = (li >= 0) & ((ls > ts[:, None]) | ((ls == ts[:, None]) & (li < tr[:, None])))
-            a_in[t0:t0 + step] = before.sum(1)
-            inside[t0:t0 + step] = (li == tr[:, None]).any(1)
-        rank = torch.where(inside, a_in, cq[t_q] + a_all - a_in)
-        return inside, sc, torch.where(flags != 0, rank, torch.zeros_like(rank))
+        return self._ranks(off, t_rows, t_flags, sc, a_all, lsc, lix)
 
     def stats(self):
         """The last search: queries, query blocks, (query, probe) segments, rows scanned, candidates refined, and with
@@ -328,6 +261,6 @@ class IVFPQIndex:
             raise ValueError("unknown option %r (ws_budget, profile)" % (key,))
 
     def close(self):
-        self._centres.close()
+        super().close()
         for name in ("codes_", "perm_", "rows_", "codebooks_"):
             setattr(self, name, None)

@@ -11,6 +11,7 @@ import numpy as np
 import torch
 
 from . import lib
+from .inputs import check_norm_at_most_1
 
 
 def _stream():
@@ -19,6 +20,11 @@ def _stream():
 
 def _ptr(t):
     return C.c_void_p(0) if t is None else C.c_void_p(t.data_ptr())
+
+
+def workspace(nbytes, device):
+    """A device scratch buffer of nbytes (at least one, so that its pointer is never null)."""
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
 
 
 def _chk(t, dtype, name):
@@ -541,12 +547,8 @@ class Index:
         dimension): below 2^-14 fp16 is subnormal and rounds to an absolute 2^-25 per entry, which the first term
         alone does not cover for small norms.  Every entry must stay below fp16's largest value, 65504."""
         _chk(db32, torch.float32, "db32")
-        if check_norms and db32.shape[0]:
-            worst = float(torch.linalg.vector_norm(db32, dim=1).max())
-            if worst > 1.0 + 1e-3:
-                raise ValueError("database rows are not unit-norm (max norm %.4g): the exact-top-k error bound assumes |row| <= 1; "
-                                 "normalise them, or pass check_norms=False and set option 'eps16' to 1.2e-3*max|q|*max|row| "
-                                 "+ 2^-24*sqrt(D)*(max|q| + max|row|) (entries below 65504)" % worst)
+        if check_norms:
+            check_norm_at_most_1(db32, "database")
         self.db32 = db32
         self.n, self.dim = db32.shape
         if db16 is None:                      # an empty shard (more ranks than rows) has nothing to convert

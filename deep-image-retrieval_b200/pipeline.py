@@ -16,8 +16,9 @@ import numpy as np
 import torch
 import tqdm
 
-from . import common, datasets, nets, ops
+from . import common, datasets, inputs, nets, ops
 from .common import matmul, pool, tonumpy
+from .inputs import rows64
 from .loader import get_loader
 from .store import DescriptorStore
 
@@ -28,12 +29,6 @@ def mkdir(fname, isfile="auto"):
     directory = os.path.split(fname)[0] if isfile else fname
     if directory and not os.path.isdir(directory):
         os.makedirs(directory)
-
-
-def _dev_f32(x):
-    if isinstance(x, torch.Tensor):
-        return x.to("cuda", torch.float32).contiguous()
-    return torch.from_numpy(np.ascontiguousarray(np.asarray(x, dtype=np.float32))).cuda()
 
 
 def _drop_self(scores, idx, own_rows, k):
@@ -56,14 +51,8 @@ def expand_descriptors(descs, db=None, alpha=0, k=0, q_block=4096, to_numpy=True
     if k == 0:
         return descs
     dim = np.shape(descs)[1]
-    pad = (-dim) % 64                      # the tensor-core search wants D % 64 == 0; zero columns change no score
-
-    def _padded(x):
-        x = _dev_f32(x)
-        return torch.nn.functional.pad(x, (0, pad)).contiguous() if pad else x
-
-    q = _padded(descs)
-    d = _padded(db) if db is not None else q
+    q = rows64(descs)
+    d = rows64(db) if db is not None else q
     index = ops.Index(d)
     out = torch.empty_like(q)
     # Queries go through in blocks so that database augmentation (an N x N self-search) needs O(block) scratch.
@@ -306,18 +295,37 @@ def extract_image_features(dataset, transforms, net, ret_imgs=False, same_size=F
 def _pool_and_normalize(descs, pooling, gemp):
     """pool() over transform chains followed by F.normalize(p=2, dim=1): test_dir.py:121-122."""
     if len(descs) == 1:
-        return ops.l2_normalize(_dev_f32(descs[0]))
+        return ops.l2_normalize(inputs.rows(descs[0]))
     if pooling not in ("mean", "gem"):
         raise ValueError("Bad pooling mode: " + str(pooling))
-    return ops.pool_scales([_dev_f32(d) for d in descs], pooling, gemp, l2=True)
+    return ops.pool_scales([inputs.rows(d) for d in descs], pooling, gemp, l2=True)
+
+
+def _rank_target_csr(db, nq):
+    """The targets of the APs of queries 0 .. nq-1 (db.rank_targets) as one host CSR -> (offsets int64 (nq+1,), rows
+    int64 (T,), flags uint8 (T,))."""
+    offs, rows, flags = [0], [], []
+    for q in range(nq):
+        r, fl = db.rank_targets(q)
+        rows.append(r)
+        flags.append(fl)
+        offs.append(offs[-1] + len(r))
+    rows = np.concatenate(rows) if rows else np.zeros(0, np.int64)
+    flags = np.concatenate(flags) if flags else np.zeros(0, np.uint8)
+    return np.array(offs, np.int64), rows, flags
+
+
+def _grade(grade, offs, rows, *per_target):
+    """Per-query APs from per-target results (CUDA tensors over the CSR offs / rows of _rank_target_csr):
+    grade(q, the rows of q, *the results at those rows) for every query q."""
+    per_target = [t.cpu().numpy() for t in per_target]
+    return [grade(q, rows[offs[q]:offs[q + 1]], *(t[offs[q]:offs[q + 1]] for t in per_target))
+            for q in range(len(offs) - 1)]
 
 
 def _aps_from_topk(db, qdescs, bdescs, k):
     """Per-query AP from the exact top-k ranking (dirb200_index_search); dense score row only where needed."""
-    dim = qdescs.shape[1]
-    pad = (-dim) % 64
-    f = lambda a: torch.nn.functional.pad(_dev_f32(a), (0, pad)).contiguous() if pad else _dev_f32(a)
-    qd, bd = f(qdescs), f(bdescs)
+    qd, bd = rows64(qdescs), rows64(bdescs)
     k = min(k, bd.shape[0])
     _, idx = ops.Index(bd).search(qd, k)
     idx = idx.cpu().numpy()
@@ -336,22 +344,10 @@ def _aps_from_counts(db, qdescs, bdescs):
     """Per-query AP without the Q x N score matrix and without any host-side ranking: the GPU returns the exact scores
     of the labelled rows and, for every positive, the number of database rows ranking before it
     (dirb200_index_rank_count); datasets.eval_query_AP_from_counts turns that into the AP of generic.py:196-224."""
-    dim = qdescs.shape[1]
-    pad = (-dim) % 64
-    f = lambda a: torch.nn.functional.pad(_dev_f32(a), (0, pad)).contiguous() if pad else _dev_f32(a)
-    qd, bd = f(qdescs), f(bdescs)
-    offs, rows, flags = [0], [], []
-    for q in range(qd.shape[0]):
-        r, fl = db.rank_targets(q)
-        rows.append(r)
-        flags.append(fl)
-        offs.append(offs[-1] + len(r))
-    rows = np.concatenate(rows) if rows else np.zeros(0, np.int64)
-    flags = np.concatenate(flags) if flags else np.zeros(0, np.uint8)
-    sc, above = ops.Index(bd).rank_counts(qd, np.array(offs, np.int32), rows, flags)
-    sc, above = sc.cpu().numpy(), above.cpu().numpy()
-    return [db.eval_query_AP_from_counts(q, rows[offs[q]:offs[q + 1]], sc[offs[q]:offs[q + 1]], above[offs[q]:offs[q + 1]])
-            for q in range(qd.shape[0])]
+    qd, bd = rows64(qdescs), rows64(bdescs)
+    offs, rows, flags = _rank_target_csr(db, qd.shape[0])
+    sc, above = ops.Index(bd).rank_counts(qd, offs, rows, flags)
+    return _grade(db.eval_query_AP_from_counts, offs, rows, sc, above)
 
 
 def _aps_from_label_counts(db, qdescs, bdescs, max_thresholds=1 << 26, q_block=4096):
@@ -361,10 +357,7 @@ def _aps_from_label_counts(db, qdescs, bdescs, max_thresholds=1 << 26, q_block=4
     dirb200_index_search.  Queries go through in blocks of at most ~max_thresholds thresholds (a class of c images
     gives c^2 of them).  -> (aps, tops)."""
     from .dist import ShardedIndex
-    dim = qdescs.shape[1]
-    pad = (-dim) % 64
-    f = lambda a: torch.nn.functional.pad(_dev_f32(a), (0, pad)).contiguous() if pad else _dev_f32(a)
-    qd, bd = f(qdescs), f(bdescs)
+    qd, bd = rows64(qdescs), rows64(bdescs)
     nq, n, dev = qd.shape[0], bd.shape[0], qd.device
     index = ShardedIndex(bd, 0)
     t_off, t_rows, skip = db.label_targets()
@@ -394,27 +387,14 @@ def _aps_from_diffusion(db, qdescs, bdescs, params):
     from .diffusion import Diffusion
     build = {k: params[k] for k in ("k", "gamma") if k in params}
     solve = {k: params[k] for k in ("kq", "alpha", "iters", "tol") if k in params}
-    offs, rows, flags = [0], [], []
-    for q in range(qdescs.shape[0]):
-        r, fl = db.rank_targets(q)
-        rows.append(r)
-        flags.append(fl)
-        offs.append(offs[-1] + len(r))
-    rows = np.concatenate(rows) if rows else np.zeros(0, np.int64)
-    flags = np.concatenate(flags) if flags else np.zeros(0, np.uint8)
+    offs, rows, flags = _rank_target_csr(db, qdescs.shape[0])
     if params.get("truncate") is not None:
         # truncated diffusion: a junk row and a positive are ordered by (inside R_q, value, index), rule T6
         d = Diffusion(bdescs, truncation=True, **build)
-        inside, sc, above = d.rank_counts_truncated(qdescs, np.array(offs, np.int64), rows, flags, params["truncate"],
-                                                    **solve)
-        inside, sc, above = inside.cpu().numpy(), sc.cpu().numpy(), above.cpu().numpy()
-        return [db.eval_query_AP_from_truncated_counts(q, rows[offs[q]:offs[q + 1]], inside[offs[q]:offs[q + 1]],
-                                                       sc[offs[q]:offs[q + 1]], above[offs[q]:offs[q + 1]])
-                for q in range(qdescs.shape[0])]
-    sc, above = Diffusion(bdescs, **build).rank_counts(qdescs, np.array(offs, np.int64), rows, flags, **solve)
-    sc, above = sc.cpu().numpy(), above.cpu().numpy()
-    return [db.eval_query_AP_from_counts(q, rows[offs[q]:offs[q + 1]], sc[offs[q]:offs[q + 1]], above[offs[q]:offs[q + 1]])
-            for q in range(qdescs.shape[0])]
+        inside, sc, above = d.rank_counts_truncated(qdescs, offs, rows, flags, params["truncate"], **solve)
+        return _grade(db.eval_query_AP_from_truncated_counts, offs, rows, inside, sc, above)
+    sc, above = Diffusion(bdescs, **build).rank_counts(qdescs, offs, rows, flags, **solve)
+    return _grade(db.eval_query_AP_from_counts, offs, rows, sc, above)
 
 
 def _aps_from_ivf(db, qdescs, bdescs, params):
@@ -422,38 +402,25 @@ def _aps_from_ivf(db, qdescs, bdescs, params):
     of the database rows (IVFIndex.train), each query ranks the union R_q of its nprobe best lists first, in exact
     order, then every other row in exact order; a junk row ranks before a positive by (inside R_q, score, index)."""
     from .ivf import IVFIndex
-    dim = qdescs.shape[1]
-    pad = (-dim) % 64                   # zero columns keep the scores and the norms
-    f = lambda a: torch.nn.functional.pad(_dev_f32(a), (0, pad)).contiguous() if pad else _dev_f32(a)
-    qd, bd = f(qdescs), f(bdescs)
-    offs, rows, flags = [0], [], []
-    for q in range(qd.shape[0]):
-        r, fl = db.rank_targets(q)
-        rows.append(r)
-        flags.append(fl)
-        offs.append(offs[-1] + len(r))
-    rows = np.concatenate(rows) if rows else np.zeros(0, np.int64)
-    flags = np.concatenate(flags) if flags else np.zeros(0, np.uint8)
+    qd, bd = rows64(qdescs), rows64(bdescs)
+    offs, rows, flags = _rank_target_csr(db, qd.shape[0])
     if params.get("pq"):
         from .ivfpq import IVFPQIndex
         index = IVFPQIndex.train(bd, params["n_lists"], params["pq"], seed=params.get("seed", 0))
         exact = ops.Index(bd)
         try:
-            inside, sc, rank = index.rank_counts(qd, np.array(offs, np.int64), rows, flags, params["nprobe"],
-                                                 refine=params.get("refine"), exact=exact)
+            inside, sc, rank = index.rank_counts(qd, offs, rows, flags, params["nprobe"], refine=params.get("refine"),
+                                                 exact=exact)
         finally:
             exact.close()
             index.close()
     else:
         index = IVFIndex.train(bd, params["n_lists"], seed=params.get("seed", 0))
         try:
-            inside, sc, rank = index.rank_counts(qd, np.array(offs, np.int64), rows, flags, params["nprobe"])
+            inside, sc, rank = index.rank_counts(qd, offs, rows, flags, params["nprobe"])
         finally:
             index.close()
-    inside, sc, rank = inside.cpu().numpy(), sc.cpu().numpy(), rank.cpu().numpy()
-    return [db.eval_query_AP_from_truncated_counts(q, rows[offs[q]:offs[q + 1]], inside[offs[q]:offs[q + 1]],
-                                                   sc[offs[q]:offs[q + 1]], rank[offs[q]:offs[q + 1]])
-            for q in range(qd.shape[0])]
+    return _grade(db.eval_query_AP_from_truncated_counts, offs, rows, inside, sc, rank)
 
 
 def ivf_params(values):
@@ -566,7 +533,7 @@ def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=Non
         qdescs = expand_descriptors(qdescs, db=bdescs, to_numpy=False, **aqe)
     res = {}
     tops = None
-    qn, bn = _dev_f32(qdescs), _dev_f32(bdescs)
+    qn, bn = inputs.rows(qdescs), inputs.rows(bdescs)
     unit = bool(float((qn.norm(dim=1) - 1).abs().max()) < 1e-3 and float((bn.norm(dim=1) - 1).abs().max()) < 1e-3)
     if ivf is not None and diffusion is not None:
         raise ValueError("ivf and diffusion are two rankings: choose one")

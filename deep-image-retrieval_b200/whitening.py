@@ -16,45 +16,13 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from . import ops
-from .store import DescriptorStore
-
-
-def _n_rows_dim(X):
-    if isinstance(X, DescriptorStore):
-        return X.n_rows, X.dim
-    shape = tuple(X.shape)
-    if len(shape) != 2:
-        raise ValueError("expected a 2-D (n_samples, n_features) array, got shape %s" % (shape,))
-    return shape
-
-
-def _chunks(X, chunk_rows, device):
-    """(N, D) rows of X as contiguous fp32 tensors on `device`, chunk_rows at a time (a CUDA tensor as one view)."""
-    if isinstance(X, torch.Tensor) and X.is_cuda:
-        x = X.to(device, torch.float32).contiguous()
-        yield x
-        return
-    n = _n_rows_dim(X)[0]
-    for s in range(0, n, chunk_rows):
-        e = min(n, s + chunk_rows)
-        if isinstance(X, DescriptorStore):
-            block = torch.from_numpy(X.read_rows(s, e))
-        elif isinstance(X, torch.Tensor):
-            block = X[s:e]
-        else:
-            block = torch.from_numpy(np.array(X[s:e]))                    # a copy: memmaps are read-only
-        yield block.to(device, torch.float32).contiguous()
+from . import inputs, ops
 
 
 def _check_n_components(n_components, n, d):
     if n_components is None:
         return min(n, d)
-    if isinstance(n_components, (bool, np.bool_)) or not isinstance(n_components, (int, np.integer)):
-        raise ValueError("n_components must be None or an int in [1, %d], got %r" % (min(n, d), n_components))
-    if not 1 <= int(n_components) <= min(n, d):
-        raise ValueError("n_components=%d must be between 1 and min(n_samples, n_features)=%d" % (n_components, min(n, d)))
-    return int(n_components)
+    return inputs.check_int(n_components, "n_components", 1, min(n, d))
 
 
 def pca_from_gram(n, sums, gram, n_components=None):
@@ -101,22 +69,25 @@ def fit_pca(X, n_components=None, chunk_rows=65536):
     device, a CUDA tensor is used on its own device.
     -> sklearn.decomposition.PCA equal to sklearn's own covariance_eigh fit of X in fp64 up to the rounding of the
     statistics (tests/test_gpu_pca.py states the bounds)."""
-    n, d = _n_rows_dim(X)
+    src = inputs.Rows(X)
+    n, d = src.n, src.d
     _check_n_components(n_components, max(n, 1), d)
     if n < 2:
         raise ValueError("a PCA fit needs at least 2 samples, got %d" % n)
-    device = X.device if isinstance(X, torch.Tensor) and X.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    device = inputs.device(None, X)
     ops.require_gpu(device.index)
+    if isinstance(X, torch.Tensor) and X.is_cuda:
+        chunk_rows = n                                # a CUDA tensor as one view
     with torch.cuda.device(device):                   # the library launches on the current device's current stream
         sums = torch.zeros(d, dtype=torch.float64, device=device)
-        for x in _chunks(X, chunk_rows, device):
+        for x in src.chunks(chunk_rows, device):
             ops.col_sums_f64(x, sums)
         sums_h = sums.cpu().numpy()
         if not np.all(np.isfinite(sums_h / n)):
             raise ValueError("Input contains NaN or infinity.")
         mean = sums / n
         gram = torch.zeros((d, d), dtype=torch.float64, device=device)
-        for x in _chunks(X, chunk_rows, device):
+        for x in src.chunks(chunk_rows, device):
             ops.gram_f64(x, mean, gram)
         gram_h = gram.cpu().numpy()
     return pca_from_gram(n, sums_h, gram_h, n_components)

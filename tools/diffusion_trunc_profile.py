@@ -18,7 +18,8 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import dirb200  # noqa: E402,F401
 from dirb200 import lib, ops  # noqa: E402
-from dirb200.diffusion import DEFAULTS, Diffusion, _rows64  # noqa: E402
+from dirb200.diffusion import DEFAULTS, Diffusion  # noqa: E402
+from dirb200.inputs import rows64  # noqa: E402
 
 
 def _card():
@@ -56,7 +57,7 @@ class _Clock:
 def _truncated(d, q, m, topk, p):
     """The four stages of search(q, topk, truncate=m), each timed with events over all blocks."""
     mm = min(m, d.n)
-    qs = _rows64(q)
+    qs = rows64(q)
     nq, kw = qs.shape[0], d.ell
     depth = max(topk, mm)
     qb = d.trunc_query_block(nq, mm, depth)
