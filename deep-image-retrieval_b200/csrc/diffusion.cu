@@ -20,8 +20,8 @@
 #include <math.h>
 
 #include <algorithm>
-#include <cub/block/block_scan.cuh>
 
+#include "block.cuh"
 #include "common.h"
 
 namespace dirb {
@@ -64,20 +64,7 @@ __global__ void __launch_bounds__(SORT_THREADS) nbr_sort_kernel(const int64_t* _
   while (P < n) P <<= 1;
   for (int e = n + threadIdx.x; e < P; e += SORT_THREADS) ix[e] = INT_MAX;
   __syncthreads();
-  for (int size = 2; size <= P; size <<= 1) {
-    for (int st = size >> 1; st > 0; st >>= 1) {
-      for (int t = threadIdx.x; t < P / 2; t += SORT_THREADS) {
-        const int lo = 2 * t - (t & (st - 1)), hi = lo + st;
-        const bool up = (lo & size) == 0;
-        const int a = ix[lo], b = ix[hi];
-        if ((a > b) == up) {
-          ix[lo] = b; ix[hi] = a;
-          const double x = sw[lo]; sw[lo] = sw[hi]; sw[hi] = x;
-        }
-      }
-      __syncthreads();
-    }
-  }
+  block_bitonic_sort<SORT_THREADS>(ix, sw, P, [](int a, double, int b, double) { return a < b; });
   for (int e = threadIdx.x; e < k; e += SORT_THREADS) {
     nbr[i * k + e] = e < n ? ix[e] : -1;
     w[i * k + e] = e < n ? sw[e] : 0.0;
@@ -321,15 +308,7 @@ __global__ void __launch_bounds__(RED_THREADS) cg_scalar_kernel(const double* __
 }
 
 // ------------------------------------------------------------------------------------------------ rank counting
-// Order of rule 6: f descending, ties -> lower index, -0 == +0.  key(f) is an order-preserving uint64 image of f.
-__device__ __forceinline__ uint64_t fkey(double v) {
-  const uint64_t b = static_cast<uint64_t>(__double_as_longlong(v + 0.0));    // -0 + 0 = +0
-  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-
-__device__ __forceinline__ bool before(uint64_t ka, int64_t a, uint64_t kb, int64_t b) {
-  return ka > kb || (ka == kb && a < b);
-}
+// Order of rule 6: f descending, ties -> lower index, -0 == +0: ranks_before on the keys fkey(f).
 
 // one block per query: t_score of every target; the flagged targets sorted by rule 6 -> skey / srow / spos, nflag[q]
 __global__ void rc_sort_kernel(const double* __restrict__ f, int64_t N, int Q, const int* __restrict__ t_off,
@@ -350,7 +329,7 @@ __global__ void rc_sort_kernel(const double* __restrict__ f, int64_t N, int Q, c
       if (b == a || !t_flags[b]) continue;
       const int64_t rb = t_rows[b];
       const uint64_t kb = fkey(f[rb * Q + q]);
-      pos += before(kb, rb, ka, ra) || (kb == ka && rb == ra && b < a);
+      pos += ranks_before(kb, rb, ka, ra) || (kb == ka && rb == ra && b < a);
     }
     skey[t0 + pos] = ka;
     srow[t0 + pos] = ra;
@@ -390,7 +369,7 @@ __global__ void __launch_bounds__(RC_THREADS) rc_count_kernel(const double* __re
     int lo = 0, hi = nf;                  // first sorted target that row j ranks before
     while (lo < hi) {
       const int mid = (lo + hi) >> 1;
-      if (before(kj, j, skey[t0 + mid], srow[t0 + mid])) hi = mid; else lo = mid + 1;
+      if (ranks_before(kj, j, skey[t0 + mid], srow[t0 + mid])) hi = mid; else lo = mid + 1;
     }
     atomicAdd(&h[lo], 1u);
   }
@@ -416,10 +395,10 @@ __global__ void rc_prefix_kernel(int Q, const int* __restrict__ t_off, const int
 // row_ptr[i + 1] = sum_{i' <= i} mcnt[i'] in tiles of SCAN_TILE rows: tile totals, their exclusive scan, then each
 // tile's own scan plus its offset
 constexpr int SCAN_THREADS = 256, SCAN_PER = 8, SCAN_TILE = SCAN_THREADS * SCAN_PER;
-using BlockScan = cub::BlockScan<int64_t, SCAN_THREADS>;
 
+// v = the thread's running sums of its SCAN_PER counts; returns the sum over the tile's earlier threads
 __device__ __forceinline__ int64_t tile_scan(const int64_t* __restrict__ c, int64_t N, int64_t (&v)[SCAN_PER],
-                                             BlockScan::TempStorage& tmp, int64_t& total) {
+                                             int64_t* warp_sums, int64_t& total) {
   const int64_t i0 = static_cast<int64_t>(blockIdx.x) * SCAN_TILE + threadIdx.x * SCAN_PER;
   int64_t s = 0;
 #pragma unroll
@@ -427,16 +406,14 @@ __device__ __forceinline__ int64_t tile_scan(const int64_t* __restrict__ c, int6
     s += i0 + e < N ? c[i0 + e] : 0;
     v[e] = s;
   }
-  int64_t excl;
-  BlockScan(tmp).ExclusiveSum(s, excl, total);
-  return excl;
+  return block_scan(s, warp_sums, &total) - s;
 }
 
 __global__ void __launch_bounds__(SCAN_THREADS) scan_tile_kernel(const int64_t* __restrict__ c, int64_t N,
                                                                  int64_t* __restrict__ tile_sum) {
-  __shared__ BlockScan::TempStorage tmp;
+  __shared__ int64_t warp_sums[SCAN_THREADS / 32];
   int64_t v[SCAN_PER], total;
-  tile_scan(c, N, v, tmp, total);
+  tile_scan(c, N, v, warp_sums, total);
   if (threadIdx.x == 0) tile_sum[blockIdx.x] = total;
 }
 
@@ -452,9 +429,9 @@ __global__ void scan_top_kernel(int64_t* __restrict__ tile_sum, int nt) {
 __global__ void __launch_bounds__(SCAN_THREADS) scan_out_kernel(const int64_t* __restrict__ c, int64_t N,
                                                                 const int64_t* __restrict__ tile_off,
                                                                 int64_t* __restrict__ row_ptr) {
-  __shared__ BlockScan::TempStorage tmp;
+  __shared__ int64_t warp_sums[SCAN_THREADS / 32];
   int64_t v[SCAN_PER], total;
-  const int64_t excl = tile_scan(c, N, v, tmp, total) + tile_off[blockIdx.x];
+  const int64_t excl = tile_scan(c, N, v, warp_sums, total) + tile_off[blockIdx.x];
   const int64_t i0 = static_cast<int64_t>(blockIdx.x) * SCAN_TILE + threadIdx.x * SCAN_PER;
 #pragma unroll
   for (int e = 0; e < SCAN_PER; ++e)

@@ -21,6 +21,7 @@
 
 #include <algorithm>
 
+#include "block.cuh"
 #include "common.h"
 
 namespace dirb {
@@ -67,17 +68,7 @@ __global__ void __launch_bounds__(TB_THREADS, 1) trunc_build_kernel(
   for (int e = threadIdx.x; e < P; e += TB_THREADS)
     key[e] = e < m ? (static_cast<uint64_t>(list_idx[qm + e]) << 32) | static_cast<uint32_t>(e) : ~0ull;
   __syncthreads();
-  for (int size = 2; size <= P; size <<= 1) {
-    for (int st = size >> 1; st > 0; st >>= 1) {
-      for (int t = threadIdx.x; t < P / 2; t += TB_THREADS) {
-        const int lo = 2 * t - (t & (st - 1)), hi = lo + st;
-        const bool up = (lo & size) == 0;
-        const uint64_t x = key[lo], z = key[hi];
-        if ((x > z) == up) { key[lo] = z; key[hi] = x; }
-      }
-      __syncthreads();
-    }
-  }
+  block_bitonic_sort<TB_THREADS>(key, P, [](uint64_t a, uint64_t b) { return a < b; });
   for (int l = threadIdx.x; l < m; l += TB_THREADS) {       // the seeds to their local rows, before dd is reused
     const int pos = static_cast<int>(key[l] & 0xffffffffu);
     y[qm + l] = pos < kq ? dd[qm + pos] : 0.0;

@@ -12,6 +12,7 @@
 
 #include <algorithm>
 
+#include "block.cuh"
 #include "common.h"
 
 namespace dirb {
@@ -80,28 +81,15 @@ __global__ void __launch_bounds__(SCAN_THREADS) group_offsets_kernel(const int64
                                                                      const int64_t* __restrict__ label, int m,
                                                                      int64_t* __restrict__ group_off,
                                                                      int64_t* __restrict__ counts) {
-  __shared__ int warp_sum[SCAN_THREADS / 32];
-  __shared__ int64_t carry;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __shared__ int warp_sums[SCAN_THREADS / 32];
+  int64_t carry = 0;
   for (int base = 0; base < m; base += SCAN_THREADS) {
     const int p = base + threadIdx.x;
     const int start = (p < m && (p == 0 || label[members[p]] != label[members[p - 1]])) ? 1 : 0;
-    int incl = start;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += y;
-    }
-    if (lane == 31) warp_sum[warp] = incl;
-    __syncthreads();
-    int before = 0;
-    for (int w = 0; w < warp; ++w) before += warp_sum[w];
-    if (start) group_off[carry + before + incl - 1] = p;
-    __syncthreads();
-    if (threadIdx.x == SCAN_THREADS - 1) carry += before + incl;
-    __syncthreads();
+    int tot;
+    const int incl = block_scan(start, warp_sums, &tot);
+    if (start) group_off[carry + incl - 1] = p;
+    carry += tot;
   }
   if (threadIdx.x == 0) {
     group_off[carry] = m;

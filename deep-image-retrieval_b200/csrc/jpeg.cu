@@ -27,6 +27,7 @@
 #include <algorithm>
 #include <vector>
 
+#include "block.cuh"
 #include "common.h"
 
 namespace dirb {
@@ -235,41 +236,12 @@ int parse_jpeg(const uint8_t* d, size_t n, Parsed* P) {
 
 // ---------------------------------------------------------------------------------------------------------- kernels
 
-__device__ __forceinline__ int warp_incl_scan(int v) {
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += t;
-  }
-  return v;
-}
-
-// Exclusive scan over a CTA of 256 threads; *total gets the sum.
-__device__ int block_excl_scan(int v, int* total) {
-  __shared__ int warp_sums[9];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int inc = warp_incl_scan(v);
-  if (lane == 31) warp_sums[wid] = inc;
-  __syncthreads();
-  if (wid == 0) {
-    const int s = lane < 8 ? warp_sums[lane] : 0;
-    const int si = warp_incl_scan(s);
-    if (lane < 8) warp_sums[lane] = si - s;
-    if (lane == 7) warp_sums[8] = si;
-  }
-  __syncthreads();
-  const int r = warp_sums[wid] + inc - v;
-  *total = warp_sums[8];
-  __syncthreads();
-  return r;
-}
-
 // 1. Unstuff: one CTA per image; tiles of 256 x 16 stuffed bytes.  segstart[seg_off + s] = first unstuffed byte of
 // segment s, segstart[seg_off + nseg] = unstuffed length.
 __global__ void __launch_bounds__(256) unstuff_kernel(const ImgDesc* __restrict__ imgs, const uint8_t* __restrict__ in,
                                                       uint8_t* __restrict__ out, int* __restrict__ segstart,
                                                       int* __restrict__ status) {
+  __shared__ int warp_sums[256 / 32];
   const ImgDesc& im = imgs[blockIdx.x];
   if (im.nsub == 0) return;                                   // rejected by the host parser
   const uint8_t* src = in + im.in_off;
@@ -294,8 +266,9 @@ __global__ void __launch_bounds__(256) unstuff_kernel(const ImgDesc* __restrict_
       }
     }
     int tot_k, tot_r;
-    const int kb = block_excl_scan(__popc(keep), &tot_k);
-    const int rb = block_excl_scan(__popc(rst), &tot_r);
+    const int nk = __popc(keep), nr = __popc(rst);
+    const int kb = block_scan(nk, warp_sums, &tot_k) - nk;
+    const int rb = block_scan(nr, warp_sums, &tot_r) - nr;
     int k = kept_base + kb, r = rst_base + rb;
     for (int i = 0; i < 16; ++i) {
       if (keep >> i & 1) dst[k++] = src[p0 + i];
@@ -524,6 +497,7 @@ __global__ void count_kernel(SubCtx c, int64_t nsub_total, const uint64_t* st, i
 // 3b. One CTA per image: exclusive scan of the block counts (in place) and the per-segment block-count check.
 __global__ void __launch_bounds__(256) scan_check_kernel(const ImgDesc* __restrict__ imgs, int* cnt,
                                                          const int* __restrict__ seg_cnt, int* status) {
+  __shared__ int warp_sums[256 / 32];
   const ImgDesc& im = imgs[blockIdx.x];
   if (im.nsub == 0) return;
   int* c = cnt + im.sub_off;
@@ -532,7 +506,7 @@ __global__ void __launch_bounds__(256) scan_check_kernel(const ImgDesc* __restri
     const int i = t0 + threadIdx.x;
     const int v = i < im.nsub ? c[i] : 0;
     int tot;
-    const int e = block_excl_scan(v, &tot);
+    const int e = block_scan(v, warp_sums, &tot) - v;
     if (i < im.nsub) c[i] = base + e;
     base += tot;
   }
@@ -580,7 +554,7 @@ __global__ void dc_kernel(const ImgDesc* __restrict__ imgs, int nimg, const int*
     if (m < m1)
       for (int b = 0; b < im.bpm; ++b) sum[im.slot_comp[b]] += cb[(static_cast<int64_t>(m) * im.bpm + b) * 64];
     for (int ci = 0; ci < im.ncomp; ++ci) {
-      const int inc = warp_incl_scan(sum[ci]);
+      const int inc = warp_scan(sum[ci]);
       int run = carry[ci] + inc - sum[ci];
       if (m < m1)
         for (int b = 0; b < im.bpm; ++b)

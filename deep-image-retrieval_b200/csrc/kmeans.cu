@@ -22,6 +22,7 @@
 
 #include <algorithm>
 
+#include "block.cuh"
 #include "common.h"
 #include "exact_dot.cuh"
 
@@ -36,27 +37,6 @@ constexpr int PP_ROWS = 256;       // rows per block of a k-means++ weight launc
 constexpr double FIX32 = 4294967296.0;
 
 unsigned grid_for(int64_t n) { return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, KM_THREADS), 8192))); }
-
-// Inclusive scan of one value per thread over a block of KM_SCAN threads; *total receives the block's sum.
-__device__ long long block_scan_incl(long long v, long long* warp_sums, long long* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  long long incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long y = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += y;
-  }
-  if (lane == 31) warp_sums[warp] = incl;
-  __syncthreads();
-  long long before = 0, tot = 0;
-  for (int w = 0; w < KM_SCAN / 32; ++w) {
-    if (w < warp) before += warp_sums[w];
-    tot += warp_sums[w];
-  }
-  __syncthreads();
-  *total = tot;
-  return incl + before;
-}
 
 // acc[0] = labels that differ from prev (every row when prev is null), acc[1] = sum of rint(score * 2^32).
 __global__ void km_stats_kernel(const int64_t* __restrict__ labels, const double* __restrict__ scores,
@@ -102,7 +82,7 @@ __global__ void __launch_bounds__(KM_SCAN) km_offsets_kernel(const int* __restri
     const int c = base + threadIdx.x;
     const long long v = c < k ? counts[c] : 0;
     long long tot;
-    const long long incl = block_scan_incl(v, warp_sums, &tot);
+    const long long incl = block_scan(v, warp_sums, &tot);
     if (c < k) off[c] = carry + incl - v;
     carry += tot;
   }
@@ -249,7 +229,7 @@ __global__ void __launch_bounds__(KM_SCAN) km_pp_select_kernel(const long long* 
   long long part = 0;
   for (int64_t b = threadIdx.x; b < nb; b += KM_SCAN) part += bsum[b];
   long long T;
-  block_scan_incl(part, warp_sums, &T);
+  block_scan(part, warp_sums, &T);
   if (T == 0) {
     if (threadIdx.x == 0) chosen[j] = -1;
     return;
@@ -261,7 +241,7 @@ __global__ void __launch_bounds__(KM_SCAN) km_pp_select_kernel(const long long* 
     const int64_t b = base + threadIdx.x;
     const long long v = b < nb ? bsum[b] : 0;
     long long tot;
-    const long long incl = carry + block_scan_incl(v, warp_sums, &tot);
+    const long long incl = carry + block_scan(v, warp_sums, &tot);
     if (b < nb && incl > t && incl - v <= t) {
       s_blk = b;
       s_before = incl - v;
@@ -272,7 +252,7 @@ __global__ void __launch_bounds__(KM_SCAN) km_pp_select_kernel(const long long* 
   const int64_t i = s_blk * PP_ROWS + threadIdx.x;
   const long long v = (threadIdx.x < PP_ROWS && i < n) ? w[i] : 0;
   long long tot;
-  const long long incl = s_before + block_scan_incl(v, warp_sums, &tot);
+  const long long incl = s_before + block_scan(v, warp_sums, &tot);
   if (v > 0 && incl > t && incl - v <= t) {
     chosen[j] = i;
     flag[i] = 1;

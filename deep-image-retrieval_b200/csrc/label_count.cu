@@ -32,6 +32,7 @@
 #include <atomic>
 #include <vector>
 
+#include "block.cuh"
 #include "conv.h"
 #include "dmma.cuh"
 #include "exact_dot.cuh"
@@ -309,13 +310,7 @@ __global__ void count_scan_kernel(int Q, const int* __restrict__ thr_off, unsign
   for (int b = thr_off[q]; b < thr_off[q + 1]; b += 32) {
     const int t = b + lane;
     const bool in = t < thr_off[q + 1];
-    unsigned long long v = in ? c[t] : 0ull;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned long long u = __shfl_up_sync(0xffffffffu, v, o);
-      if (lane >= o) v += u;
-    }
-    v += carry;
+    const unsigned long long v = warp_scan(in ? c[t] : 0ull) + carry;
     if (in) c[t] = v;
     carry = __shfl_sync(0xffffffffu, v, 31);
   }

@@ -12,13 +12,14 @@
 //   pq_scan_kernel     P5: one CTA per (query, group of probes): the query's table in shared memory, one thread per
 //                      list row; a = fl32(e(q, c)), then a = fl32(a + T[m][code_m]) for m ascending.  Dense output in
 //                      the query's segment of the block (qoff), probes in probe order.
-//   pq_select_kernel   P6: one CTA per query: radix select (8 passes of 8 bits) of the R-th largest key (a desc, row
-//                      asc) over the query's segment, then the rows with a key >= it.
+//   pq_select_kernel   P6: one CTA per query: radix select (block_radix_kth, 8 passes of 8 bits) of the R-th largest
+//                      key (a desc, row asc) over the query's segment, then the rows with a key >= it.
 //   pq_refine_kernel   P7: one warp per candidate, exact_dot_warp; sort_runs_merge orders them (e desc, row asc).
 #include <math.h>
 
 #include <algorithm>
 
+#include "block.cuh"
 #include "common.h"
 #include "exact_dot.cuh"
 
@@ -204,50 +205,22 @@ __global__ void __launch_bounds__(PQ_THREADS) pq_scan_kernel(const float* __rest
 
 // (a desc, row asc) as one unsigned key, larger = earlier; -0 and +0 are the same score.
 __device__ __forceinline__ uint64_t adc_key(float a, int row) {
-  uint32_t u = __float_as_uint(a == 0.f ? 0.f : a);
-  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-  return (static_cast<uint64_t>(u) << 32) | static_cast<uint32_t>(0x7fffffff - row);
+  return (static_cast<uint64_t>(f2key(a == 0.f ? 0.f : a)) << 32) | static_cast<uint32_t>(0x7fffffff - row);
 }
 
 __global__ void __launch_bounds__(SEL_THREADS) pq_select_kernel(const float* __restrict__ a, const int* __restrict__ arow,
                                                                 const int64_t* __restrict__ qoff, int R, int cap2,
                                                                 int* __restrict__ rows, int* __restrict__ cnt) {
-  __shared__ int hist[256];
-  __shared__ int s_bin, s_need, s_slot;
+  __shared__ uint32_t hist[256], bc[2];
+  __shared__ int s_slot;
   const int q = blockIdx.x;
   const int64_t b = qoff[q], n = qoff[q + 1] - b;
   int* out = rows + static_cast<int64_t>(q) * cap2;
   if (threadIdx.x == 0) s_slot = 0;
   __syncthreads();
-  uint64_t thr = 0;
-  if (n > R) {
-    uint64_t prefix = 0, mask = 0;
-    int need = R;
-    for (int shift = 56; shift >= 0; shift -= 8) {
-      for (int i = threadIdx.x; i < 256; i += SEL_THREADS) hist[i] = 0;
-      __syncthreads();
-      for (int64_t i = threadIdx.x; i < n; i += SEL_THREADS) {
-        const uint64_t k = adc_key(a[b + i], arow[b + i]);
-        if ((k & mask) == prefix) atomicAdd(&hist[(k >> shift) & 255], 1);
-      }
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        int cum = 0, bin = 0;
-        for (bin = 255; bin > 0; --bin) {
-          if (cum + hist[bin] >= need) break;
-          cum += hist[bin];
-        }
-        s_bin = bin;
-        s_need = need - cum;
-      }
-      __syncthreads();
-      prefix |= static_cast<uint64_t>(s_bin) << shift;
-      mask |= 255ull << shift;
-      need = s_need;
-      __syncthreads();
-    }
-    thr = prefix;   // the R-th largest key: keys are distinct, so exactly R rows reach it
-  }
+  // the R-th largest key: keys are distinct, so exactly R rows reach it
+  const uint64_t thr =
+      n > R ? block_radix_kth<uint64_t>([&](int64_t i) { return adc_key(a[b + i], arow[b + i]); }, n, R, hist, bc) : 0;
   for (int64_t i = threadIdx.x; i < n; i += SEL_THREADS)
     if (n <= R || adc_key(a[b + i], arow[b + i]) >= thr) out[atomicAdd(&s_slot, 1)] = arow[b + i];
   __syncthreads();

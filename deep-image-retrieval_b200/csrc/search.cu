@@ -35,6 +35,7 @@
 #include <string>
 #include <vector>
 
+#include "block.cuh"
 #include "conv.h"
 #include "conv_pers.cuh"
 #include "exact_dot.cuh"
@@ -45,14 +46,6 @@ namespace {
 
 constexpr int SEL_THREADS = 512;
 
-__device__ __forceinline__ uint32_t f2key(float f) {  // monotone increasing map float -> uint32
-  const uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key2f(uint32_t k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
 struct DenseAcc {
   const float* p;
   __device__ float operator()(int i) const { return p[i]; }
@@ -62,68 +55,11 @@ struct CandAcc {
   __device__ float operator()(int i) const { return __uint_as_float(static_cast<uint32_t>(p[i] >> 32)); }
 };
 
-// k-th largest of n values (block-wide MSB-first radix select, 4 passes of 8 bits). n < k -> -inf.
+// k-th largest of n values (block_radix_kth on f2key). n < k -> -inf.
 template <class Acc>
 __device__ float block_kth_largest(Acc acc, int n, int k, uint32_t* hist /*[256]*/, uint32_t* bc /*[2]*/) {
   if (n < k) return -INFINITY;
-  uint32_t prefix = 0, mask = 0;
-  int kk = k;
-  for (int pass = 3; pass >= 0; --pass) {
-    const int shift = pass * 8;
-    for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0;
-    __syncthreads();
-    // similarity scores share their high bits, so most keys of a pass land in one or two bins: aggregate the
-    // lanes of a warp that hit the same bin and let one of them add the whole group
-    const int n_round = (n + 31) & ~31;
-    for (int i = threadIdx.x; i < n_round; i += blockDim.x) {
-      uint32_t bin = 0xffffffffu;
-      if (i < n) {
-        const uint32_t key = f2key(acc(i));
-        if ((key & mask) == prefix) bin = (key >> shift) & 255u;
-      }
-      const uint32_t peers = __match_any_sync(0xffffffffu, bin);
-      if (bin != 0xffffffffu && (threadIdx.x & 31) == (__ffs(peers) - 1)) atomicAdd(&hist[bin], static_cast<uint32_t>(__popc(peers)));
-    }
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      // Find the bin holding the kk-th largest key: lane l owns bins [8l, 8l+8); a suffix scan over the lanes gives
-      // the number of keys in higher bins, the owning lane walks its 8 bins.  (A single thread walking 256 bins
-      // serially cost ~10 us per pass.)
-      const int lane = threadIdx.x;
-      uint32_t loc[8], sum = 0;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        loc[j] = hist[8 * lane + j];
-        sum += loc[j];
-      }
-      uint32_t suf = sum;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t v = __shfl_down_sync(0xffffffffu, suf, o);
-        if (lane + o < 32) suf += v;
-      }
-      const uint32_t above = suf - sum;
-      const uint32_t want = static_cast<uint32_t>(kk);
-      if (above < want && want <= above + sum) {
-        uint32_t cum = above;
-#pragma unroll
-        for (int j = 7; j >= 0; --j) {
-          if (cum + loc[j] >= want) {
-            bc[0] = 8 * lane + j;
-            bc[1] = want - cum;
-            break;
-          }
-          cum += loc[j];
-        }
-      }
-    }
-    __syncthreads();
-    prefix |= bc[0] << shift;
-    mask |= 255u << shift;
-    kk = bc[1];
-    __syncthreads();
-  }
-  return key2f(prefix);
+  return key2f(block_radix_kth<uint32_t>([&](int i) { return f2key(acc(i)); }, n, k, hist, bc));
 }
 
 // thr[q] = (k-th largest of dense[q][0..S)) - band; k2 > 0: also thr2[q] = (k2-th largest) - band (the seed bound a shard
@@ -419,23 +355,8 @@ __global__ void __launch_bounds__(FIN_THREADS) search_finish_kernel(
     ix[i] = INT_MAX;
   }
   __syncthreads();
-  for (int size = 2; size <= P; size <<= 1) {
-    for (int st = size >> 1; st > 0; st >>= 1) {
-      for (int i = threadIdx.x; i < P / 2; i += FIN_THREADS) {
-        const int lo = 2 * i - (i & (st - 1));
-        const int hi = lo + st;
-        const bool up = ((lo & size) == 0);  // "up" = this block sorted best-first
-        const double va = sc[lo], vb = sc[hi];
-        const int ia = ix[lo], ib = ix[hi];
-        const bool a_first = (va > vb) || (va == vb && ia < ib);
-        if (a_first != up) {
-          sc[lo] = vb; sc[hi] = va;
-          ix[lo] = ib; ix[hi] = ia;
-        }
-      }
-      __syncthreads();
-    }
-  }
+  block_bitonic_sort<FIN_THREADS>(sc, ix, P,
+                                  [](double sa, int ia, double sb, int ib) { return ranks_before(sa, ia, sb, ib); });
   if (x.world > 0) {
     const size_t slot = (static_cast<size_t>(epoch & 1u) * x.world + x.rank) * x_list_elems(x.max_q, x.max_k) + static_cast<size_t>(q) * k;
     const size_t o_sc = x_off_score(x.world, x.max_q) + slot * 8, o_ix = x_off_idx(x.world, x.max_q, x.max_k) + slot * 8;
@@ -538,23 +459,8 @@ __global__ void __launch_bounds__(FIN_THREADS) deep_run_sort_kernel(const int* _
     ix[i] = ok ? surv_row[o + i] : INT_MAX;
   }
   __syncthreads();
-  for (int size = 2; size <= P; size <<= 1) {
-    for (int st = size >> 1; st > 0; st >>= 1) {
-      for (int i = threadIdx.x; i < P / 2; i += FIN_THREADS) {
-        const int lo = 2 * i - (i & (st - 1));
-        const int hi = lo + st;
-        const bool up = ((lo & size) == 0);
-        const double va = sc[lo], vb = sc[hi];
-        const int ia = ix[lo], ib = ix[hi];
-        const bool a_first = (va > vb) || (va == vb && ia < ib);
-        if (a_first != up) {
-          sc[lo] = vb; sc[hi] = va;
-          ix[lo] = ib; ix[hi] = ia;
-        }
-      }
-      __syncthreads();
-    }
-  }
+  block_bitonic_sort<FIN_THREADS>(sc, ix, P,
+                                  [](double sa, int ia, double sb, int ib) { return ranks_before(sa, ia, sb, ib); });
   for (int i = threadIdx.x; i < SORT_RUN; i += FIN_THREADS) {
     const bool ok = i < n;
     surv_sc[o + i] = ok ? sc[i] : -INFINITY;
@@ -730,7 +636,7 @@ __global__ void __launch_bounds__(RC_THREADS) rank_count_kernel(
       const int row = band[w];
       const double sc = exact_dot_warp(q32 + static_cast<int64_t>(q) * D, db32 + static_cast<int64_t>(row) * D, D, lane);
       const int64_t g = static_cast<int64_t>(row) + offset;
-      if (lane == 0 && g != trow && (sc > s || (sc == s && g < trow))) ++mine;
+      if (lane == 0 && g != trow && ranks_before(sc, g, s, trow)) ++mine;
     }
     for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
     if (lane == 0 && mine) atomicAdd(&s_count, static_cast<unsigned long long>(mine));
@@ -761,7 +667,7 @@ __global__ void __launch_bounds__(RCE_THREADS) rank_count_exact_kernel(
       if (!t_flags[t0 + i]) continue;
       const double s = t_score[t0 + i];
       const int64_t trow = t_rows[t0 + i];
-      if (g != trow && (sc > s || (sc == s && g < trow))) atomicAdd(&cnts[i], 1u);
+      if (g != trow && ranks_before(sc, g, s, trow)) atomicAdd(&cnts[i], 1u);
     }
   }
   __syncthreads();
@@ -809,18 +715,8 @@ __global__ void __launch_bounds__(1024) merge_lists_kernel(const double* in_scor
     if (ie < 0) continue;
     ++my_valid;
     int rank = j;
-    for (int h = 0; h < G; ++h) {
-      if (h == g) continue;
-      const double* hs = sc + h * k;
-      const int64_t* hi = ix + h * k;
-      int lo = 0, hi_ = k;                      // first position of list h that does NOT come before (se, ie)
-      while (lo < hi_) {
-        const int mid = (lo + hi_) >> 1;
-        const bool before = hi[mid] >= 0 && (hs[mid] > se || (hs[mid] == se && hi[mid] < ie));
-        if (before) lo = mid + 1; else hi_ = mid;
-      }
-      rank += lo;
-    }
+    for (int h = 0; h < G; ++h)
+      if (h != g) rank += rank_in_run(sc + h * k, ix + h * k, k, se, ie, [](auto p) { return *p; });
     if (rank < k) {
       out_score[static_cast<int64_t>(q) * k + rank] = se;
       out_idx[static_cast<int64_t>(q) * k + rank] = ie;
@@ -865,20 +761,9 @@ __global__ void merge_runs_kernel(const double* __restrict__ in_score, const int
     const int64_t ie = __ldcg(iq + g * run_stride + j);
     if (ie < 0) continue;
     int rank = j;
-    for (int h = 0; h < Gq && rank < k; ++h) {
-      if (h == g) continue;
-      const double* hs = sq + h * run_stride;
-      const int64_t* hi = iq + h * run_stride;
-      int lo = 0, hi_ = Lk;                     // first position of run h that does NOT come before (se, ie)
-      while (lo < hi_) {
-        const int mid = (lo + hi_) >> 1;
-        const int64_t im = __ldcg(hi + mid);
-        const double sm = __ldcg(hs + mid);
-        const bool before = im >= 0 && (sm > se || (sm == se && im < ie));
-        if (before) lo = mid + 1; else hi_ = mid;
-      }
-      rank += lo;
-    }
+    for (int h = 0; h < Gq && rank < k; ++h)
+      if (h != g)
+        rank += rank_in_run(sq + h * run_stride, iq + h * run_stride, Lk, se, ie, [](auto p) { return __ldcg(p); });
     if (rank < k) {
       out_score[static_cast<int64_t>(q) * k + rank] = se;
       out_idx[static_cast<int64_t>(q) * k + rank] = ie;
@@ -1139,10 +1024,6 @@ __global__ void nearest_prep_kernel(const float* __restrict__ q32, __half* __res
     q16[i] = __float2half_rn(q32[i]);
 }
 
-__device__ __forceinline__ bool nearest_better(double s, int64_t c, double bs, int64_t bc) {
-  return s > bs || (s == bs && c < bc);
-}
-
 __global__ void __launch_bounds__(NEAREST_THREADS) nearest_kernel(const float* __restrict__ G, int ng, const float* __restrict__ q32,
                                                                   const float* __restrict__ db32, int64_t K, int D,
                                                                   double eps16, int cap, int64_t offset,
@@ -1183,7 +1064,7 @@ __global__ void __launch_bounds__(NEAREST_THREADS) nearest_kernel(const float* _
     const int64_t c = full ? j : static_cast<int64_t>(groups[j >> 5]) * 32 + (j & 31);
     if (c >= K) continue;                                      // uniform over the warp
     const double e = exact_dot_warp(a, db32 + c * D, D, lane);
-    if (nearest_better(e, c, bs, bc)) { bs = e; bc = c; }
+    if (ranks_before(e, c, bs, bc)) { bs = e; bc = c; }
     ++scored;
   }
   if (lane == 0) {
@@ -1194,7 +1075,7 @@ __global__ void __launch_bounds__(NEAREST_THREADS) nearest_kernel(const float* _
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int w = 1; w < NEAREST_THREADS / 32; ++w)
-      if (nearest_better(best_s[w], best_c[w], bs, bc)) { bs = best_s[w]; bc = best_c[w]; }
+      if (ranks_before(best_s[w], best_c[w], bs, bc)) { bs = best_s[w]; bc = best_c[w]; }
     labels[q] = offset + bc;
     scores[q] = bs;
     if (nc > 1) atomicAdd(stats, 1ull);
@@ -2428,27 +2309,6 @@ enum { LT_PAIRS = 0, LT_SLOTS = 1, LT_TILES = 2, LT_GROUPS = 3, LT_ROWS = 4, LT_
 
 __device__ __forceinline__ int64_t list_size(const int64_t* cell_off, int c) { return cell_off[c + 1] - cell_off[c]; }
 
-// Inclusive scan of one value per thread over a block of `nthreads` threads (a multiple of 32); *total = block sum.
-__device__ long long ivf_block_scan(long long v, long long* warp_sums, long long* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  long long incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long y = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += y;
-  }
-  if (lane == 31) warp_sums[warp] = incl;
-  __syncthreads();
-  long long before = 0, tot = 0;
-  for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) {
-    if (w < warp) before += warp_sums[w];
-    tot += warp_sums[w];
-  }
-  __syncthreads();
-  *total = tot;
-  return incl + before;
-}
-
 // M[c][q] = j + 1 for probe j of query q (M cleared before); a probe outside [0, K) or a list probed twice is an error.
 __global__ void ivf_mark_kernel(const int64_t* __restrict__ probes, int nq, int np, int K, int* __restrict__ M,
                                 long long* __restrict__ tot) {
@@ -2516,9 +2376,9 @@ __global__ void __launch_bounds__(IVF_SCAN) ivf_scan_kernel(const int* __restric
       }
     }
     long long t1, t2, t3;
-    const long long is = ivf_block_scan(slots, ws, &t1);
-    const long long it = ivf_block_scan(tiles, ws, &t2);
-    ivf_block_scan(pairs, ws, &t3);
+    const long long is = block_scan(slots, ws, &t1);
+    const long long it = block_scan(tiles, ws, &t2);
+    block_scan(pairs, ws, &t3);
     if (c < K) {
       seg_off[c] = cs + is - slots;
       tile_off[c] = ct + it - tiles;
@@ -2532,7 +2392,7 @@ __global__ void __launch_bounds__(IVF_SCAN) ivf_scan_kernel(const int* __restric
     const int q = base + threadIdx.x;
     const long long v = q < nq ? qgroups[q] : 0;
     long long t;
-    const long long incl = ivf_block_scan(v, ws, &t);
+    const long long incl = block_scan(v, ws, &t);
     if (q < nq) qgoff[q] = cg + incl - v;
     cg += t;
   }
@@ -2568,7 +2428,7 @@ __global__ void __launch_bounds__(IVF_THREADS) ivf_list_fill_kernel(const int* _
     const int q = base + threadIdx.x;
     const int j1 = q < nq ? M[static_cast<int64_t>(c) * nq + q] : 0;
     long long t;
-    const long long incl = ivf_block_scan(j1 != 0, ws, &t);
+    const long long incl = block_scan<long long>(j1 != 0, ws, &t);
     if (j1 != 0) {
       const int64_t s = s0 + carry + incl - 1;
       slot_q[s] = q;

@@ -110,7 +110,10 @@ def built():
     index.close()
 
 
-@pytest.mark.parametrize("nprobe,k,R", [(1, 10, 10), (2, 10, 40), (3, 50, 200), (6, 1, 3000), (2, 100, 100)])
+# (1, 10, 310): query 29 has rows 5 and 11 (equal codes, equal ADC scores) at positions 310 and 311, so the R-th key is
+# decided by the row bits
+@pytest.mark.parametrize("nprobe,k,R", [(1, 10, 10), (2, 10, 40), (3, 50, 200), (6, 1, 3000), (2, 100, 100),
+                                        (1, 10, 310)])
 def test_search_equals_model(built, nprobe, k, R):
     b = built
     assert np.array_equal(b["codes"], b["index"].codes_.cpu().numpy())
