@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["common.cu", "conv.cu", "ops.cu", "search.cu", "net.cu", "api.cu", "resize.cu", "label_count.cu", "jpeg.cu", "pca.cu",
-           "aploss.cu", "diffusion.cu", "diffusion_trunc.cu", "join.cu", "kmeans.cu", "pq.cu"]
+           "aploss.cu", "diffusion.cu", "diffusion_trunc.cu", "join.cu", "kmeans.cu", "pq.cu", "graph.cu"]
 LIB = os.path.join(HERE, "libdirb200.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]

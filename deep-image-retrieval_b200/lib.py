@@ -159,6 +159,11 @@ SIGNATURES = {
     "dirb200_pq_tables": (i32, [p, i32, i32, p, i32, p, p]),
     "dirb200_pq_search_ws_bytes": (C.c_size_t, [i32, i64, i32]),
     "dirb200_pq_search": (i32, [p, i32, i32, p, i32, p, p, i32, p, p, p, p, i64, p, i32, i32, p, p, p, p, p]),
+    # graph search over a pruned kNN graph: forward edges, reverse edges merged in, best-first traversal
+    "dirb200_graph_prune": (i32, [p, i64, i32, i32, p, p]),
+    "dirb200_graph_merge": (i32, [p, i64, i32, p, p, p, p]),
+    "dirb200_graph_search_smem_bytes": (C.c_size_t, [i32, i32, i32, i32, i32]),
+    "dirb200_graph_search": (i32, [p, i32, i32, p, i64, p, i32, p, i32, i32, i32, i32, i32, p, p, p, p, p, p, p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

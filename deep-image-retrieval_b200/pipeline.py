@@ -423,6 +423,41 @@ def _aps_from_ivf(db, qdescs, bdescs, params):
     return _grade(db.eval_query_AP_from_truncated_counts, offs, rows, inside, sc, rank)
 
 
+def _aps_from_graph(db, qdescs, bdescs, params):
+    """Per-query AP with graph-search ranking (extension; DESIGN.md section 4.12, rule G8): the pruned kNN graph of the
+    database rows (GraphIndex), each query ranks the rows its traversal visited, V_q, first, in exact order, then every
+    other row in exact order; a junk row ranks before a positive by (inside V_q, score, index)."""
+    from .graph import GraphIndex
+    qd, bd = rows64(qdescs), rows64(bdescs)
+    offs, rows, flags = _rank_target_csr(db, qd.shape[0])
+    build = {k: params[k] for k in ("degree", "build_k", "n_entry", "seed") if k in params}
+    walk = {k: params[k] for k in ("itopk", "width", "max_iter", "n_seeds") if k in params}
+    index = GraphIndex(bd, **build)
+    walk["n_seeds"] = min(walk.get("n_seeds", 16), index.entry_.shape[0])     # see eval_model
+    exact = ops.Index(bd)
+    try:
+        inside, sc, rank = index.rank_counts(qd, offs, rows, flags, exact=exact, **walk)
+    finally:
+        exact.close()
+        index.close()
+    return _grade(db.eval_query_AP_from_truncated_counts, offs, rows, inside, sc, rank)
+
+
+def graph_params(values):
+    """--graph DEGREE ITOPK -> the eval_model `graph` dict (integers, 1 <= DEGREE <= 128, ITOPK >= 1)."""
+    from .graph import MAX_DEGREE
+    if len(values) != 2:
+        raise ValueError("--graph takes DEGREE ITOPK (got %d values)" % len(values))
+    out = {}
+    for key, v in zip(("degree", "itopk"), values):
+        if float(v) != int(v) or int(v) < 1:
+            raise ValueError("--graph: %s must be an integer >= 1 (got %r)" % (key.upper(), v))
+        out[key] = int(v)
+    if out["degree"] > MAX_DEGREE:
+        raise ValueError("--graph: DEGREE must be at most %d (got %d)" % (MAX_DEGREE, out["degree"]))
+    return out
+
+
 def ivf_params(values):
     """--ivf NLIST NPROBE -> the eval_model `ivf` dict (integers, 1 <= NPROBE <= NLIST; NLIST <= N is checked by the
     k-means fit)."""
@@ -481,7 +516,7 @@ def diffusion_truncate(value):
 
 def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=None, aqe=None, adba=None, threads=8,
                batch_size=16, save_feats=None, load_feats=None, dbg=(), rank_topk=0, dense_scores=False, diffusion=None,
-               ivf=None):
+               ivf=None, graph=None):
     """Evaluate a network on a retrieval dataset (test_dir.py:97-180).  aqe / adba: dict(k=..., alpha=...).
     diffusion (extension): dict of dirb200.diffusion parameters (k, kq, gamma, alpha, iters, tol, and optionally
     truncate = m: each query solved on the subgraph of its own m nearest rows); the rows are then
@@ -492,6 +527,11 @@ def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=Non
     lists only (NotImplementedError otherwise), not together with diffusion (ValueError).  With pq=M (and refine=R,
     default 400) the lists hold product-quantisation codes and the ranking is rule P8's: the best R probed rows by ADC
     score first, in exact order, then every other row.
+    graph (extension): dict(degree=..., itopk=..., and optionally build_k, n_entry, seed, width, max_iter, n_seeds):
+    graph-search ranking (rule G8): the rows each query's traversal of the database's pruned kNN graph visited first,
+    in exact order, then every other row; relevance lists only, not together with ivf or diffusion (ValueError).
+    n_seeds (default 16) is lowered to the size of the entry sample, min(N, n_entry), when it exceeds it, so that the
+    default grades databases of fewer than 16 rows; GraphIndex.search itself refuses such an n_seeds.
     Ranking: datasets with relevance lists (Oxford/Paris style) are graded from GPU rank counts and label datasets
     from GPU threshold counts + the exact top-100 - no Q x N score matrix, no host argsort; dense_scores=True
     (extension) forces the literal matmul + per-query sort of the reference; rank_topk > 0 (extension) grades
@@ -537,7 +577,15 @@ def eval_model(db, net, trfs, pooling="mean", gemp=3, detailed=False, whiten=Non
     unit = bool(float((qn.norm(dim=1) - 1).abs().max()) < 1e-3 and float((bn.norm(dim=1) - 1).abs().max()) < 1e-3)
     if ivf is not None and diffusion is not None:
         raise ValueError("ivf and diffusion are two rankings: choose one")
-    if ivf is not None:
+    if graph is not None and (ivf is not None or diffusion is not None):
+        raise ValueError("graph and %s are two rankings: choose one" % ("ivf" if ivf is not None else "diffusion"))
+    if graph is not None:
+        if not hasattr(db, "eval_query_AP_from_truncated_counts"):
+            raise NotImplementedError("graph-search ranking grades datasets with relevance lists (Oxford / Paris "
+                                      "style) only; %s has none" % type(db).__name__)
+        aps = _aps_from_graph(db, qn, bn, graph)
+        scores = None
+    elif ivf is not None:
         if not hasattr(db, "eval_query_AP_from_truncated_counts"):
             raise NotImplementedError("inverted-file ranking grades datasets with relevance lists (Oxford / Paris "
                                       "style) only; %s has none" % type(db).__name__)
@@ -754,10 +802,18 @@ def test_dir_main(argv=None):
                              "query's best R probed rows by ADC score first, in exact order, then the other rows")
     parser.add_argument("--refine", type=int, default=None, metavar="R",
                         help="(extension, with --pq) rows re-ranked exactly per query (default 400)")
+    parser.add_argument("--graph", type=float, nargs="+", metavar="DEGREE ITOPK",
+                        help="(extension) rank by graph search: a pruned kNN graph of the database with DEGREE edges "
+                             "per row; the rows each query's traversal visits (running list of ITOPK) first, in exact "
+                             "order, then the other rows")
     args = parser.parse_args(argv)
     try:
         if args.ivf is not None and args.diffusion is not None:
             raise ValueError("--ivf and --diffusion are two rankings: choose one")
+        if args.graph is not None and (args.ivf is not None or args.diffusion is not None):
+            raise ValueError("--graph and --%s are two rankings: choose one"
+                             % ("ivf" if args.ivf is not None else "diffusion"))
+        graph = graph_params(args.graph) if args.graph is not None else None
         ivf = pq_params(ivf_params(args.ivf) if args.ivf is not None else None, args.pq, args.refine)
         diffusion = diffusion_params(args.diffusion) if args.diffusion is not None else None
         if args.diffusion_truncate is not None:
@@ -776,7 +832,7 @@ def test_dir_main(argv=None):
     res = eval_model(dataset, net, args.trfs, pooling=args.pooling, gemp=args.gemp, detailed=args.detailed,
                      threads=args.threads, dbg=args.dbg, whiten=whiten, aqe=aqe, adba=adba,
                      save_feats=args.save_feats, load_feats=args.load_feats, rank_topk=args.rank_topk,
-                     dense_scores=args.dense_scores, diffusion=diffusion, ivf=ivf)
+                     dense_scores=args.dense_scores, diffusion=diffusion, ivf=ivf, graph=graph)
     # (the reference's '%s = %g' line raises on the list-valued entries that --detailed adds; print scalars only)
     print(" * " + "\n * ".join(["%s = %g" % p for p in res.items() if isinstance(p[1], (int, float))]))
     if args.out_json:

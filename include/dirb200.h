@@ -623,6 +623,27 @@ int dirb200_pq_search(const float* q_dev, int Q, int D, const float* tables_dev,
                       const int64_t* list_off_dev, const int64_t* qoff_dev, int64_t total, const float* rows, int R,
                       int k, void* ws_dev, double* out_scores, int64_t* out_rows, double* ms, void* stream);
 
+/* Graph search over a pruned kNN graph of the database (DESIGN.md section 4.12, rules G1-G8).  Rows are int32; none of
+ * these synchronises the stream or needs a workspace.
+ * Rules G3 / G4: knn_dev [n][K] (row r's kNN list without r, -1 entries allowed, the non-negative entries of a row
+ * distinct), K <= 128 -> fwd_dev [n][degree] = F(r), -1 padded; degree <= 128 (else DIRB200_ENOTSUP). */
+int dirb200_graph_prune(const int* knn_dev, int64_t n, int K, int degree, int* fwd_dev, void* stream);
+/* Rule G5: fwd_dev [n][degree] of dirb200_graph_prune and Rev as a CSR (rev_off_dev [n + 1] int64, rev_src_dev the
+ * sources s of each target r ordered by (r's position in F(s), s)) -> graph_dev [n][degree], -1 padded. */
+int dirb200_graph_merge(const int* fwd_dev, int64_t n, int degree, const int64_t* rev_off_dev, const int* rev_src_dev,
+                        int* graph_dev, void* stream);
+/* The shared memory one query of dirb200_graph_search takes (0 for bad arguments, SIZE_MAX beyond any device). */
+size_t dirb200_graph_search_smem_bytes(int n_seeds, int itopk, int width, int degree, int max_iter);
+/* Rule G7 for Q queries (q_dev [Q][D] fp32, D % 4 == 0) over x_dev [n][D] fp32 and graph_dev [n][degree], from the
+ * seeds_dev [Q][n_seeds] (distinct rows, rule G6) -> out_scores fp64 / out_rows int64 [Q][k] (k <= itopk), padded
+ * (-inf, -1); n_visited [Q] = |V|, n_iter [Q] = the iterations run.  vis_rows int64 / vis_scores fp64 [Q][n_seeds +
+ * max_iter * width * degree], or both null: V in arrival order with its exact scores (entries past |V| unwritten).
+ * Parameters whose shared memory exceeds the device's per-block opt-in limit are DIRB200_EINVAL. */
+int dirb200_graph_search(const float* q_dev, int Q, int D, const float* x_dev, int64_t n, const int* graph_dev,
+                         int degree, const int* seeds_dev, int n_seeds, int itopk, int width, int max_iter, int k,
+                         double* out_scores, int64_t* out_rows, int64_t* vis_rows, double* vis_scores, int* n_visited,
+                         int* n_iter, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
