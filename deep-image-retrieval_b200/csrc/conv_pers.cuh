@@ -30,7 +30,7 @@
 namespace dirb {
 
 enum { PERS_EPI_CONV = 0, PERS_EPI_SIM_DENSE = 1, PERS_EPI_SIM_FILTER = 2, PERS_EPI_SIM_GMAX = 3, PERS_EPI_F32 = 4,
-       PERS_EPI_SIM_JOIN = 5, PERS_EPI_SIM_LGMAX = 6, PERS_EPI_SIM_LFILTER = 7 };
+       PERS_EPI_SIM_JOIN = 5, PERS_EPI_SIM_LGMAX = 6, PERS_EPI_SIM_LFILTER = 7, PERS_EPI_SIM_FILTER_ALLOW = 8 };
 
 struct ConvPersParams {
   int a_spatial, taps, kw_taps, cin_blocks, stride, pad;
@@ -76,6 +76,10 @@ struct ConvPersParams {
   const int* slot_q;
   const int64_t* perm;
   const int64_t* gbase;
+  // PERS_EPI_SIM_FILTER_ALLOW (filtered search): the filter pass keeps column n of query row q only if bit allow_bit0 + n
+  // of the allow bitmap's row q is set (word b >> 5, bit b & 31); allow_ld = words per query row, 0 = one row shared.
+  const uint32_t* allow;
+  int64_t allow_ld, allow_bit0;
 };
 
 // Whether accumulator row r of tile c lies inside its image's extent (ragged batches; true without an extent table).
@@ -565,18 +569,38 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       for (int h = 0; h < 2; ++h) {
         const int64_t qi = static_cast<int64_t>(c.m_tile) * 128 + r0 + 8 * h;
         const bool valid = qi < p.M;
-        if (EPI == PERS_EPI_SIM_FILTER || EPI == PERS_EPI_SIM_JOIN) {
+        if (EPI == PERS_EPI_SIM_FILTER || EPI == PERS_EPI_SIM_JOIN || EPI == PERS_EPI_SIM_FILTER_ALLOW) {
           // every match of the row (score >= the query's threshold) is appended to its candidate list: the four threads
           // holding a row reserve their slots with ONE atomicAdd and split them by a prefix sum over the quad.  The
           // self-join keeps only the columns after the row (col > row: the pair (i, j) once, i < j, never (i, i)).
+          // The filtered search keeps only the columns whose allow bit is set: aw[g] holds the bits of the tile's
+          // columns 32g .. 32g + 31, funnel-shifted out of the bitmap's words (allow_bit0 need not be a multiple of 32).
           constexpr bool JOIN = EPI == PERS_EPI_SIM_JOIN;
+          constexpr bool ALLOW = EPI == PERS_EPI_SIM_FILTER_ALLOW;
           const float t_q = valid ? __ldg(p.thr + qi) : INFINITY;
+          uint32_t aw[ALLOW ? BN / 32 : 1];
+          if constexpr (ALLOW) {
+            const int64_t b0 = p.allow_bit0 + static_cast<int64_t>(c.n_tile) * BN;   // bit of the tile's column 0
+            const int64_t w_last = (p.allow_bit0 + p.N - 1) >> 5;                   // last word holding a row's bit
+            const uint32_t* wq = p.allow + (valid ? qi : 0) * p.allow_ld;
+            const int sh = static_cast<int>(b0 & 31);
+            uint32_t lo = valid ? __ldg(wq + (b0 >> 5)) : 0u;
+#pragma unroll
+            for (int g = 0; g < BN / 32; ++g) {
+              const int64_t w = (b0 >> 5) + g + 1;
+              const uint32_t hi = (valid && w <= w_last) ? __ldg(wq + w) : 0u;
+              aw[g] = __funnelshift_r(lo, hi, sh);
+              lo = hi;
+            }
+          }
+          auto allowed = [&](int cl) { return !ALLOW || ((aw[ALLOW ? cl >> 5 : 0] >> (cl & 31)) & 1u); };
           int cnt = 0;
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             const int col = c.n_tile * BN + j * 8 + 2 * t4;
-            cnt += (acc[0][4 * j + 2 * h] >= t_q && col < p.N && (!JOIN || col > qi)) ? 1 : 0;
-            cnt += (acc[0][4 * j + 2 * h + 1] >= t_q && col + 1 < p.N && (!JOIN || col + 1 > qi)) ? 1 : 0;
+            cnt += (acc[0][4 * j + 2 * h] >= t_q && col < p.N && (!JOIN || col > qi) && allowed(j * 8 + 2 * t4)) ? 1 : 0;
+            cnt += (acc[0][4 * j + 2 * h + 1] >= t_q && col + 1 < p.N && (!JOIN || col + 1 > qi) && allowed(j * 8 + 2 * t4 + 1))
+                       ? 1 : 0;
           }
           int incl = cnt;
 #pragma unroll
@@ -597,7 +621,7 @@ conv_pers_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               for (int e = 0; e < 2; ++e) {
                 const float v = acc[0][4 * j + 2 * h + e];
                 const int col = c.n_tile * BN + j * 8 + 2 * t4 + e;
-                if (v >= t_q && col < p.N && (!JOIN || col > qi)) {
+                if (v >= t_q && col < p.N && (!JOIN || col > qi) && allowed(j * 8 + 2 * t4 + e)) {
                   if (pos < p.cand_cap)
                     dst[pos] = (static_cast<unsigned long long>(__float_as_uint(v)) << 32) | static_cast<unsigned int>(col);
                   ++pos;

@@ -25,6 +25,10 @@
 // captured and re-runs the filter pass.  With several shards the phases are split (search_begin / search_finish)
 // so that the caller can MIN-reduce the per-shard selection thresholds in between (see cand_kth_kernel).
 // The GEMMs run on the persistent warp-specialised kernel of conv_pers.cuh (128 x 128 tiles, K = D).
+// Filtered search (an allow bitmap attached with dirb200_index_set_allow, DESIGN.md section 4.13, rules F1-F6): the seed
+// rows are the first S rows allowed for every query of the block, gathered into a buffer of their own (allow_and_kernel,
+// allow_seed_rows_kernel, allow_gather_kernel, allow_kth_kernel), and the filter pass tests each column's bit
+// (PERS_EPI_SIM_FILTER_ALLOW; always the GEMM pass, never the dense scan of step 3).  Steps 4-5 are unchanged.
 #include <math.h>
 
 #include <limits.h>
@@ -191,6 +195,102 @@ __global__ void fill_empty_result_kernel(double* __restrict__ sc, int64_t* __res
   if (i < n) {
     sc[i] = -INFINITY;
     ix[i] = -1;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Seed of the filtered search (rule F2).  The allow bitmap is in global row numbering: local row r of this shard is bit
+// bit0 + r of a query's row of words (ld words apart; ld = 0: one row shared by every query).
+// iw[j] = AND over the nrow bitmap rows of the bits of local rows 32j .. 32j + 31 (rows >= N cleared).
+__global__ void allow_and_kernel(const uint32_t* __restrict__ allow, int64_t ld, int64_t bit0, int nrow, int64_t N,
+                                 uint32_t* __restrict__ iw) {
+  const int64_t j = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (j >= (N + 31) >> 5) return;
+  const int64_t b = bit0 + 32 * j, w = b >> 5;
+  const int sh = static_cast<int>(b & 31);
+  const bool two = sh != 0 && (w + 1) * 32 < bit0 + N;      // the window spans two words
+  uint32_t v = 0xffffffffu;
+#pragma unroll 4
+  for (int q = 0; q < nrow; ++q) {
+    const uint32_t* a = allow + q * ld;
+    v &= __funnelshift_r(__ldg(a + w), two ? __ldg(a + w + 1) : 0u, sh);
+  }
+  const int64_t rem = N - 32 * j;
+  if (rem < 32) v &= (1u << rem) - 1u;
+  iw[j] = v;
+}
+
+// The first S set bits of iw[0 .. W) in row order -> rows[0 .. n), *n_out = n = min(popcount, S).  One block; each thread
+// takes four words per step, and the block's popcounts are placed by one block_scan.
+constexpr int ALLOW_SCAN_THREADS = 1024;
+__global__ void __launch_bounds__(ALLOW_SCAN_THREADS) allow_seed_rows_kernel(const uint32_t* __restrict__ iw, int64_t W, int S,
+                                                                             int* __restrict__ rows, int* __restrict__ n_out) {
+  __shared__ int warp_sums[ALLOW_SCAN_THREADS / 32];
+  int base = 0;
+  for (int64_t w0 = 0; w0 < W && base < S; w0 += 4 * ALLOW_SCAN_THREADS) {
+    const int64_t j0 = w0 + 4 * static_cast<int64_t>(threadIdx.x);
+    uint32_t bits[4];
+    int cnt = 0;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      bits[e] = j0 + e < W ? __ldg(iw + j0 + e) : 0u;
+      cnt += __popc(bits[e]);
+    }
+    int total;
+    int pos = base + block_scan(cnt, warp_sums, &total) - cnt;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      uint32_t m = bits[e];
+      while (m != 0u && pos < S) {
+        rows[pos++] = static_cast<int>(32 * (j0 + e)) + __ffs(m) - 1;
+        m &= m - 1u;
+      }
+    }
+    base += total;                                 // the same on every thread: the loop ends for the whole block
+  }
+  if (threadIdx.x == 0) *n_out = min(base, S);
+}
+
+// seed16[p] = db16[rows[p]] for p < *n_seed (one warp per row, 16-byte copies); the rows past it are not written.
+__global__ void allow_gather_kernel(const __half* __restrict__ db16, int D, const int* __restrict__ rows,
+                                    const int* __restrict__ n_seed, int S, __half* __restrict__ seed16) {
+  const int p = static_cast<int>((blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
+  if (p >= S || p >= *n_seed) return;
+  const uint4* src = reinterpret_cast<const uint4*>(db16 + static_cast<int64_t>(__ldg(rows + p)) * D);
+  uint4* dst = reinterpret_cast<uint4*>(seed16 + static_cast<int64_t>(p) * D);
+  for (int i = lane; i < D / 8; i += 32) dst[i] = __ldg(src + i);
+}
+
+// kth_dense_kernel over the gathered seed rows: only the first *n_seed of the S rows hold allowed rows.  Group maxima
+// (gmax) count the full groups of 32 of them (all S rows valid: every group, the last one clipped by the GEMM itself);
+// fewer than k values give -inf (rule F2: no allowed row is certified).
+__global__ void __launch_bounds__(SEL_THREADS) allow_kth_kernel(const float* __restrict__ dense, int64_t ld, int S, int gmax,
+                                                                const int* __restrict__ n_seed, int k, float band,
+                                                                float* __restrict__ thr, int k2, float* __restrict__ thr2) {
+  __shared__ uint32_t hist[256];
+  __shared__ uint32_t bc[2];
+  const int q = blockIdx.x;
+  const int n = *n_seed;
+  const int n_vals = !gmax ? n : (n == S ? (S + 31) / 32 : n / 32);
+  const float t = block_kth_largest(DenseAcc{dense + q * ld}, n_vals, k, hist, bc);
+  if (threadIdx.x == 0) thr[q] = t - band;
+  if (k2 > 0) {
+    __syncthreads();
+    const float t2 = (k2 == k) ? t : block_kth_largest(DenseAcc{dense + q * ld}, n_vals, k2, hist, bc);
+    if (threadIdx.x == 0) thr2[q] = t2 - band;
+  }
+}
+
+// Clear bit rows[i] of bitmap row q for every i in [off[q], off[q + 1]) (rows outside [0, 32 ld) are skipped).
+// atomicAnd: the result does not depend on the order, and a row listed twice is cleared once.
+__global__ void allow_exclude_kernel(uint32_t* __restrict__ words, int64_t ld, const int64_t* __restrict__ off,
+                                     const int64_t* __restrict__ rows) {
+  const int q = blockIdx.x;
+  uint32_t* wq = words + q * ld;
+  for (int64_t i = off[q] + threadIdx.x; i < off[q + 1]; i += blockDim.x) {
+    const int64_t r = rows[i];
+    if (r >= 0 && r < 32 * ld) atomicAnd(wq + (r >> 5), ~(1u << (r & 31)));
   }
 }
 
@@ -922,6 +1022,9 @@ struct dirb200_index {
     // deep path (k > 1024): survivors in global memory, in sort_runs_merge's layout
     SortScratch surv{};
     int* surv_cnt = nullptr;
+    // filtered search: the bitmap rows of this block's queries (null = unfiltered)
+    const uint32_t* allow = nullptr;
+    int64_t allow_ld = 0, allow_bit0 = 0;
   } pend;
   // range search / self-join: workspace, options and the last result (CSR, kept until the next call)
   int join_cap = 0;                // candidate capacity per row of the first filter pass (0 = min(columns, 4096))
@@ -952,6 +1055,12 @@ struct dirb200_index {
   int profile = 0;                 // option "profile": time the phases of a search with CUDA events
   PhaseEvents<10> ev;              // separate from jev / lev: the list search's finish marks these
   double phase_ms[9] = {};
+  // filter of the exact search (dirb200_index_set_allow): caller-owned bitmap, words per query row (0 = shared), bit of
+  // local row 0; its seed buffers live in a workspace of their own
+  const uint32_t* allow = nullptr;
+  int64_t allow_ld = 0, allow_bit0 = 0;
+  void* aws = nullptr;
+  size_t aws_bytes = 0;
 };
 
 // Similarity GEMM on the persistent wgmma kernel (conv_pers.cuh): A = queries [Q][D], B = database rows [rows][D],
@@ -964,6 +1073,7 @@ struct SimArgs {
   const float* thr = nullptr; unsigned long long* cand = nullptr; int* cand_cnt = nullptr; int cand_cap = 0;
   const int* gate = nullptr;
   const int4* tiles = nullptr; int64_t n_tiles = 0; const int* slot_q = nullptr; const int64_t* gbase = nullptr;
+  const uint32_t* allow = nullptr; int64_t allow_ld = 0, allow_bit0 = 0;
 };
 static int sim_gemm(dirb200_index* h, int epi, const __half* q16, int64_t Q, const __half* db16, int64_t rows, int D,
                     const SimArgs& a, cudaStream_t stream) {
@@ -994,6 +1104,7 @@ static int sim_gemm(dirb200_index* h, int epi, const __half* q16, int64_t Q, con
   p.gate = a.gate;
   p.tiles = a.tiles; p.slot_q = a.slot_q; p.gbase = a.gbase;
   if (a.tiles) p.perm = h->lperm;
+  p.allow = a.allow; p.allow_ld = a.allow_ld; p.allow_bit0 = a.allow_bit0;
   const int sms = num_sms();
   switch (epi) {
     case PERS_EPI_SIM_DENSE: return conv_pers_launch<BN, 6, PERS_EPI_SIM_DENSE>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
@@ -1002,6 +1113,8 @@ static int sim_gemm(dirb200_index* h, int epi, const __half* q16, int64_t Q, con
     case PERS_EPI_SIM_LGMAX: return conv_pers_launch<BN, 6, PERS_EPI_SIM_LGMAX>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
     case PERS_EPI_SIM_LFILTER:
       return conv_pers_launch<BN, 6, PERS_EPI_SIM_LFILTER>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
+    case PERS_EPI_SIM_FILTER_ALLOW:
+      return conv_pers_launch<BN, 6, PERS_EPI_SIM_FILTER_ALLOW>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
     default: return conv_pers_launch<BN, 6, PERS_EPI_SIM_FILTER>(a_copy, b_copy, a_copy, a_copy, p, sms, stream);
   }
 }
@@ -1120,6 +1233,8 @@ int dirb200_index_set_db(dirb200_index* h, const float* db32_dev, const void* db
   h->lperm = nullptr;
   h->lcell_off = nullptr;
   h->lists_k = 0;
+  h->allow = nullptr;          // so does the filter: its bit0 numbered the old rows
+  h->allow_ld = h->allow_bit0 = 0;
   return 0;
 }
 
@@ -1197,6 +1312,7 @@ int dirb200_index_destroy(dirb200_index* h) {
   if (h->jws) cudaFree(h->jws);
   if (h->jws2) cudaFree(h->jws2);
   for (void* b : h->lws) if (b) cudaFree(b);
+  if (h->aws) cudaFree(h->aws);
   if (h->res_sc) cudaFree(h->res_sc);
   if (h->res_ix) cudaFree(h->res_ix);
   if (h->sel_own) cudaFree(h->sel_own);
@@ -1291,8 +1407,29 @@ static int search_max_queries(const dirb200_index* h, int k) {
   return lo;
 }
 
+// The seed buffers of a filtered search of depth k (rule F2): the gathered fp16 seed rows, their row numbers, the AND of
+// the block's bitmap rows over this shard's rows, and the number of seed rows found.  A workspace of its own (h->aws), so
+// that the unfiltered layout and the query block of dirb200_index_search_max_queries do not change.
+struct AllowWs {
+  __half* seed16;
+  int *rows, *n_seed;
+  uint32_t* iw;
+  size_t total;
+};
+static AllowWs allow_ws(void* base, const dirb200_index* h, int64_t S) {
+  Carver c(base);
+  AllowWs w;
+  w.seed16 = c.take<__half>(static_cast<size_t>(S) * h->dim);
+  w.rows = c.take<int>(S);
+  w.n_seed = c.take<int>(1);
+  w.iw = c.take<uint32_t>(static_cast<size_t>(ceil_div(h->N, 32)));
+  w.total = c.used;
+  return w;
+}
+
+// allow_row0: the block's first query within the rows of the attached bitmap (dirb200_index_search's query blocks).
 static int search_begin_seed(dirb200_index* h, const float* q32, int Q, int k, int k_shard, float* sel_dev, cudaStream_t stream,
-                             float* seed2) {
+                             float* seed2, int64_t allow_row0 = 0) {
   DIRB_REQUIRE(h && q32 && sel_dev, DIRB200_EINVAL, "null argument");
   DIRB_REQUIRE(h->has_db, DIRB200_ESTATE, "index has no database attached");
   DIRB_REQUIRE(Q > 0 && k > 0 && k <= K_MAX, DIRB200_ENOTSUP, "need 0 < Q and 0 < k <= %d (got Q=%d k=%d)", K_MAX, Q, k);
@@ -1312,6 +1449,11 @@ static int search_begin_seed(dirb200_index* h, const float* q32, int Q, int k, i
   P.launches0 = launches_total();
   P.cap2 = (k > 256) ? 2048 : 1024;
   P.sel_dev = sel_dev;
+  if (h->allow) {
+    P.allow = h->allow + allow_row0 * h->allow_ld;
+    P.allow_ld = h->allow_ld;
+    P.allow_bit0 = h->allow_bit0;
+  }
   if (N == 0) {   // empty shard: nothing can be selected; +inf never lowers the MIN over the shards
     fill_f32_kernel<<<static_cast<unsigned>(ceil_div(Q, 256)), 256, 0, stream>>>(sel_dev, Q, INFINITY);
     count_launch();
@@ -1331,6 +1473,14 @@ static int search_begin_seed(dirb200_index* h, const float* q32, int Q, int k, i
   P.cap = z.cap;
   P.cap2 = z.cap2;
   P.band = band;
+  const bool filtered = P.allow != nullptr;
+  if (filtered) {
+    const double seed_bytes = static_cast<double>(S) * h->dim * 2;
+    DIRB_REQUIRE(seed_bytes <= h->ws_budget, DIRB200_ENOTSUP,
+                 "a filtered search of depth k=%d gathers %lld seed rows (%.0f bytes), more than option ws_budget=%.0f bytes",
+                 k, static_cast<long long>(S), seed_bytes, h->ws_budget);
+    DIRB_TRY(grow_ws(h, &h->aws, &h->aws_bytes, allow_ws(nullptr, h, S).total));
+  }
   DIRB_TRY(grow_ws(h, &h->ws, &h->ws_bytes, search_ws(nullptr, h, z, Q).total));
   const SearchWs w = search_ws(h->ws, h, z, Q);
   P.cnt = w.cnt;
@@ -1351,8 +1501,26 @@ static int search_begin_seed(dirb200_index* h, const float* q32, int Q, int k, i
     count_launch();
   }
   if (h->profile) h->ev.mark(P.mark_i++, stream);  // 1: convert
-  // ---- 2. seed pass over the first S rows
-  {
+  // ---- 2f. filtered: seed pass over the first S rows allowed for every query of the block (rule F2)
+  if (filtered) {
+    const AllowWs aw = allow_ws(h->aws, h, S);
+    const int64_t W = ceil_div(N, 32);
+    allow_and_kernel<<<static_cast<unsigned>(ceil_div(W, 256)), 256, 0, stream>>>(P.allow, P.allow_ld, P.allow_bit0,
+                                                                                 P.allow_ld == 0 ? 1 : Q, N, aw.iw);
+    allow_seed_rows_kernel<<<1, ALLOW_SCAN_THREADS, 0, stream>>>(aw.iw, W, static_cast<int>(S), aw.rows, aw.n_seed);
+    allow_gather_kernel<<<static_cast<unsigned>(ceil_div(S, 8)), 256, 0, stream>>>(h->db16, D, aw.rows, aw.n_seed,
+                                                                                  static_cast<int>(S), aw.seed16);
+    count_launch(3);
+    SimArgs a;
+    a.dense = w.dense;
+    a.dense_ld = S_ld;
+    DIRB_TRY(sim_gemm(h, use_gmax ? PERS_EPI_SIM_GMAX : PERS_EPI_SIM_DENSE, w.q16, Q, aw.seed16, S, D, a, stream));
+    if (h->profile) h->ev.mark(P.mark_i++, stream);  // 2: seed gather + GEMM
+    allow_kth_kernel<<<Q, SEL_THREADS, 0, stream>>>(w.dense, S_ld, static_cast<int>(S), use_gmax ? 1 : 0, aw.n_seed, k, band,
+                                                    w.thr, seed2 ? k_shard : 0, seed2);
+    count_launch();
+    if (h->profile) h->ev.mark(P.mark_i++, stream);  // 3: k-th of the seed scores
+  } else {
     SimArgs a;
     a.dense = w.dense;
     a.dense_ld = S_ld;
@@ -1370,7 +1538,7 @@ static int search_begin_seed(dirb200_index* h, const float* q32, int Q, int k, i
   P.q16 = w.q16;
   P.gates = w.gates;
   P.S_ld = S_ld;
-  P.small = small;
+  P.small = small && !filtered;          // a filtered search always runs the filter as the GEMM pass (rule F3)
   P.ks = std::min<int>(k_shard, static_cast<int>(std::min<int64_t>(k, N)));
   DIRB_CUDA(cudaGetLastError());
   return 0;
@@ -1408,7 +1576,10 @@ static int search_begin_filter(dirb200_index* h, cudaStream_t stream) {
       a.cand_cnt = cnt;
       a.cand_cap = cap;
       a.gate = gate_in;
-      DIRB_TRY(sim_gemm(h, PERS_EPI_SIM_FILTER, q16, Q, h->db16, N, D, a, stream));
+      a.allow = P.allow;
+      a.allow_ld = P.allow_ld;
+      a.allow_bit0 = P.allow_bit0;
+      DIRB_TRY(sim_gemm(h, P.allow ? PERS_EPI_SIM_FILTER_ALLOW : PERS_EPI_SIM_FILTER, q16, Q, h->db16, N, D, a, stream));
     }
     if (r == 0 && h->profile) h->ev.mark(P.mark_i++, stream);  // 4: filter pass
     cand_kth_kernel<<<Q, SEL_THREADS, 0, stream>>>(cand, cnt, cap, k, ks, band, P.kth_k, sel_dev, thr, N, gate_in, gates + r,
@@ -1524,9 +1695,43 @@ int dirb200_index_search(dirb200_index* h, const float* q32, int Q, int k, doubl
     const int nb = std::min(qb, Q - q0);
     const float* qq = q32 + static_cast<int64_t>(q0) * h->dim;
     const int64_t o = static_cast<int64_t>(q0) * k;
-    DIRB_TRY(dirb200_index_search_begin(h, qq, nb, k, k, h->sel_own, stream_));
+    DIRB_TRY(search_begin_seed(h, qq, nb, k, k, h->sel_own, static_cast<cudaStream_t>(stream_), nullptr, q0));
+    DIRB_TRY(search_begin_filter(h, static_cast<cudaStream_t>(stream_)));
     DIRB_TRY(dirb200_index_search_finish(h, qq, h->sel_own, scores_dev + o, idx_dev + o, stream_));
   }
+  return 0;
+}
+
+int dirb200_index_set_allow(dirb200_index* h, const uint32_t* words_dev, int64_t ld_words, int64_t bit0) {
+  DIRB_REQUIRE(h, DIRB200_EINVAL, "null");
+  h->allow = nullptr;
+  h->allow_ld = h->allow_bit0 = 0;
+  if (words_dev == nullptr) return 0;
+  DIRB_REQUIRE(ld_words >= 0 && bit0 >= 0, DIRB200_EINVAL, "need ld_words >= 0 and bit0 >= 0");
+  DIRB_REQUIRE(ld_words == 0 || ld_words * 32 >= bit0 + h->N, DIRB200_EINVAL,
+               "a bitmap row of %lld words does not reach bit %lld (bit0 + N - 1)", static_cast<long long>(ld_words),
+               static_cast<long long>(bit0 + h->N - 1));
+  h->allow = words_dev;
+  h->allow_ld = ld_words;
+  h->allow_bit0 = bit0;
+  return 0;
+}
+
+int dirb200_allow_exclude(uint32_t* words_dev, int Q, int64_t ld_words, const int64_t* off_dev, const int64_t* rows_dev,
+                          void* stream_) {
+  DIRB_REQUIRE(Q >= 0 && ld_words >= 1, DIRB200_EINVAL, "need Q >= 0 and ld_words >= 1");
+  if (Q == 0) return 0;
+  DIRB_REQUIRE(words_dev && off_dev && rows_dev, DIRB200_EINVAL, "null argument");
+  allow_exclude_kernel<<<Q, 256, 0, static_cast<cudaStream_t>(stream_)>>>(words_dev, ld_words, off_dev, rows_dev);
+  count_launch();
+  DIRB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Entry points that rank, count or select rows without the filter refuse to run while one is attached.
+static int no_filter(const dirb200_index* h) {
+  DIRB_REQUIRE(h->allow == nullptr, DIRB200_ESTATE,
+               "a filter is attached (dirb200_index_set_allow): only the top-k search applies it; detach it first");
   return 0;
 }
 
@@ -1536,6 +1741,7 @@ int dirb200_index_target_scores(dirb200_index* h, const float* q32, int Q, const
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DIRB_REQUIRE(h && q32 && Q > 0 && T >= 0, DIRB200_EINVAL, "bad arguments");
   DIRB_REQUIRE(h->has_db, DIRB200_ESTATE, "index has no database attached");
+  DIRB_TRY(no_filter(h));
   if (T == 0) return 0;
   DIRB_REQUIRE(t_q_dev && t_rows_dev && t_score_dev, DIRB200_EINVAL, "null argument");
   DIRB_CUDA(cudaSetDevice(h->device));
@@ -1552,6 +1758,7 @@ int dirb200_index_rank_count(dirb200_index* h, const float* q32, int Q, const in
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DIRB_REQUIRE(h && q32 && Q > 0 && T >= 0 && t_off_host, DIRB200_EINVAL, "bad arguments");
   DIRB_REQUIRE(h->has_db, DIRB200_ESTATE, "index has no database attached");
+  DIRB_TRY(no_filter(h));
   if (T == 0) return 0;
   DIRB_REQUIRE(t_off_dev && t_rows_dev && t_flags_dev && t_score_dev && above_dev, DIRB200_EINVAL, "null argument");
   DIRB_REQUIRE(t_off_host[0] == 0 && t_off_host[Q] == T, DIRB200_EINVAL, "target offsets must run from 0 to T");
@@ -1652,6 +1859,7 @@ int dirb200_index_count_ge(dirb200_index* h, const float* q32, int Q, const int*
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DIRB_REQUIRE(h && Q >= 0 && T >= 0, DIRB200_EINVAL, "bad arguments");
   DIRB_REQUIRE(h->has_db, DIRB200_ESTATE, "index has no database attached");
+  DIRB_TRY(no_filter(h));
   DIRB_REQUIRE(Q <= 65535 * 64, DIRB200_ENOTSUP, "count_ge takes at most %d queries per call (got %d)", 65535 * 64, Q);
   h->stats[0] = h->stats[1] = h->stats[2] = h->stats[3] = h->stats[4] = 0;
   if (Q == 0 || T == 0) return 0;
@@ -1903,6 +2111,7 @@ int join_rows(const JoinRun& R, int64_t r0, int M, int64_t col0, int cap) {
 
 int join_begin(dirb200_index* h, double tau) {
   DIRB_REQUIRE(h->has_db, DIRB200_ESTATE, "index has no database attached");
+  DIRB_TRY(no_filter(h));
   DIRB_REQUIRE(std::isfinite(tau), DIRB200_EINVAL, "tau must be finite");
   DIRB_CUDA(cudaSetDevice(h->device));
   DIRB_TRY(dirb200_index_check(h));
@@ -1992,6 +2201,7 @@ int dirb200_index_join_stats(dirb200_index* h, int64_t stats[5], double ms[3]) {
 int dirb200_index_nearest(dirb200_index* h, const float* q32_dev, int Q, int64_t* labels_dev, double* scores_dev,
                           void* stream_) {
   DIRB_REQUIRE(h && h->has_db, DIRB200_EINVAL, "index has no database");
+  DIRB_TRY(no_filter(h));
   DIRB_REQUIRE(Q >= 0 && (Q == 0 || (q32_dev && labels_dev && scores_dev)), DIRB200_EINVAL, "bad arguments");
   DIRB_REQUIRE(h->N >= 1, DIRB200_EINVAL, "the index is empty");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -2703,6 +2913,7 @@ int dirb200_index_set_lists(dirb200_index* h, const void* db16_lists_dev, const 
 int dirb200_index_search_lists(dirb200_index* h, const float* q32_dev, int Q, int k, const int64_t* probes_dev, int nprobe,
                                double* scores_dev, int64_t* idx_dev, void* stream_) {
   DIRB_REQUIRE(h && h->lists_k > 0, DIRB200_ESTATE, "index has no lists attached (dirb200_index_set_lists)");
+  DIRB_TRY(no_filter(h));
   DIRB_REQUIRE(Q >= 0 && (Q == 0 || (q32_dev && probes_dev && scores_dev && idx_dev)), DIRB200_EINVAL, "bad arguments");
   DIRB_REQUIRE(k >= 1 && k <= K_MAX, DIRB200_ENOTSUP, "need 0 < k <= %d (got %d)", K_MAX, k);
   DIRB_REQUIRE(nprobe >= 1 && nprobe <= h->lists_k, DIRB200_EINVAL, "nprobe must be in [1, %d] (got %d)", h->lists_k, nprobe);

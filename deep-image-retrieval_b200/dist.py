@@ -70,6 +70,7 @@ class ShardedIndex:
             self.shard_sizes = [int(v) for v in sizes.tolist()]
         else:
             self.shard_sizes = [int(self.local.n)]
+        self.local.n_global = sum(self.shard_sizes)   # allow sets number the rows of the whole database
 
     def enable_peer_exchange(self, max_q: int = 1024, max_k: int = 128):
         """Switch search() to the peer-memory protocol (dirb200_index_search_sharded): the MIN of the selection thresholds
@@ -121,7 +122,7 @@ class ShardedIndex:
         self.local.search(q32, k, out=packed)
         return packed
 
-    def search(self, q32: torch.Tensor, k: int, check: bool = True):
+    def search(self, q32: torch.Tensor, k: int, check: bool = True, allow=None):
         """Global exact top-k.  Phase 1 on every shard (tensor-core passes) -> MIN all-reduce of the per-query
         selection thresholds (4*Q bytes: the local c-th best scores, c = shard_quota(k, shard sizes) = ceil(k/G) for
         evenly filled shards, bound the global k-th best, so each shard re-scores only ~k/G rows) -> phase 2 (exact
@@ -129,16 +130,22 @@ class ShardedIndex:
 
         Nothing on this path waits for the GPU except the status check of the local shard (candidate overflow that the
         device-side retry passes could not resolve).  check=True collects it before returning; check=False leaves it
-        to the next search() / an explicit check() so that the host can enqueue the next search while this one runs."""
+        to the next search() / an explicit check() so that the host can enqueue the next search while this one runs.
+
+        allow: filtered search (DESIGN.md section 4.13, rule F6) - the same allow set on every rank, in global row
+        numbering: (W,) int32 words shared by every query or (Q, W) one per query, W = ceil(total rows / 32)."""
         world = dist.get_world_size(self.group) if dist.is_initialized() else 1
+        filt = {} if allow is None else {"allow": allow}
         if world == 1:
             self.local.set_option("deferred_check", 0 if check else 1)
-            return self.local.search(q32, k)                 # the shard's ordered list IS the result: no merge pass
+            return self.local.search(q32, k, **filt)         # the shard's ordered list IS the result: no merge pass
+        if allow is not None:
+            self.local._allow_ld(allow, q32.shape[0])        # bad arguments raise before any device call
         self.local.set_option("deferred_check", 1)
         k_shard = shard_quota(k, self.shard_sizes)
         x = self.xchg
         if x is not None and q32.shape[0] <= x.max_q and k <= x.max_k:
-            out = self.local.search_sharded(x, q32, k, k_shard)   # thresholds + lists travel through peer memory
+            out = self.local.search_sharded(x, q32, k, k_shard, **filt)   # thresholds + lists travel through peer memory
             if check:
                 self.local.check()
             return out
@@ -146,7 +153,9 @@ class ShardedIndex:
         parts = []
         for q0 in range(0, q32.shape[0], qb):               # query blocks whose workspace fits every shard's budget
             qc = q32[q0:q0 + qb].contiguous()
-            sel = self.local.search_begin(qc, k, k_shard)
+            if allow is not None:
+                filt["allow"] = allow if allow.dim() == 1 else allow[q0:q0 + qb]
+            sel = self.local.search_begin(qc, k, k_shard, **filt)
             dist.all_reduce(sel, op=dist.ReduceOp.MIN, group=self.group)
             packed = torch.empty((2, qc.shape[0], k), dtype=torch.int64, device=q32.device)
             self.local.search_finish(qc, k, sel, out=packed)

@@ -85,6 +85,9 @@ SIGNATURES = {
     "dirb200_index_search_begin": (i32, [p, p, i32, i32, i32, p, p]),
     "dirb200_index_search_finish": (i32, [p, p, p, p, p, p]),
     "dirb200_index_check": (i32, [p]),
+    # filtered exact search: an allow bitmap on the index, and per-query row exclusion into such a bitmap
+    "dirb200_index_set_allow": (i32, [p, p, i64, i64]),
+    "dirb200_allow_exclude": (i32, [p, i32, i64, p, p, p]),
     "dirb200_index_last_stats": (i32, [p, C.POINTER(i64)]),
     "dirb200_index_last_profile": (i32, [p, C.POINTER(f64)]),
     "dirb200_index_target_scores": (i32, [p, p, i32, p, p, i32, p, p]),

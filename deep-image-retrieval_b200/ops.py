@@ -492,6 +492,47 @@ def aqe_expand(q, db32, nn_idx, nn_scores, alpha, partial=False, row_offset=0, n
     return out
 
 
+def allow_rows(mask: torch.Tensor) -> torch.Tensor:
+    """Allow set of a filtered search (DESIGN.md section 4.13, rule F1) from a bool mask (..., N): row r is bit r & 31 of
+    int32 word r >> 5 -> (..., ceil(N / 32)) int32 words, on the mask's device."""
+    if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool or mask.dim() < 1:
+        raise ValueError("mask must be a bool tensor (..., N)")
+    n = mask.shape[-1]
+    w = (n + 31) // 32
+    bits = torch.zeros(mask.shape[:-1] + (32 * w,), dtype=torch.int64, device=mask.device)
+    bits[..., :n] = mask.to(torch.int64)
+    weights = torch.ones(32, dtype=torch.int64, device=mask.device) << torch.arange(32, device=mask.device)
+    words = (bits.view(mask.shape[:-1] + (w, 32)) * weights).sum(dim=-1)
+    return torch.where(words >= 1 << 31, words - (1 << 32), words).to(torch.int32).contiguous()
+
+
+def allow_exclude(base: torch.Tensor, n_queries: int, rows_per_query) -> torch.Tensor:
+    """Per-query allow sets (Q, W) = the shared set base (W,) int32 CUDA words with each query's rows cleared
+    (dirb200_allow_exclude): leave-one-out when the queries are database rows, per-query junk lists.  rows_per_query:
+    Q sequences of global row numbers in [0, 32 W)."""
+    _chk(base, torch.int32, "base")
+    if base.dim() != 1:
+        raise ValueError("base must be one shared allow set (W,)")
+    nq = int(n_queries)
+    lists = [np.asarray(r, dtype=np.int64).reshape(-1) for r in rows_per_query]
+    if len(lists) != nq:
+        raise ValueError("rows_per_query must hold %d lists (got %d)" % (nq, len(lists)))
+    w = base.shape[0]
+    rows = np.concatenate(lists) if lists else np.zeros(0, np.int64)
+    if rows.size and (rows.min() < 0 or rows.max() >= 32 * w):
+        raise ValueError("excluded rows must lie in [0, %d)" % (32 * w))
+    off = np.zeros(nq + 1, np.int64)
+    off[1:] = np.cumsum([len(r) for r in lists])
+    out = base.unsqueeze(0).expand(nq, w).contiguous()
+    if nq == 0 or rows.size == 0:
+        return out
+    off_d = torch.from_numpy(off).to(base.device)
+    rows_d = torch.from_numpy(rows).to(base.device)
+    with torch.cuda.device(base.device):
+        lib.call("dirb200_allow_exclude", _ptr(out), nq, w, _ptr(off_d), _ptr(rows_d), _stream())
+    return out
+
+
 class Exchange:
     """This rank's window of the peer-memory exchange of a sharded search (include/dirb200.h: dirb200_exchange_*)."""
 
@@ -555,6 +596,9 @@ class Index:
             db16 = f32_to_f16(db32) if self.n else torch.empty((0, self.dim), dtype=torch.float16, device=db32.device)
         self.db16 = db16
         self.offset = int(index_offset)
+        # rows numbered by the allow sets of a filtered search: a shard searched together with others (dist.ShardedIndex,
+        # or the phases driven by hand) sets it to the rows of the whole database
+        self.n_global = self.offset + self.n
         self._h = C.c_void_p()
         lib.call("dirb200_index_create", db32.device.index or 0, self.dim, C.byref(self._h))
         lib.call("dirb200_index_set_db", self._h, _ptr(self.db32), _ptr(self.db16), self.n, self.offset)
@@ -562,10 +606,47 @@ class Index:
     def set_option(self, key, value):
         lib.call("dirb200_index_set_option", self._h, key.encode(), float(value))
 
-    def search(self, q32: torch.Tensor, k: int, out=None):
+    def _allow_ld(self, allow, nq):
+        """Checks an allow set (rule F1) against this index and nq queries -> words per query row (0 = shared)."""
+        if allow is None:
+            return None
+        w = (self.n_global + 31) // 32
+        if not isinstance(allow, torch.Tensor) or allow.dtype != torch.int32:
+            raise ValueError("allow must be an int32 tensor of bitmap words (ops.allow_rows)")
+        if not allow.is_cuda or allow.device != self.db32.device:
+            raise ValueError("allow must live on the index's device %s" % self.db32.device)
+        if not allow.is_contiguous():
+            raise ValueError("allow must be contiguous")
+        if allow.dim() == 1 and allow.shape[0] == w:
+            return 0
+        if allow.dim() == 2 and allow.shape[1] == w:
+            if allow.shape[0] != nq:
+                raise ValueError("a per-query allow set needs one row per query (%d), got %d" % (nq, allow.shape[0]))
+            return w
+        raise ValueError("allow must be (%d,) or (Q, %d) words for %d rows, got %s" % (w, w, self.n_global, tuple(allow.shape)))
+
+    def _set_allow(self, allow, ld):
+        lib.call("dirb200_index_set_allow", self._h, _ptr(allow), 0 if ld is None else ld, self.offset)
+
+    def search(self, q32: torch.Tensor, k: int, out=None, allow=None):
         """-> (scores fp64 (Q,k), idx int64 (Q,k)), exact order: score desc, index asc.
-        out: optional (2,Q,k) int64 buffer that receives [score bits, indices] (the all-gather payload)."""
+        out: optional (2,Q,k) int64 buffer that receives [score bits, indices] (the all-gather payload).
+        allow: filtered search (DESIGN.md section 4.13): int32 CUDA words of one allow set (W,) shared by every query or
+        one per query (Q, W), W = ceil(rows / 32) in global row numbering (ops.allow_rows, ops.allow_exclude); each
+        query gets the exact top-k of its allowed rows, tail (-inf, -1).  Per-query sets take Q * W * 4 bytes (125 MB
+        for 1000 queries over 2^20 rows): pass very large Q in blocks."""
         _chk(q32, torch.float32, "q32")
+        nq = q32.shape[0]
+        ld = self._allow_ld(allow, nq)
+        if ld is None:
+            return self._search(q32, k, out)
+        self._set_allow(allow, ld)
+        try:
+            return self._search(q32, k, out)
+        finally:
+            self._set_allow(None, None)
+
+    def _search(self, q32, k, out):
         nq = q32.shape[0]
         if out is not None:
             _chk(out, torch.int64, "out")
@@ -597,11 +678,19 @@ class Index:
         lib.call("dirb200_index_search_max_queries", self._h, int(k), C.byref(out))
         return int(out.value)
 
-    def search_begin(self, q32: torch.Tensor, k: int, k_shard: int):
-        """Phase 1 of a sharded search -> sel (Q,) fp32: local k_shard-th best fp16-path score (MIN-reduce it)."""
+    def search_begin(self, q32: torch.Tensor, k: int, k_shard: int, allow=None):
+        """Phase 1 of a sharded search -> sel (Q,) fp32: local k_shard-th best fp16-path score (MIN-reduce it).
+        allow: the filter of search(), applied by this search through its search_finish."""
         _chk(q32, torch.float32, "q32")
+        ld = self._allow_ld(allow, q32.shape[0])
         sel = torch.empty(q32.shape[0], dtype=torch.float32, device=q32.device)
-        lib.call("dirb200_index_search_begin", self._h, _ptr(q32), q32.shape[0], int(k), int(k_shard), _ptr(sel), _stream())
+        if ld is not None:
+            self._set_allow(allow, ld)
+        try:
+            lib.call("dirb200_index_search_begin", self._h, _ptr(q32), q32.shape[0], int(k), int(k_shard), _ptr(sel), _stream())
+        finally:
+            if ld is not None:
+                self._set_allow(None, None)
         return sel
 
     def search_finish(self, q32: torch.Tensor, k: int, sel: torch.Tensor, out=None):
@@ -616,13 +705,25 @@ class Index:
                  _ptr(idx), _stream())
         return scores, idx
 
-    def search_sharded(self, exchange: "Exchange", q32: torch.Tensor, k: int, k_shard: int, phase: int = 0):
+    def search_sharded(self, exchange: "Exchange", q32: torch.Tensor, k: int, k_shard: int, phase: int = 0, allow=None):
         """Collective exact top-k over all shards through the peer-memory exchange (no library collective): every rank
         calls it with the same (Q, k, k_shard).  phase 0 = the whole search; 1 .. 4 = one phase (seed bounds, filter +
         selection, re-scoring, merge: several shards driven shard by shard from one process).
         -> (scores fp64, idx int64) (Q,k) after phase 0 / 4, else None.
+        allow: the filter of search() in global row numbering, the same on every rank; read by phase 0 / 1 (the later
+        phases use what their search began with).
         Never synchronises: call check() (or the next search) to collect the status."""
         _chk(q32, torch.float32, "q32")
+        ld = self._allow_ld(allow, q32.shape[0]) if phase in (0, 1) else None
+        if ld is None:
+            return self._search_sharded(exchange, q32, k, k_shard, phase)
+        self._set_allow(allow, ld)
+        try:
+            return self._search_sharded(exchange, q32, k, k_shard, phase)
+        finally:
+            self._set_allow(None, None)
+
+    def _search_sharded(self, exchange, q32, k, k_shard, phase):
         nq = q32.shape[0]
         scores = idx = None
         if phase in (0, 4):

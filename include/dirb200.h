@@ -282,6 +282,25 @@ int dirb200_index_search_begin(dirb200_index* idx, const float* q32_dev, int Q, 
                                void* stream);
 int dirb200_index_search_finish(dirb200_index* idx, const float* q32_dev, const float* sel_dev, double* scores_dev,
                                 int64_t* idx_dev, void* stream);
+/* Filtered search (DESIGN.md section 4.13, rules F1-F6).  Replaces building a new index over the allowed rows,
+ * Index(X[subset]) (and the k + 1 over-fetch + host-side drop that pipeline._drop_self does for one excluded row): the
+ * exact top-k of each query over the rows its allow set admits.  words_dev: caller-owned device bitmap of uint32 words
+ * in global row numbering (row r = bit r & 31 of word r >> 5), one row of ld_words words per query, or ld_words = 0
+ * for one row shared by every query; bit0 = the global number of this shard's row 0 (its index_offset).  Null detaches
+ * it.  While it is attached, dirb200_index_search, _search_begin and _search_sharded(_phase) phase 1 apply it (later
+ * phases use what their search began with; _search_finish does not read it), and every other entry point that ranks,
+ * counts or selects rows (target_scores, rank_count, count_ge, range_search, self_join, nearest, search_lists) returns
+ * DIRB200_ESTATE.  The result of each query is the exact top-k of its allowed rows, tail (-inf, -1); with every bit
+ * set it equals the unfiltered search bit for bit.  The seed rows of a query block (the first S rows allowed for all of
+ * its queries) are gathered into a buffer of S * dim * 2 bytes; a search whose buffer exceeds option "ws_budget" is
+ * refused with DIRB200_ENOTSUP.  dirb200_index_set_db detaches the filter. */
+int dirb200_index_set_allow(dirb200_index* idx, const uint32_t* words_dev, int64_t ld_words, int64_t bit0);
+/* Builds per-query allow sets from lists of rows to leave out (replaces the over-fetch by one + host-side drop of
+ * pipeline._drop_self, and per-query junk lists): clears bit rows_dev[i] of bitmap row q (ld_words words apart) for
+ * every i in [off_dev[q], off_dev[q + 1]), q < Q.  Rows outside [0, 32 ld_words) are skipped.  Order-independent
+ * (atomicAnd).  off_dev int64 [Q + 1], rows_dev int64, both on the device of words_dev; enqueued on `stream`. */
+int dirb200_allow_exclude(uint32_t* words_dev, int Q, int64_t ld_words, const int64_t* off_dev, const int64_t* rows_dev,
+                          void* stream);
 /* Status of the last search, for option "deferred_check": waits for it to finish; DIRB200_EOVERFLOW if a candidate
  * list still overflowed after the retry passes or more than cap2 rows sat within the band of the k-th score. */
 int dirb200_index_check(dirb200_index* idx);
