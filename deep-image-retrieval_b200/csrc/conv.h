@@ -1,5 +1,7 @@
 // Internal C++ interface of the convolution kernels (conv.cu) and the small fused operators (ops.cu).
 #pragma once
+#include <mutex>
+
 #include "common.h"
 
 namespace dirb {
@@ -101,9 +103,22 @@ int f32_to_f16(const float* x, int64_t n, __half* out, cudaStream_t stream);
 int whiten(const float* x, int64_t N, int D, const float* comp, const float* mean, const float* colscale, int Dout,
            int l2norm, float* y, __half* y16, cudaStream_t stream);
 
-// Per-device scratch buffer kept for the life of the process (ops.cu): acquire grows it to `bytes` and orders `stream`
-// after the previous user; release marks the end of this stream's use.
-int scratch_acquire(size_t bytes, cudaStream_t stream, void** out);
-int scratch_release(cudaStream_t stream);
+// Lease on the per-device scratch buffer kept for the life of the process (ops.cu).  acquire takes the device's
+// scratch mutex, grows the buffer to `bytes` and orders `stream` after the previous lease's work; the mutex is held
+// until the lease goes out of scope, whose destructor records the end of this stream's use on every return path
+// (including errors after kernels were enqueued).  Enqueue all work on the buffer while the lease is alive.
+class ScratchLease {
+ public:
+  ScratchLease() = default;
+  ScratchLease(const ScratchLease&) = delete;
+  ScratchLease& operator=(const ScratchLease&) = delete;
+  ~ScratchLease();
+  int acquire(size_t bytes, cudaStream_t stream, void** out);
+
+ private:
+  std::unique_lock<std::mutex> lock_;
+  cudaEvent_t last_use_ = nullptr;
+  cudaStream_t stream_ = nullptr;
+};
 
 }  // namespace dirb

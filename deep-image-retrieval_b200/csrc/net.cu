@@ -459,6 +459,9 @@ int dirb200_net_finalize(dirb200_net* n) {
   }
   DIRB_TRY(dev_alloc(n, reinterpret_cast<void**>(&n->head_bar), 128));
   DIRB_CUDA(cudaMemset(n->head_bar, 0, 128));
+  // The memset and the pageable copies above run on the legacy stream and may still be in flight when they return;
+  // a forward on a non-blocking stream is not ordered after them.  Finish them before the network is usable.
+  DIRB_CUDA(cudaStreamSynchronize(cudaStreamLegacy));
   n->sd.clear();
   n->finalized = true;
   return 0;

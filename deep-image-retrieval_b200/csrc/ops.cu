@@ -677,23 +677,26 @@ __global__ void __launch_bounds__(256) whiten_gemm_kernel(const float* __restric
 // dirb200_whiten has no handle, and allocating ~1 GB of split buffers per call (cudaMallocAsync after every
 // synchronisation point, i.e. a driver-level allocation) serialises badly when 8 processes share a box.  One scratch
 // buffer per device is therefore kept for the life of the process (grown on demand).  Users on different streams are
-// ordered through an event: acquire makes the caller's stream wait for the previous user, release records it.
+// ordered through an event: acquire makes the caller's stream wait for the previous user, and the lease records the
+// event once its work is enqueued.  The device's mutex is held for the whole lease, so a second caller cannot acquire
+// between the first one's acquire and its record (it would wait on an older event and share the buffer).
 namespace {
 struct DevScratch {
   void* ptr = nullptr;
   size_t bytes = 0;
   cudaEvent_t last_use = nullptr;
+  std::mutex mu;
 };
 DevScratch g_scratch[64];
-std::mutex g_scratch_mu;
 }  // namespace
 
-int scratch_acquire(size_t bytes, cudaStream_t stream, void** out) {
+int ScratchLease::acquire(size_t bytes, cudaStream_t stream, void** out) {
   int dev = 0;
   DIRB_CUDA(cudaGetDevice(&dev));
   DIRB_REQUIRE(dev >= 0 && dev < 64, DIRB200_ENOTSUP, "device index %d out of range", dev);
-  std::lock_guard<std::mutex> lock(g_scratch_mu);
+  DIRB_REQUIRE(!lock_.owns_lock(), DIRB200_ESTATE, "scratch lease acquired twice");
   DevScratch& s = g_scratch[dev];
+  lock_ = std::unique_lock<std::mutex>(s.mu);
   if (!s.last_use) DIRB_CUDA(cudaEventCreateWithFlags(&s.last_use, cudaEventDisableTiming));
   if (bytes > s.bytes) {
     // cudaFree synchronises the device: no earlier user is still running
@@ -701,16 +704,16 @@ int scratch_acquire(size_t bytes, cudaStream_t stream, void** out) {
   } else {
     DIRB_CUDA(cudaStreamWaitEvent(stream, s.last_use, 0));
   }
+  last_use_ = s.last_use;
+  stream_ = stream;
   *out = s.ptr;
   return 0;
 }
 
-int scratch_release(cudaStream_t stream) {
-  int dev = 0;
-  DIRB_CUDA(cudaGetDevice(&dev));
-  std::lock_guard<std::mutex> lock(g_scratch_mu);
-  DIRB_CUDA(cudaEventRecord(g_scratch[dev].last_use, stream));
-  return 0;
+ScratchLease::~ScratchLease() {
+  // the next lease's stream waits for everything this one enqueued (a destructor has no status to return: the record
+  // fails only when the context is already broken, which the caller's next CUDA call reports)
+  if (lock_.owns_lock() && last_use_) cudaEventRecord(last_use_, stream_);
 }
 
 // ---- fp16 hi/lo split with an adaptive power-of-two prescale --------------------------------------------------------
@@ -800,7 +803,8 @@ static int whiten_tc(const float* x, int64_t N, int D, const float* comp, const 
     return c.used;
   };
   void* base = nullptr;
-  DIRB_TRY(scratch_acquire(layout(nullptr), stream, &base));
+  ScratchLease lease;
+  DIRB_TRY(lease.acquire(layout(nullptr), stream, &base));
   layout(base);
   DIRB_CUDA(cudaMemsetAsync(ws, 0, 32, stream));
   const unsigned gx = static_cast<unsigned>(std::min<int64_t>(ceil_div(ceil_div(xe, 4), 256), num_sms() * 16));
@@ -836,8 +840,7 @@ static int whiten_tc(const float* x, int64_t N, int D, const float* comp, const 
   p.dense = y;
   p.dense_ld = Dout;
   p.scale = cs;
-  DIRB_TRY((conv_pers_launch<BN, 6, PERS_EPI_F32>(tmAh, tmBh, tmAl, tmBl, p, num_sms(), stream)));
-  return scratch_release(stream);
+  return conv_pers_launch<BN, 6, PERS_EPI_F32>(tmAh, tmBh, tmAl, tmBl, p, num_sms(), stream);
 }
 
 int whiten(const float* x, int64_t N, int D, const float* comp, const float* mean, const float* colscale, int Dout,

@@ -230,13 +230,14 @@ int dirb200_col_sums_f64(const float* x_dev, int64_t N, int D, double* sum_dev, 
   const int64_t rows = std::max(CS_ROWS, ceil_div(N, CS_MAX_PARTS));
   const int P = static_cast<int>(ceil_div(N, rows));
   void* ws = nullptr;
-  DIRB_TRY(scratch_acquire(static_cast<size_t>(P) * D * 8, stream, &ws));
+  ScratchLease lease;
+  DIRB_TRY(lease.acquire(static_cast<size_t>(P) * D * 8, stream, &ws));
   double* part = static_cast<double*>(ws);
   col_sum_part_kernel<<<dim3(static_cast<unsigned>(ceil_div(D, 32)), P), dim3(32, 8), 0, stream>>>(x_dev, N, D, rows, part);
   col_sum_reduce_kernel<<<static_cast<unsigned>(ceil_div(D, 256)), 256, 0, stream>>>(part, P, D, sum_dev);
   count_launch(2);
   DIRB_CUDA(cudaGetLastError());
-  return scratch_release(stream);
+  return 0;
 }
 
 int dirb200_gram_f64(const float* x_dev, int64_t N, int D, const double* mean_dev, double* gram_dev, void* stream_) {
@@ -257,7 +258,8 @@ int dirb200_gram_f64(const float* x_dev, int64_t N, int D, const double* mean_de
   const int64_t rows = ceil_div(ceil_div(N, s_want), GK) * GK;
   const int S = static_cast<int>(ceil_div(N, rows));
   void* ws = nullptr;
-  DIRB_TRY(scratch_acquire(static_cast<size_t>(S) * tiles * GRAM_TILE_BYTES, stream, &ws));
+  ScratchLease lease;
+  DIRB_TRY(lease.acquire(static_cast<size_t>(S) * tiles * GRAM_TILE_BYTES, stream, &ws));
   double* part = static_cast<double*>(ws);
   static std::atomic<uint64_t> attr_done{0};
   if (first_launch_on_device(attr_done))
@@ -266,7 +268,7 @@ int dirb200_gram_f64(const float* x_dev, int64_t N, int D, const double* mean_de
   gram_reduce_kernel<<<dim3(tiles, GT * GT / 1024), 256, 0, stream>>>(part, S, T, D, gram_dev);
   count_launch(2);
   DIRB_CUDA(cudaGetLastError());
-  return scratch_release(stream);
+  return 0;
 }
 
 }  // extern "C"

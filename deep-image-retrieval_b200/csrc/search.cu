@@ -2326,6 +2326,9 @@ int dirb200_exchange_create(int device, int world, int rank, int max_q, int max_
     const uint32_t one = 1;          // epochs start at 1: the zero-initialised flags read as "not yet published"
     e = cudaMemcpy(x->base + X_OFF_EPOCH, &one, 4, cudaMemcpyHostToDevice);
   }
+  // the memsets and the pageable copy run on the legacy stream, which a search on a non-blocking stream does not wait
+  // for: finish them before the window is handed out
+  if (e == cudaSuccess) e = cudaStreamSynchronize(cudaStreamLegacy);
   if (e != cudaSuccess) {
     set_error("exchange window of %zu bytes: %s", x->bytes, cudaGetErrorString(e));
     dirb200_exchange_destroy(x);

@@ -11,6 +11,8 @@
  *   - "dev" pointers are device memory owned by the caller; the library allocates only inside
  *     opaque handles (packed weights, workspaces) freed by the matching *_destroy;
  *   - all launches are asynchronous on the given stream unless the name ends in _host;
+ *   - create, finalize and set calls (no stream argument) have finished on the device when they
+ *     return: their results may be used at once from any stream, blocking or not;
  *   - a handle is bound to one device and is not re-entrant (one handle per GPU / stream);
  *   - there is NO CPU fallback: on a machine without an sm_90 device every compute entry
  *     point fails with DIRB200_ENODEVICE.
