@@ -1,4 +1,5 @@
-"""Build libdirb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a."""
+"""Build libdirb200.so (the C-ABI CUDA library) and libdirb200_blocktest.so (test-only wrappers of csrc/block.cuh)
+in-tree with nvcc for sm_90a."""
 import os
 import subprocess
 import sys
@@ -8,6 +9,8 @@ CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["common.cu", "conv.cu", "ops.cu", "search.cu", "net.cu", "api.cu", "resize.cu", "label_count.cu", "jpeg.cu", "pca.cu",
            "aploss.cu", "diffusion.cu", "diffusion_trunc.cu", "join.cu", "kmeans.cu", "pq.cu", "graph.cu"]
 LIB = os.path.join(HERE, "libdirb200.so")
+BLOCKTEST_SRC = os.path.join(os.path.dirname(HERE), "tests", "block_harness.cu")
+BLOCKTEST_LIB = os.path.join(HERE, "libdirb200_blocktest.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
@@ -44,6 +47,17 @@ def build(force=False, verbose=False):
     if procs or not os.path.exists(LIB):
         cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
         subprocess.check_call(cmd)
+    # the test-only wrappers of block.cuh's primitives (tests/test_gpu_block.py), a library of their own
+    if force or _newer(BLOCKTEST_SRC, BLOCKTEST_LIB) or any(_newer(h, BLOCKTEST_LIB) for h in headers):
+        cmd = [nvcc] + NVCC_FLAGS + ["-shared", BLOCKTEST_SRC, "-o", BLOCKTEST_LIB, "-cudart", "static"]
+        p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+        if p.returncode != 0 or verbose:
+            print("==== nvcc block_harness.cu ->", p.returncode)
+            print(p.stdout)
+        with open(os.path.join(objdir, "block_harness.cu.log"), "w") as f:
+            f.write(p.stdout)
+        if p.returncode != 0:
+            raise RuntimeError("nvcc failed")
     return LIB
 
 
